@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Benchmark of the NHD placement hot path (contract: see the task's bench.py section).
+"""Benchmark of the NHD placement hot path.
 
-    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference]
+    python bench.py [--gpus N] [--steps K] [--warmup W] [--impl reference] [--dump-outputs DIR]
     torchrun --nproc-per-node N bench.py --gpus N ...        (N > 1, one rank per GPU)
 
 A *step* is one pass of the hot path over one batch: 4 096 pending pods scheduled, with the
@@ -11,7 +11,8 @@ reference's sequential semantics, on the 65 536-node synthetic cluster of BASELI
 Own arm (CUDA):
   value   decisions/s with the batch and the cluster resident in HBM; the timed region is the
           solver's kernels (snapshot filter [+ NCCL all-reduce] + sweep), timed with CUDA events
-          on the stream they are launched on; L2 is flushed between steps.
+          on the stream they are launched on; L2 is flushed between steps.  --dump-outputs DIR writes
+          the bindings of the last timed step to DIR/<field>.npy (float64, one array per field).
   e2e     the same metric through the C-ABI with HOST buffers: per step, upload of the cluster
           records and of the pod batch from host memory, the kernels, and the download of the
           bindings (wall clock around nhd_load_nodes + nhd_solve_batch).
@@ -47,7 +48,7 @@ def measured_peaks():
         with open(os.path.join(ROOT, 'MEASURED_PEAKS.json')) as f:
             return float(json.load(f)['hbm_gbs']), 'measured (MEASURED_PEAKS.json)'
     except Exception:
-        return 6650.0, 'fallback (B200_PROFILING.md)'
+        return 3350.0, 'H100 SXM data sheet (HBM3), not measured'
 
 
 class ClockSampler:
@@ -261,16 +262,25 @@ def quick_value(Solver, recs, speed, pods, now, steps=3, pre_step=None, **kw):
 
 def python_reference_baseline(recs, speed, pods, now, n_pods=8):
     """The reference's own Python path (unmodified nhd/Matcher.py + Node.py through oracle/ref_loader) on the first
-    pods of the stream at full N, one thread — only where the reference is reachable (NHD_REFERENCE_ROOT or
-    /root/reference; never on the GPU box).  Returns None otherwise."""
-    root = os.environ.get('NHD_REFERENCE_ROOT', '/root/reference')
-    if not os.path.isfile(os.path.join(root, 'nhd', 'Matcher.py')):
+    pods of the stream at full N, one thread — only where NHD_REFERENCE_ROOT names a checkout of the reference.
+    Returns None otherwise."""
+    root = os.environ.get('NHD_REFERENCE_ROOT', '')
+    if not root or not os.path.isfile(os.path.join(root, 'nhd', 'Matcher.py')):
         return None
     try:
         from tests import pyref
         return pyref.time_reference(recs, speed, pods[:n_pods], now[:n_pods])
     except Exception as e:                      # never let the optional leg take the bench down
         return {'error': str(e)[:200]}
+
+
+def dump_outputs(path, bindings):
+    """The bindings a caller of the timed path receives, one array per field as <path>/<field>.npy.  Every field is
+    an integer of at most 32 bits, so float64 holds it exactly (4 096 pods: about 4 MB in all)."""
+    os.makedirs(path, exist_ok=True)
+    for name in bindings.dtype.names:
+        if name != 'pad_':
+            np.save(os.path.join(path, name + '.npy'), np.ascontiguousarray(bindings[name], dtype=np.float64))
 
 
 def run_reference_arm(args, rank):
@@ -316,6 +326,7 @@ def main():
     ap.add_argument('--cpu-sample-pods', type=int, default=128)
     ap.add_argument('--no-extra', action='store_true', help='skip the side workloads (config 5, heterogeneous, moving clock)')
     ap.add_argument('--stop-after-e2e', action='store_true', help='developer switch: print value / e2e / clocks only and stop')
+    ap.add_argument('--dump-outputs', metavar='DIR', help='write the bindings of the last timed step as DIR/<field>.npy')
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3) if args.impl != 'reference' else args.warmup
 
@@ -333,7 +344,7 @@ def main():
     from nhd_b200.solver import Solver, nccl_unique_id, pinned_array, shard_min_pairs
 
     if not torch.cuda.is_available():
-        raise SystemExit('bench.py: no CUDA device; the B200 solver has no CPU fallback')
+        raise SystemExit('bench.py: no CUDA device; the solver has no CPU fallback')
     torch.cuda.set_device(local_rank)
     pinned = pin_near_gpu(torch, local_rank)          # before any host buffer is allocated; undone before the CPU legs
     if world > 1:
@@ -353,7 +364,7 @@ def main():
     solver.load_nodes(recs)
     solver.snapshot()
 
-    flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')      # > 126 MB L2
+    flush = torch.empty(256 << 20, dtype=torch.uint8, device='cuda')      # > 50 MB L2 of the H100
 
     def barrier():
         torch.cuda.synchronize()
@@ -396,6 +407,8 @@ def main():
     clocks = sampler.stop() if rank == 0 else None
     bindings = solver.fetch_bindings()
     n_types = t['n_types']
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, bindings)
 
     step_ms = float(np.sum(phase['total_ms']))
     if world > 1:
@@ -500,14 +513,6 @@ def main():
     dominant = 'sweep_kernel' if sweep_ms >= filter_ms else 'filter_kernel'
     dom_ms = max(sweep_ms, filter_ms)
     achieved = alg_bytes / (dom_ms / 1e3) / 1e9
-    traffic = traffic_at = None
-    try:
-        with open(os.path.join(ROOT, 'profiles', 'traffic.json')) as f:
-            tj = json.load(f)
-            traffic = tj.get(dominant)
-            traffic_at = tj.get('captured_at')          # commit / date of the ncu capture the figure comes from
-    except Exception:
-        pass
 
     # ---------------- CPU baseline on this box's host cores (bounded sample) ------------------
     cpu = None
@@ -574,13 +579,12 @@ def main():
                       'wall_per_step_incl_restore_and_flush': 1e3 * wall_s / args.steps},
         'roofline': {'bound': 'latency (1 SM, one warp: sequential first-fit chain)', 'bound_metric': 'hbm (algorithmic bytes)',
                      'kernel': dominant, 'achieved': achieved, 'peak': peak, 'unit': 'GB/s',
-                     'frac': achieved / peak, 'traffic': traffic, 'traffic_captured_at': traffic_at,
-                     'peak_source': peak_src, 'frac_of_nominal_8000': achieved / 8000.0,
+                     'frac': achieved / peak, 'peak_source': peak_src,
                      'algorithmic_bytes_per_launch': int(alg_bytes),
                      'note': 'achieved/frac use ALGORITHMIC bytes = reference-equivalent work (every eligible node '
                              'record read once per decision, SURVEY 8d), not DRAM traffic: the sweep keeps its working '
-                             'set in shared memory / L2 (traffic = ncu dram bytes per launch) and is bound by the '
-                             'latency of the dependent chain on one SM, not by HBM'},
+                             'set in shared memory / L2 and is bound by the latency of the dependent chain on one SM, '
+                             'not by HBM'},
         'roofline_filter': {
             'kernel': 'filter_kernel (+ fast_tables_kernel in front of it, inside the same pair of events)', 'bound': 'hbm',
             'bytes_per_launch': int(N * 128 + (n_types + 2) * N // 8 + N * 32),

@@ -1,5 +1,5 @@
 /*
- * nhd_b200.h — C-ABI of the B200-native NHD placement solver.
+ * nhd_b200.h — C-ABI of the H100-native NHD placement solver.
  *
  * This is the drop-in boundary for the one hot path of Viasat/nhd: the node
  * filter -> NUMA/PCIe intersection -> node select -> physical assignment loop.

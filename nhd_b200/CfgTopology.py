@@ -2,7 +2,7 @@
 
 Same class, attribute and method names as the reference (``CfgTopology.py:8-243``)
 so that code written against the reference scheduler (``NHDScheduler.py``,
-``TriadCfgParser.py:107-304``) can build requests for the B200 solver unchanged.
+``TriadCfgParser.py:107-304``) can build requests for the CUDA solver unchanged.
 These classes only *describe* a request; the solver reads them through
 ``nhd_b200.packing.pack_pod`` and writes its answer back into ``Core.core``,
 ``GPU.device_id``, ``NICGroup.mac`` and the VLAN fields, exactly where

@@ -1,5 +1,5 @@
 """``Matcher`` — drop-in replacement of the reference's ``nhd/Matcher.py`` backed by the
-B200 solver.
+CUDA solver.
 
 Same surface as the reference (``Matcher()`` no-arg constructor, ``FindNode(nl, top)``
 returning ``(nodename, mapping)`` or ``(None,)``, ``Matcher.py:22-63``), so

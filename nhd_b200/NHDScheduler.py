@@ -392,7 +392,7 @@ class NHDScheduler:
         if e.unsupported is not None:
             self._error(f'Pod {ns}.{podname} is outside the solver\'s limits: {e.unsupported}')
             k8s.GeneratePodEvent(pobj, podname, ns, 'FailedScheduling', K8SEventType.EVENT_TYPE_WARNING,
-                                 f'Pod {podname} cannot be placed by the B200 solver: {e.unsupported}')
+                                 f'Pod {podname} cannot be placed by the CUDA solver: {e.unsupported}')
             self.failed_schedule_count += 1
             self.unsupported_pods.append((ns, podname, e.unsupported))
             return False

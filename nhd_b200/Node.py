@@ -331,7 +331,7 @@ class Node:
         binding = mapping.get('_nhd_binding') if isinstance(mapping, dict) else None
         if binding is None:
             raise RuntimeError('mapping was not produced by nhd_b200.Matcher.FindNode; '
-                               'the B200 solver has no CPU fallback for physical assignment')
+                               'the CUDA solver has no CPU fallback for physical assignment')
         return apply_binding(self, top, binding)
 
     # ---- busy window (Node.py:843-853) ----------------------------------------------

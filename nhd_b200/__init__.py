@@ -1,7 +1,7 @@
-"""nhd_b200 — B200-native batched placement solver for the NHD scheduler's hot path.
+"""nhd_b200 — H100-native batched placement solver for the NHD scheduler's hot path.
 
 Layout:
-  csrc/            CUDA kernels (sm_100a) and the C-ABI library (include/nhd_b200.h)
+  csrc/            CUDA kernels (sm_90a) and the C-ABI library (include/nhd_b200.h)
   _lib, solver     ctypes binding and handle wrapper
   wire, packing    packed record formats and object <-> record conversion
   CfgTopology, Node, Matcher, NHDScheduler   host-side mirrors of the reference interface

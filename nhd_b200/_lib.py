@@ -40,13 +40,13 @@ def load():
         return _lib
     if not os.path.exists(LIB_PATH):
         raise RuntimeError(f'{LIB_PATH} is missing: build it with `python -m nhd_b200.build` '
-                           '(nvcc, sm_100a). The B200 solver has no CPU fallback.')
+                           '(nvcc, sm_90a). The solver has no CPU fallback.')
     L = ctypes.CDLL(LIB_PATH)
     if hasattr(L, 'nhd_emulated_device') and os.environ.get('NHD_B200_ALLOW_EMULATED') != '1':
         # tests build the library's sources on a CPU emulation of CUDA to exercise the kernels' logic without a
         # GPU; that build is never a way to *run* the solver
         raise RuntimeError(f'{LIB_PATH} is a CPU-emulated test build, not the CUDA library; refusing to load it '
-                           '(set NHD_B200_ALLOW_EMULATED=1 only in tests). The B200 solver has no CPU fallback.')
+                           '(set NHD_B200_ALLOW_EMULATED=1 only in tests). The solver has no CPU fallback.')
     vp, i32, i64 = ctypes.c_void_p, ctypes.c_int32, ctypes.c_int64
     sig = {
         'nhd_default_params': (None, [ctypes.POINTER(Params)]),

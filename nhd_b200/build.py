@@ -1,7 +1,7 @@
-"""Builds nhd_b200/libnhd_b200.so (the C-ABI library with the sm_100a kernels) in-tree.
+"""Builds nhd_b200/libnhd_b200.so (the C-ABI library with the sm_90a kernels) in-tree.
 
-nvcc cross-compiles without a GPU; the resulting .so travels to the B200 box with the
-repository snapshot (it is git-ignored, not gpurun-ignored)."""
+nvcc cross-compiles without a GPU; the resulting .so is a build product (git-ignored) that
+_lib.py loads from the package directory."""
 import os
 import shutil
 import subprocess
@@ -12,7 +12,7 @@ CSRC = os.path.join(HERE, 'csrc')
 LIB = os.path.join(HERE, 'libnhd_b200.so')
 SOURCES = [os.path.join(CSRC, 'nhd_api.cu'), os.path.join(CSRC, 'nhd_ingest.cpp')]
 DEPS = SOURCES + [os.path.join(CSRC, f) for f in ('nhd_kernels.cuh', 'nhd_core.cuh')] + \
-    [os.path.join(HERE, '..', 'include', 'nhd_b200.h')]
+    [os.path.join(HERE, '..', 'include', 'nhd_b200.h'), os.path.abspath(__file__)]   # this file: the nvcc flags
 
 
 def nvcc_path():
@@ -40,7 +40,7 @@ def build(force=False, verbose=False, profile=False, checks=False):
 
 
 def _compile(LIB, verbose, extra):
-    cmd = [nvcc_path(), '-gencode', 'arch=compute_100a,code=sm_100a', '-lineinfo', '-O3', '-std=c++17',
+    cmd = [nvcc_path(), '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
            '--fmad=false',                      # fp64 NIC arithmetic must stay subtract-then-compare (no contraction)
            '-Xcompiler', '-fPIC', '-shared', '-Xptxas', '-v' if verbose else '-O3',
            '-o', LIB] + extra + SOURCES + ['-ldl']

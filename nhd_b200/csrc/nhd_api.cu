@@ -1,5 +1,5 @@
 /*
- * nhd_api.cu — the C-ABI of include/nhd_b200.h on top of the sm_100a kernels.
+ * nhd_api.cu — the C-ABI of include/nhd_b200.h on top of the sm_90a kernels.
  *
  * Host side of the drop-in boundary: owns the device mirror of the cluster (tiled node
  * records in HBM), de-duplicates the pod descriptors of a batch into pod types, launches
@@ -66,7 +66,7 @@ struct nhd_handle {
     double cap[NHD_MAX_SPEED_CLASSES];
     cudaStream_t stream = nullptr;
     cudaEvent_t ev[4] = {nullptr, nullptr, nullptr, nullptr};
-    int sm_count = 148;
+    int sm_count = 132;
     int smem_optin = 48 * 1024;
     ncclComm_t comm = nullptr;
 
@@ -235,9 +235,10 @@ extern "C" void nhd_default_params(nhd_params* p)
 
 /*
  * Node-sharding threshold: (nodes x distinct pod types) from which the snapshot filter is split over the ranks.
- * Below it the exchange costs more than the shard saves — measured on B200s over NVSwitch: the whole filter of
- * 65 536 nodes x 16 types takes 0.047 ms on one GPU, the all-gather + unpack of its bitmaps 0.026 / 0.029 / 0.070 ms
- * on 2 / 4 / 8 ranks — so every rank filters the whole cluster and no collective runs.  Every rank must use the same
+ * Below it every rank filters the whole cluster and no collective runs.  The default was chosen where an earlier GPU's
+ * all-gather + unpack of the bitmaps cost more than the shard saves; the whole filter of 65 536 nodes x 16 types takes
+ * 0.05 ms on one H100 SXM (400 W power limit), but the exchange cost on H100s has not been measured, so the threshold
+ * is carried over unchanged.  Every rank must use the same
  * value (it decides whether the collective is entered): NHD_SHARD_MIN_PAIRS in the environment of all ranks, read
  * when a handle is created; default 2^21.
  */

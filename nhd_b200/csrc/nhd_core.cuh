@@ -1,5 +1,5 @@
 /*
- * nhd_core.cuh — per-(pod type, node) placement arithmetic of the B200 solver.
+ * nhd_core.cuh — per-(pod type, node) placement arithmetic of the CUDA solver.
  *
  * Everything here is scalar, branch-light bitmask code over the packed
  * nhd_node_rec (include/nhd_b200.h).  The CUDA kernels (nhd_kernels.cu) call
@@ -9,7 +9,7 @@
  * with g++ and diff it against the oracle without a GPU; the shipped library
  * never runs them on the host.
  *
- * What each block replaces in the reference (file:line under /root/reference):
+ * What each block replaces in the reference (file:line in the reference checkout):
  *   free_cores / free_gpus / nic tables   nhd/Node.py:250-296, 456-462
  *   gpu_ok / cpu_ok / nic_first_fit       nhd/Matcher.py:95-276 (+ PCI pruning :295-335)
  *   choose_mapping (+ the set emulator)   nhd/Matcher.py:337-389, 423-452

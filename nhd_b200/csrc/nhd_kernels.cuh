@@ -1,5 +1,5 @@
 /*
- * nhd_kernels.cuh — sm_100a kernels of the NHD placement solver (one batch = 5 launches).
+ * nhd_kernels.cuh — sm_90a kernels of the NHD placement solver (one batch = 5 launches).
  *
  *   ingest / validate / classify / export   layout conversion of uploaded wire records, device-side
  *                   record validation, exact hardware-class ids of the nodes' static descriptions

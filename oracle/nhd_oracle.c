@@ -19,7 +19,7 @@
  * eligible node is evaluated for every pod, candidate lists are materialised,
  * and Python set semantics come from pyset_model.c.
  *
- * Reference functions restated (file:line under /root/reference):
+ * Reference functions restated (file:line in the reference checkout):
  *   NHDScheduler.InitialNodeFilter        nhd/NHDScheduler.py:235-247
  *   NHDScheduler.AttemptScheduling        nhd/NHDScheduler.py:277-304 (compute lines)
  *   Matcher.FindNode                      nhd/Matcher.py:27-63

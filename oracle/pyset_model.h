@@ -6,7 +6,7 @@
  *   - the tuple hash of CPython >= 3.8 (Objects/tupleobject.c, tuplehash), and
  *   - the open-addressing table of `set` (Objects/setobject.c: set_add_entry,
  *     set_insert_clean, set_table_resize, set_intersection, iteration order).
- * CPython is not part of /root/reference; the algorithm is the published one of
+ * CPython is not part of the reference; the algorithm is the published one of
  * CPython 3.8 .. 3.12 and is pinned against the running interpreter (3.12.3) by
  * tests/test_pyset_model.py.
  *

@@ -1,10 +1,11 @@
-"""Load the UNMODIFIED reference hot-path modules from /root/reference.
+"""Load the UNMODIFIED reference hot-path modules from the checkout named by
+NHD_REFERENCE_ROOT.
 
-TEST INFRASTRUCTURE ONLY (oracle).  Works only in the build container: the GPU
-box has no /root/reference, so nothing under `-m gpu`, smoke() or bench.py may
-import this module.  It is used by tests/golden/make_golden.py (to freeze
-golden vectors) and by the live differential tests (skipped when the reference
-is absent).
+TEST INFRASTRUCTURE ONLY (oracle).  The reference is not part of this
+repository, so no test or smoke() imports this module.  It is used by the
+generators under tests/golden/ (make_golden.py, make_live_golden.py, ...) to
+freeze golden vectors, and by the optional Python-reference leg of bench.py
+(through tests/pyref.py), which runs only when NHD_REFERENCE_ROOT is set.
 
 Recipe follows SURVEY.md appendix D: a `colorlog` stub on sys.path, logging
 disabled, and a fake clock patched into nhd.Node.time.monotonic so the 30 s
@@ -15,12 +16,12 @@ import os
 import sys
 import types
 
-REFERENCE_ROOT = os.environ.get('NHD_REFERENCE_ROOT', '/root/reference')
+REFERENCE_ROOT = os.environ.get('NHD_REFERENCE_ROOT', '')
 _SHIM = os.path.join(os.path.dirname(os.path.abspath(__file__)), '_shim')
 
 
 def available() -> bool:
-    return os.path.isfile(os.path.join(REFERENCE_ROOT, 'nhd', 'Matcher.py'))
+    return bool(REFERENCE_ROOT) and os.path.isfile(os.path.join(REFERENCE_ROOT, 'nhd', 'Matcher.py'))
 
 
 class FakeClock:

@@ -1,6 +1,6 @@
-"""Load the UNMODIFIED reference scheduler (nhd/NHDScheduler.py) from /root/reference.
+"""Load the UNMODIFIED reference scheduler (nhd/NHDScheduler.py) from NHD_REFERENCE_ROOT.
 
-TEST INFRASTRUCTURE ONLY (oracle), build container only — same rules as ref_loader.py.
+TEST INFRASTRUCTURE ONLY (oracle), golden-vector generators only — same rules as ref_loader.py.
 
 ``nhd.NHDScheduler`` imports ``kubernetes`` (through ``nhd.K8SMgr``), ``libconf`` and
 ``magicattr`` (through ``nhd.TriadCfgParser``), none of which exist here (SURVEY 8c).  The last two

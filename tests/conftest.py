@@ -9,12 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line('markers', 'gpu: needs a CUDA device (run on the B200 box)')
-    config.addinivalue_line('markers', 'reference: needs the unmodified reference under /root/reference')
-
-
-def has_reference():
-    return os.path.isfile('/root/reference/nhd/Matcher.py')
+    config.addinivalue_line('markers', 'gpu: needs a CUDA device (an H100)')
 
 
 @pytest.fixture(scope='session')

@@ -142,7 +142,7 @@ void run_grid(const char* name, dim3 grid, dim3 block, size_t dyn_smem, std::fun
     if (g_blk) fail("nested kernel launch");
     if ((block.x * block.y * block.z + 31) / 32 > 64) fail("blocks of more than 64 warps are not supported");
     if (dyn_smem > 227 * 1024 || dyn_smem > sizeof(nhd::smem))          /* sharedMemPerBlockOptin of the emulated device */
-        fail("launch asks for %zu bytes of dynamic shared memory (the B200 allows 232448)", dyn_smem);
+        fail("launch asks for %zu bytes of dynamic shared memory (the H100 allows 232448)", dyn_smem);
     if (block.x * block.y * block.z > 1024) fail("launch with %u threads per block", block.x * block.y * block.z);
     Block& b = g_block;
     const int n = (int)(block.x * block.y * block.z);

@@ -14,7 +14,7 @@
  *     mask or kind: undefined behaviour on the GPU) aborts with a message;
  *   - memory is sequentially consistent (one OS thread), so fences are no-ops: the emulation checks the
  *     logic and the control-flow convergence rules, not the memory model;
- *   - cudaMalloc is calloc, copies are memcpy, streams and events do nothing, one device with 148 SMs;
+ *   - cudaMalloc is calloc, copies are memcpy, streams and events do nothing, one device with 132 SMs (an H100 SXM);
  *   - mbarrier + cp.async.bulk (the TMA staging of filter_kernel) are emulated with a byte-counting
  *     phase barrier and a synchronous memcpy.
  */
@@ -71,8 +71,8 @@ static inline cudaError_t cudaGetDeviceProperties(cudaDeviceProp* p, int)
 {
     memset(p, 0, sizeof(*p));
     snprintf(p->name, sizeof(p->name), "CPU emulation (tests/emu)");
-    p->multiProcessorCount = 148; p->sharedMemPerBlockOptin = 227 * 1024; p->sharedMemPerBlock = 48 * 1024;
-    p->major = 10; p->minor = 0; p->totalGlobalMem = (size_t)180 << 30;
+    p->multiProcessorCount = 132; p->sharedMemPerBlockOptin = 227 * 1024; p->sharedMemPerBlock = 48 * 1024;
+    p->major = 9; p->minor = 0; p->totalGlobalMem = (size_t)80 << 30;
     return cudaSuccess;
 }
 static inline const char* cudaGetErrorString(cudaError_t e) { return e == cudaSuccess ? "no error" : "emulated CUDA error"; }

@@ -1,11 +1,12 @@
 """SURVEY 8f row 2 — the request codec: a pod's libconfig text <-> ``CfgTopology``
 (``nhd_b200.TriadCfgParser`` on ``nhd_b200.libconfig``) against the UNMODIFIED reference class
-``nhd.TriadCfgParser`` (build container; it runs on stand-ins for the absent third-party ``libconf`` /
+``nhd.TriadCfgParser`` (run on stand-ins for the absent third-party ``libconf`` /
 ``magicattr`` under ``oracle/_shim`` — parity of the libconfig *text layout* with the real package is
 therefore unpinned, see DESIGN 8.4; parity of everything the reference class itself computes is pinned).
 
-* live: random Triad configs (``tests/triad_cfg.py``) through both — parsed topology, rewritten
-  config text after a placement, GPU-map annotation, re-parse with the network section; broken configs;
+* random Triad configs (``tests/triad_cfg.py``) — parsed topology, rewritten config text after a
+  placement, GPU-map annotation, re-parse with the network section; broken configs — against
+  the reference's outcomes, frozen by ``tests/golden/make_live_golden.py``;
 * frozen: ``tests/golden/codec/cases.json`` made from the reference by ``make_codec_golden.py``;
 * properties of the libconfig reader / writer on their own (round trip, number forms, escapes, paths).
 """
@@ -18,7 +19,7 @@ import pytest
 from nhd_b200 import libconfig
 from nhd_b200.TriadCfgParser import TriadCfgParser
 from tests import triad_cfg as T
-from tests.conftest import has_reference
+from tests.golden import make_live_golden as live
 
 GOLDEN = os.path.join(os.path.dirname(__file__), 'golden', 'codec', 'cases.json')
 
@@ -133,29 +134,24 @@ def test_codec_reproduces_golden():
     assert kinds['topology'] > 80 and kinds['none'] > 20 and kinds['raises'] > 5, kinds
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not has_reference(), reason='needs /root/reference (build container)')
 def test_codec_matches_live_reference():
-    from oracle import ref_sched_loader
-    Ref = ref_sched_loader.load_codec().codec.TriadCfgParser
-    rng = np.random.default_rng(77)
+    """Random configs against the reference's outcomes, frozen in tests/golden/live/codec.json.gz
+    (tests/golden/make_live_golden.py)."""
+    golden = live.load('codec')
     n = texts = 0
-    for seed in range(120):
-        pod = T.codec_pod(rng, 'wild' if seed % 2 else 'mixed')
-        text = T.pod_to_cfg(pod, rng, gpu_type=[None, 'V100', 'bogus'][seed % 3])
-        want = run_case(Ref, text, False, seed)
+    for (seed, text, broken), want in zip(live.codec_stream(), golden, strict=True):
+        assert want['seed'] == seed
         got = run_case(TriadCfgParser, text, False, seed)
-        assert got == want, seed
-        assert want['topology'] is not None
+        assert got == want['parsed'], seed
+        assert got['topology'] is not None
         texts += 1
         # the rewritten config, read back with its network section (a deployed pod after a restart)
-        want2 = run_case(Ref, want['cfg'], True, seed)
         got2 = run_case(TriadCfgParser, got['cfg'], True, seed)
-        assert got2 == want2 and got2['topology'] is not None, seed
+        assert got2 == want['reread'] and got2['topology'] is not None, seed
         ids = [c[4] for g in got2['topology']['groups'] for c in g['proc'] + g['helpers']]
         assert all(x > 0 for x in ids)                           # physical ids survived the trip
-        if seed % 4 == 0:
-            for bad in broken_variants(text, rng):
-                assert run_case(TriadCfgParser, bad, False, seed) == run_case(Ref, bad, False, seed), (seed, bad[:80])
-                n += 1
+        assert len(broken) == len(want['broken']), seed
+        for bad, outcome in zip(broken, want['broken']):
+            assert run_case(TriadCfgParser, bad, False, seed) == outcome, (seed, bad[:80])
+            n += 1
     assert texts == 120 and n > 200

@@ -68,7 +68,7 @@ def test_every_sweep_mode_against_the_oracle_random(emu_cuda_lib, oracle_lib, sc
 
 
 def test_driver_smoke_entry_point_on_the_emulated_device(emu_cuda_lib, oracle_lib):
-    """``__graft_entry__.smoke()`` — what the driver runs on the B200 before the bench — end to end."""
+    """``__graft_entry__.smoke()`` — the one small run on the GPU — end to end."""
     env = dict(os.environ, NHD_B200_LIB=emu_cuda_lib, NHD_B200_ALLOW_EMULATED='1', EMU_LANE_ORDER='d')
     res = subprocess.run([sys.executable, '-c', 'import __graft_entry__ as g; g.smoke()'], cwd=ROOT, env=env,
                          capture_output=True, text=True, timeout=600)

@@ -11,7 +11,8 @@ import pytest
 from nhd_b200 import Node as mirror_node
 from nhd_b200 import packing, wire
 from nhd_b200.ingest import LabelError, LabelIngest
-from tests import conftest, scenarios
+from tests import scenarios
+from tests.golden import make_live_golden as live
 
 GOLDEN = os.path.join(os.path.dirname(os.path.abspath(__file__)), 'golden', 'ingest', 'cases.json')
 
@@ -149,28 +150,33 @@ def test_batch_ingest_brings_a_cluster_up_like_build_initial_node_list():
         assert recs[i].tobytes() == r.tobytes(), i
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not conftest.has_reference(), reason='reference not present on this machine')
 def test_fuzzed_labels_against_the_live_reference():
-    """Seeded damage to valid label dictionaries: the native parser and the unmodified reference must agree on
-    accept / return False / raise / beyond-limits, and on every byte of the accepted records."""
-    from oracle import ref_loader
+    """Seeded damage to valid label dictionaries: the native parser and the unmodified reference (its outcomes frozen
+    in tests/golden/live/ingest.json.gz by tests/golden/make_live_golden.py) must agree on accept / return False /
+    raise / beyond-limits, and on every byte of the accepted records."""
     from tests.golden import make_ingest_golden as mk
-    ref = ref_loader.load()
+    golden = live.load('ingest')
     rng = random.Random(5)
     cases = mk.mutations(rng, 400)
-    ing, layout = LabelIngest(), packing.ClusterLayout()
+    ing = LabelIngest()
     kinds = {}
-    for case in cases:
+    for case, want in zip(cases, golden['fuzz'], strict=True):
         kind, rec, aux = _native(ing, case)
-        okind, orec, n = _object_path(ref.node, case, layout)
-        assert kind == okind, (case['name'], kind, okind, case['labels'])
+        assert kind == want['kind'], (case['name'], kind, want['kind'], case['labels'])
         kinds[kind] = kinds.get(kind, 0) + 1
         if kind == 'ok':
-            assert rec.tobytes() == orec.tobytes(), case['name']
-            _check_aux(case, rec, aux, n)
+            assert rec.tobytes().hex() == want['record'], case['name']
+            assert int(aux['data_vlan']) == want['data_vlan']
+            assert int(aux['res_hugepages_gb']) == want['res_hugepages_gb']
+            assert int(aux['n_reserved_cores']) == want['n_reserved_cores']
+            n_gpus = len(want['gpu_device_id'])
+            assert aux['gpu_device_id'][:n_gpus].tolist() == want['gpu_device_id']
+            assert (aux['gpu_device_id'][n_gpus:] == -1).all()
+            keys = list(case['labels'].keys())
+            assert [keys[i].split('.')[4] for i in aux['nic_label'][:len(want['nic_ifname'])]] == want['nic_ifname']
+            assert keys[int(aux['gw_label'])] == 'DATA_DEFAULT_GW'
     assert kinds.get('ok', 0) > 100 and kinds.get('raises', 0) > 10 and kinds.get('false', 0) > 5, kinds
-    assert ing.speed_table().tolist() == layout.speed_table().tolist()
+    assert ing.speed_table().tolist() == golden['speed_table']
 
 
 # ---- node statistics off packed records (SURVEY 8f row 4, the part the packed state carries) -------------
@@ -229,26 +235,16 @@ def test_node_stats_match_mirror_getters_after_scheduling(oracle_lib, flavor):
         _check_stats(final, _stats_of_objects(order))
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not conftest.has_reference(), reason='reference not present on this machine')
 def test_node_stats_match_reference_getters_after_scheduling():
     """Same against the unmodified reference: its own scheduler loop leaves Node objects behind whose getters
-    (what GetBasicNodeStats calls, nhd/NHDScheduler.py:355-378) must agree with the packed records' counters."""
-    from oracle import ref_loader
-    ref = ref_loader.load()
-    import contextlib
-    import io
-    for seed, flavor in enumerate(['mixed', 'wild', 'vf', 'big', 'mixed', 'big']):
-        scn = scenarios.random_scenario(45000 + seed, n_nodes=8, n_pods=30, flavor=flavor)
-        nodes = scenarios.build_nodes(scn, ref.node)
-        matcher = ref.matcher.Matcher()
-        for pod, t in zip(scn['pods'], scn['now']):
-            top = scenarios.build_top(pod, ref.cfg)
-            with contextlib.redirect_stdout(io.StringIO()):
-                ref_loader.attempt_scheduling(ref, matcher, nodes, top, pod['groups'], t)
-        order = list(nodes.values())
-        recs = packing.pack_nodes(order, packing.ClusterLayout())
-        _check_stats(recs, _stats_of_objects(order))
+    (what GetBasicNodeStats calls, nhd/NHDScheduler.py:355-378) must agree with the packed records' counters.
+    Those records and getter values are frozen in tests/golden/live/ingest.json.gz (tests/golden/make_live_golden.py)."""
+    golden = live.load('ingest')['stats']
+    assert len(golden) == 6
+    for want in golden:
+        recs = np.frombuffer(bytes.fromhex(want['records']), dtype=wire.NODE_DTYPE)
+        assert len(recs) == 8
+        _check_stats(recs, want['rows'])
 
 
 @pytest.mark.parametrize('config,wild', [(4, False), (5, False), (4, True)])

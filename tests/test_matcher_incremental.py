@@ -1,13 +1,13 @@
 """``Matcher.FindNode`` under the reference scheduler's calling pattern (one call per pod on the filtered node dict,
 ``NHDScheduler.py:235-247,277-304``) with the change counters of ``nhd_b200/tracking.py``: only the nodes that
 changed since the previous call are packed and uploaded, and every answer equals that of a matcher that packs the
-whole dict on every call.  Runs on the B200 (``-m gpu``) and, in the CPU suite, on the emulated device."""
+whole dict on every call.  Runs on the GPU (``-m gpu``) and, in the CPU suite, on the emulated device."""
 import numpy as np
 import pytest
 
 import nhd_b200.CfgTopology as cfg_mod
 import nhd_b200.Node as node_mod
-from tests import conftest, scenarios
+from tests import scenarios
 
 
 def _initial_filter(nodes, groups):
@@ -89,16 +89,3 @@ def _session(nmod, cmod, seed, n_nodes, n_steps, flavor):
 @pytest.mark.parametrize('flavor', ['mixed', 'wild'])
 def test_incremental_matcher_equals_full_repack_on_mirror_nodes(flavor):
     _session(node_mod, cfg_mod, 9100 + len(flavor), n_nodes=24, n_steps=70, flavor=flavor)
-
-
-@pytest.mark.gpu
-@pytest.mark.skipif(not conftest.has_reference(), reason='needs the unmodified reference (build container only)')
-def test_incremental_matcher_on_the_references_own_node_objects():
-    """Route 1 of INTEGRATION.md: the reference's nhd.Node.Node objects, instrumented in place, mutated by the
-    reference's own SetPhysicalIdsFromMapping / AddResourcesFromTopology."""
-    import contextlib
-    import io
-    from oracle import ref_loader
-    ref = ref_loader.load()
-    with contextlib.redirect_stdout(io.StringIO()):
-        _session(ref.node, ref.cfg, 9207, n_nodes=24, n_steps=70, flavor='mixed')

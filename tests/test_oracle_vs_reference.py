@@ -1,71 +1,64 @@
-"""Live differential test: the C oracle against the UNMODIFIED reference modules imported from
-/root/reference (build container only; skipped on the GPU box).  This is the pin that makes the
-oracle trustworthy; the frozen copies of such runs are tests/golden/*.json."""
+"""Differential test: the C oracle against the UNMODIFIED reference, whose outcomes on these scenarios are frozen in
+tests/golden/live/oracle.json.gz (tests/golden/make_live_golden.py).  This is the pin that makes the oracle
+trustworthy; tests/golden/*.json are further frozen runs of the same kind."""
+import numpy as np
 import pytest
 
-from tests import conftest, ref_compare, scenarios
+from nhd_b200 import wire
+from tests import ref_compare, scenarios
+from tests.golden import make_live_golden as live
 
-pytestmark = pytest.mark.skipif(not conftest.has_reference(), reason='reference not present on this machine')
+
+def _records(hexstr):
+    return np.frombuffer(bytes.fromhex(hexstr), dtype=wire.NODE_DTYPE)
+
+
+def _compare(oracle_lib, scn, want, tag):
+    """-> (attempts, placed) after checking the oracle's run of scn against the reference's frozen one."""
+    init, final = _records(want['init']), _records(want['final'])
+    recs, pods, now, layout2 = ref_compare.pack_scenario(scn)
+    # the packer gives identical records from the reference's Node objects and from the mirrors
+    assert ref_compare.records_equal(recs, init), ref_compare.diff_records(recs, init)[:3]
+    b, orecs = oracle_lib.solve(recs, layout2.speed_table(), pods, now, min_busy_secs=scn['min_busy_secs'])
+    assert len(want['outs']) == len(b)
+    placed = 0
+    for i, (o, bb) in enumerate(zip(want['outs'], b)):
+        errs = ref_compare.diff_outcome(o, bb)
+        assert not errs, (tag, i, errs)
+        placed += o['status'] == 'placed'
+    assert not ref_compare.diff_records(orecs, final), tag
+    return len(b), placed
 
 
 @pytest.mark.parametrize('flavor', ['mixed', 'wild', 'vf', 'big'])
 def test_oracle_matches_live_reference(oracle_lib, flavor):
     attempts = placed = 0
-    for seed in range(30):
-        scn = scenarios.random_scenario(seed * 7 + {'mixed': 1, 'wild': 2, 'vf': 3, 'big': 4}[flavor] * 100003,
-                                        n_nodes=6, n_pods=30, flavor=flavor)
-        outs, init, final, layout, names = ref_compare.run_reference(scn)
-        recs, pods, now, layout2 = ref_compare.pack_scenario(scn)
-        # the packer gives identical records from the reference's Node objects and from the mirrors
-        assert ref_compare.records_equal(recs, init), ref_compare.diff_records(recs, init)[:3]
-        b, orecs = oracle_lib.solve(recs, layout2.speed_table(), pods, now, min_busy_secs=scn['min_busy_secs'])
-        for i, (o, bb) in enumerate(zip(outs, b)):
-            errs = ref_compare.diff_outcome(o, bb)
-            assert not errs, (flavor, seed, i, errs)
-            attempts += 1
-            placed += o['status'] == 'placed'
-        assert not ref_compare.diff_records(orecs, final), (flavor, seed)
+    golden = live.load('oracle')[flavor]
+    for seed, (scn, want) in enumerate(zip(live.oracle_scenarios(flavor), golden, strict=True)):
+        a, p = _compare(oracle_lib, scn, want, (flavor, seed))
+        attempts += a
+        placed += p
     assert attempts == 900 and placed > 150
 
 
-def test_mirror_node_ingest_matches_reference_labels(oracle_lib):
+def test_mirror_node_ingest_matches_reference_labels():
     """nhd_b200.Node.ParseLabels builds the same node as nhd.Node.ParseLabels (Node.py:312-487)."""
-    from oracle import ref_loader
     import nhd_b200.Node as mirror
-    ref = ref_loader.load()
-    for seed in range(40):
-        scn = scenarios.random_scenario(4242 + seed, n_nodes=5, n_pods=1, flavor='wild' if seed % 2 else 'vf')
-        a = scenarios.build_nodes(scn, ref.node)
-        b = scenarios.build_nodes(scn, mirror)
-        for name in a:
-            x, y = a[name], b[name]
-            assert [(c.core, c.socket, c.sibling, c.used) for c in x.cores] == \
-                [(c.core, c.socket, c.sibling, c.used) for c in y.cores]
-            assert [(g.device_id, g.numa_node, g.pciesw, g.gtype.value) for g in x.gpus] == \
-                [(g.device_id, g.numa_node, g.pciesw, g.gtype.value) for g in y.gpus]
-            assert [(n.ifname, n.mac, n.speed, n.numa_node, n.pciesw, n.idx, n.card, n.port) for n in x.nics] == \
-                [(n.ifname, n.mac, n.speed, n.numa_node, n.pciesw, n.idx, n.card, n.port) for n in y.nics]
-            assert (x.groups, x.maintenance, x.data_vlan, x.gwip, x.mem.free_hugepages_gb, x.reserved_cores,
-                    x.sockets, x.numa_nodes, x.smt_enabled, x.cores_per_proc) == \
-                (y.groups, y.maintenance, y.data_vlan, y.gwip, y.mem.free_hugepages_gb, y.reserved_cores,
-                 y.sockets, y.numa_nodes, y.smt_enabled, y.cores_per_proc)
+    golden = live.load('oracle')['node_descriptions']
+    for seed, (scn, want) in enumerate(zip(live.ingest_node_scenarios(), golden, strict=True)):
+        got = {name: live.node_description(n) for name, n in scenarios.build_nodes(scn, mirror).items()}
+        assert list(got) == list(want), seed
+        for name in want:
+            assert got[name] == want[name], (seed, name)
 
 
 def test_oracle_matches_live_reference_near_the_limits(oracle_lib):
     """Nodes with up to 256 logical cores / 16 GPUs / 32 NICs / 4 NUMA nodes and pods with up to 72 cores: the
     reference itself is slow here (seconds per pod), so a few short streams."""
     attempts = placed = 0
-    for seed in range(3):
-        scn = scenarios.huge_scenario(81000 + seed, min_busy_secs=30.0 if seed % 3 else 0.0)
-        scn['nodes'], scn['pods'], scn['now'] = scn['nodes'][:5], scn['pods'][:14], scn['now'][:14]
-        outs, init, final, layout, names = ref_compare.run_reference(scn)
-        recs, pods, now, layout2 = ref_compare.pack_scenario(scn)
-        assert ref_compare.records_equal(recs, init)
-        b, orecs = oracle_lib.solve(recs, layout2.speed_table(), pods, now, min_busy_secs=scn['min_busy_secs'])
-        for i, (o, bb) in enumerate(zip(outs, b)):
-            errs = ref_compare.diff_outcome(o, bb)
-            assert not errs, (seed, i, errs)
-            attempts += 1
-            placed += o['status'] == 'placed'
-        assert not ref_compare.diff_records(orecs, final), seed
+    golden = live.load('oracle')['near_limits']
+    for seed, (scn, want) in enumerate(zip(live.near_limit_scenarios(), golden, strict=True)):
+        a, p = _compare(oracle_lib, scn, want, seed)
+        attempts += a
+        placed += p
     assert attempts == 42 and placed > 20

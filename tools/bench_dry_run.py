@@ -1,5 +1,5 @@
 """bench.py's own arm on the CPU-emulated device of tests/emu with a stand-in `torch`: a dry run of the script's control
-flow before it is spent on the B200.  The numbers it prints describe the emulation, not the GPU.  Developer tool.
+flow before it is spent on the GPU.  The numbers it prints describe the emulation, not the GPU.  Developer tool.
 
     python tools/bench_dry_run.py --steps 2 --warmup 3 --cpu-sample-pods 16             (N = 1, full-size workload)
     python tools/bench_dry_run.py --world 2 --small --steps 2 --warmup 3                 (2 ranks: stand-ins for

@@ -1,5 +1,5 @@
 import sys, os
-sys.path.insert(0, '/root/repo')
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np, workload
 from nhd_b200.solver import Solver
 cfg = int(sys.argv[1]); cw = int(sys.argv[2])

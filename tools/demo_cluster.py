@@ -2,7 +2,7 @@
 libconfig text, `nhd_b200.NHDScheduler` batching the pending set through the solver, the rewritten config of one pod,
 and the gRPC statistics service answering a client.  Developer tool.
 
-    python tools/demo_cluster.py             # on the B200 (CUDA solver)
+    python tools/demo_cluster.py             # on the GPU (CUDA solver)
     python tools/demo_cluster.py --emulated  # anywhere: the same kernels on the CPU emulation of tests/emu
 """
 import os

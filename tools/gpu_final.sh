@@ -1,5 +1,5 @@
 #!/bin/bash
-# Developer script: everything the profiles/ directory records, on one GPU, for the current tree.
+# Developer script: GPU tests, profile, quick timings, checks build and scheduler bench on one GPU, for the current tree.
 mkdir -p gpurun_out
 timeout 2400 python -m pytest tests -m gpu -x -q > gpurun_out/pytest_gpu.log 2>&1
 bash tools/gpu_profile.sh > gpurun_out/gpu_profile.out 2>&1

@@ -1,5 +1,5 @@
 #!/bin/bash
-# Developer script: sanitizers + ncu evidence for profiles/ + bench line.  Output under gpurun_out/.
+# Developer script: sanitizers + ncu captures + bench line.
 mkdir -p gpurun_out
 for tool in racecheck synccheck memcheck; do
   timeout 900 compute-sanitizer --tool $tool --print-limit 20 python tools/sanitizer_run.py > gpurun_out/sanitizer_$tool.log 2>&1

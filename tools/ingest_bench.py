@@ -1,5 +1,5 @@
 """Node-ingest throughput (host side): labels -> packed records, native parser (nhd_ingest_node) against the
-Python object path (ParseLabels + SetHugepages + pack_node) of the mirror and, where /root/reference exists, of
+Python object path (ParseLabels + SetHugepages + pack_node) of the mirror and, where NHD_REFERENCE_ROOT names a checkout of it, of
 the unmodified reference.  python tools/ingest_bench.py [n_nodes]"""
 import os
 import sys

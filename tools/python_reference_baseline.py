@@ -1,7 +1,7 @@
 """The reference's own Python path timed on the BASELINE workloads (BASELINE.md section 3): the unmodified
 nhd/Matcher.py + nhd/Node.py, driven like NHDScheduler.AttemptScheduling, one thread, on the first pods of the stream
-at full cluster size.  Needs /root/reference (build container); the GPU box has none, so this number is reported from
-here and bench.py adds it to its line only where the reference is reachable.
+at full cluster size.  Needs a checkout of the reference named by NHD_REFERENCE_ROOT; bench.py adds the same number
+to its line only where that variable is set.
 
     python tools/python_reference_baseline.py [config] [n_pods]
 """
