@@ -13,6 +13,8 @@ LIB = os.path.join(HERE, 'libnhd_b200.so')
 SOURCES = [os.path.join(CSRC, 'nhd_api.cu'), os.path.join(CSRC, 'nhd_ingest.cpp')]
 DEPS = SOURCES + [os.path.join(CSRC, f) for f in ('nhd_kernels.cuh', 'nhd_core.cuh')] + \
     [os.path.join(HERE, '..', 'include', 'nhd_b200.h'), os.path.abspath(__file__)]   # this file: the nvcc flags
+NVCC_FLAGS = ['-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
+              '--fmad=false']                   # fp64 NIC arithmetic must stay subtract-then-compare (no contraction)
 
 
 def nvcc_path():
@@ -40,9 +42,7 @@ def build(force=False, verbose=False, profile=False, checks=False):
 
 
 def _compile(LIB, verbose, extra):
-    cmd = [nvcc_path(), '-gencode', 'arch=compute_90a,code=sm_90a', '-lineinfo', '-O3', '-std=c++17',
-           '--fmad=false',                      # fp64 NIC arithmetic must stay subtract-then-compare (no contraction)
-           '-Xcompiler', '-fPIC', '-shared', '-Xptxas', '-v' if verbose else '-O3',
+    cmd = [nvcc_path()] + NVCC_FLAGS + ['-Xcompiler', '-fPIC', '-shared', '-Xptxas', '-v' if verbose else '-O3',
            '-o', LIB] + extra + SOURCES + ['-ldl']
     res = subprocess.run(cmd, capture_output=True, text=True)
     if verbose or res.returncode != 0:

@@ -35,6 +35,12 @@
 
 #include "nhd_core.cuh"
 
+/* sweep_kernel's parameter attribute; only the CUDA headers define it, and a host compiler building these sources
+ * as plain C++ has nothing to do with it */
+#ifndef __grid_constant__
+#define __grid_constant__
+#endif
+
 namespace nhd {
 
 constexpr int TILE_NODES = 32;
@@ -197,6 +203,7 @@ struct ClsFast {             /* per hardware class, 16 bytes */
     uint8_t n0, n1;          /* NICs per NUMA node */
     uint32_t ok;             /* 1: covered by the direct path */
 };
+static_assert(sizeof(ClsFast) == 16, "fast_node_aux reads a class entry as one uint4");
 
 struct TyFast {              /* per pod type, 16 bytes */
     uint8_t G, n_misc, misc_smt, nic_groups;
@@ -1478,14 +1485,21 @@ __device__ __forceinline__ bool fast_node_aux(const FastTables& ft, const DynU& 
 {
     ax.iu = ax.li0 = ax.li1 = ax.sig = 0;
     if (((du.d.info >> 2) & 7) != 2 || du.d.hw_class == NHD_NO_CLASS) return false;
-    const ClsFast cf = ft.cls[du.d.hw_class];
+    /* one 16-byte load: its address hangs off the summary load, so a second round trip is all it may cost
+     * (the table only changes at load / update time, between sweeps) */
+    union { uint4 q; ClsFast c; } cu;
+    cu.q = __ldg(reinterpret_cast<const uint4*>(ft.cls) + du.d.hw_class);
+    const ClsFast cf = cu.c;
     /* the sweep keeps the table rows of the first few NIC signatures in shared memory (a generic or global load on
      * this chain costs 3-5 % of the whole sweep, measured); rarer signatures take the general path */
     if (!cf.ok || (smem_rows && (cf.sig0 >= FAST_NSIG_SMEM || cf.sig1 >= FAST_NSIG_SMEM))) return false;
     const uint32_t inuse = du.d.nic_inuse;
     uint32_t iu = 0;
-    for (int j = 0; j < cf.n0; j++) iu |= ((inuse >> ((cf.li0 >> (8 * j)) & 31)) & 1u) << j;
-    for (int j = 0; j < cf.n1; j++) iu |= ((inuse >> ((cf.li1 >> (8 * j)) & 31)) & 1u) << (4 + j);
+#pragma unroll
+    for (int j = 0; j < 4; j++) {            /* n0, n1 <= 4 wherever ok is set: unrolled, no branches on the chain */
+        iu |= (j < cf.n0 ? (inuse >> ((cf.li0 >> (8 * j)) & 31)) & 1u : 0u) << j;
+        iu |= (j < cf.n1 ? (inuse >> ((cf.li1 >> (8 * j)) & 31)) & 1u : 0u) << (4 + j);
+    }
     ax.iu = iu; ax.li0 = cf.li0; ax.li1 = cf.li1;
     ax.sig = (uint32_t)cf.sig0 | ((uint32_t)cf.sig1 << 8) | ((uint32_t)cf.n0 << 16) | ((uint32_t)cf.n1 << 24);
     return true;
@@ -1905,10 +1919,13 @@ __device__ __noinline__ int ordinary_pod(const SweepArgs& a, const SweepCtx& cx,
  *               write-back (Node.py:663-841 minus the core ids);
  *   invalidate  every pod type that can no longer fit on the node loses its bit right away.
  * On a constant clock the standing decisions above short-cut all of this for the common cases.
+ * The arguments are __grid_constant__: the general path takes `a` by reference, and a by-value kernel parameter whose
+ * address escapes is copied to the stack, which turns every field read of the per-pod chain into a local load plus a
+ * generic access (tools/sass_check.py checks the direct path for both).
  */
 template <bool SMEM_BITMAPS>
 __global__ void __launch_bounds__(SWEEP_THREADS, 1)
-sweep_kernel(const SweepArgs a)
+sweep_kernel(const __grid_constant__ SweepArgs a)
 {
     extern __shared__ __align__(1024) uint8_t smem[];
     const int tid = threadIdx.x, lane = tid & 31;
@@ -2064,7 +2081,7 @@ sweep_kernel(const SweepArgs a)
         uint64_t* const BMg = SMEM_BITMAPS ? s_bitmaps : a.bitmaps;
         uint64_t* const BUSYg = BMg + (size_t)(T + 1) * W;
         int32_t* const curs = s_cursors;
-        const PodType* tys = cx.types_in_smem ? s_types : a.types;
+        const PodType* tys = s_types;                /* split implies standing decisions, so the types are in shared memory */
         for (int i0 = 0; i0 < a.n_pods; i0 += 32) {
             const int my_ti = (i0 + lane < a.n_pods) ? a.pod_type[i0 + lane] : 0;
             const double my_now = (i0 + lane < a.n_pods) ? a.now[i0 + lane] : 0.0;
@@ -2213,7 +2230,6 @@ sweep_kernel(const SweepArgs a)
         const int ti = __shfl_sync(0xFFFFFFFFu, my_ti, j);
         const double now = cclock ? now0 : __shfl_sync(0xFFFFFFFFu, my_now, j);
         const unsigned long long gm = multi ? (__shfl_sync(0xFFFFFFFFu, my_gm, j) & a.names_used) : 0ULL;
-        const PodType& t = types[ti];
         nhd_binding* bout = &a.out[i];
         uint64_t* F = BM + (size_t)ti * W;
 
@@ -2235,6 +2251,7 @@ sweep_kernel(const SweepArgs a)
                 dax.li1 = __shfl_sync(0xFFFFFFFFu, sl.ax.li1, ti); dax.sig = __shfl_sync(0xFFFFFFFFu, sl.ax.sig, ti);
 #ifdef NHD_CHECKS
                 {
+                    const PodType& t = types[ti];
                     DynU dx; load_dyn(a, cx, node, dx);
                     CHK_SANE(dx, node, 2);
                     if (dx.q[0].y != w14) CHK_FAIL(3, node, dx.q[0].y, w14);
@@ -2291,7 +2308,8 @@ sweep_kernel(const SweepArgs a)
                 handled = true;
                 PROF_COUNT(12);
             } else if (kind == NHD_SLOT_NONE) {
-                if (lane < 8) reinterpret_cast<uint4*>(bout)[lane] = make_uint4(lane == 0 ? NHD_NO_CANDIDATE : 0, lane == 0 ? 0xFFFFFFFFu : 0, lane == 0 ? t.G : 0, 0);
+                const int G = s_types[ti].G;           /* standing decisions imply the types are in shared memory */
+                if (lane < 8) reinterpret_cast<uint4*>(bout)[lane] = make_uint4(lane == 0 ? NHD_NO_CANDIDATE : 0, lane == 0 ? 0xFFFFFFFFu : 0, lane == 0 ? G : 0, 0);
                 handled = true;
             }
         }

@@ -1,6 +1,10 @@
 """Developer A/B probe: BASELINE config 4 on the library named by NHD_B200_LIB (relative to nhd_b200/), device-timed,
 L2 flushed between solves; prints one JSON line with the per-phase means and a digest of the bindings, so that builds of
-different revisions can be compared in one visit to the GPU box."""
+different revisions can be compared in one visit to the GPU box.
+
+    python tools/ab_bench.py [4 | 5 | wild | moving]
+
+`wild` and `moving` are bench.py's side workloads on config 4: heterogeneous NICs, and per-pod clocks."""
 import hashlib
 import json
 import os
@@ -11,8 +15,10 @@ import torch
 import workload
 from nhd_b200.solver import Solver
 
-cfg = int(sys.argv[1]) if len(sys.argv) > 1 else 4
-recs, speed, pods, now = workload.make_workload(cfg)
+cfg = sys.argv[1] if len(sys.argv) > 1 else '4'
+recs, speed, pods, now = workload.make_workload(4 if cfg in ('wild', 'moving') else int(cfg), wild=cfg == 'wild')
+if cfg == 'moving':
+    now = now + 0.001 * np.arange(len(pods))
 s = Solver(speed)
 s.load_nodes(recs)
 s.snapshot()
