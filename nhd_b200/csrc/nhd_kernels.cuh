@@ -207,7 +207,7 @@ static_assert(sizeof(ClsFast) == 16, "fast_node_aux reads a class entry as one u
 
 struct TyFast {              /* per pod type, 16 bytes */
     uint8_t G, n_misc, misc_smt, nic_groups;
-    uint8_t direct;          /* CPU-only, NUMA mode, G <= 2 */
+    uint8_t direct;          /* CPU-only, NUMA mode, G <= 2, at most 63 physical cores in all */
     uint8_t pad_[3];
     int32_t hugepages_gb;
     uint32_t pad2_;
@@ -328,7 +328,10 @@ __global__ void fast_tables_kernel(const TablesArgs a)
     const int T = a.n_types, tt = blockIdx.x, i = threadIdx.x;
     if (tt >= T) return;
     const PodType& ty = a.types[tt];
-    const bool direct = ty.valid_map && !ty.needs_gpu && !ty.pci && ty.G <= 2;
+    /* TB indexes the free cores of a socket clamped at 63: exact only while no tuple asks a socket for more than 63,
+     * which holds when the whole demand does (larger types: node_feasible_k2 in the filter, the general path in the sweep) */
+    const bool direct = ty.valid_map && !ty.needs_gpu && !ty.pci && ty.G <= 2 &&
+                        (ty.need_smt > ty.need_nosmt ? ty.need_smt : ty.need_nosmt) <= 63;
     {
         /* NIC stage per NUMA node (Matcher.py:242-268): per (type, NIC signature, NICs in use) and tuple p, whether
          * the groups p puts on NUMA 0 (SUB0) / NUMA 1 (SUB1) get NICs there, and which; blockIdx.y walks the signatures */
@@ -362,7 +365,7 @@ __global__ void fast_tables_kernel(const TablesArgs a)
         for (int q = 0; q < (1 << L) && L <= 3; q++) {
             int n = 0;
             for (int g = 0; g < L; g++) if (((q >> (L - 1 - g)) & 1) == k) n += cl[g];
-            if (n <= c || (c == 63 && n <= 255)) m |= 1u << q;       /* the free count saturates at 63 in the index */
+            if (n <= c) m |= 1u << q;           /* c = 63 stands for 63 or more free: exact for the direct types, n <= 63 */
         }
         a.out[ftab_off_tb(T) + (size_t)tt * 256 + i] = (uint8_t)m;
     }

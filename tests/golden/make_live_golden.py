@@ -5,7 +5,7 @@ compares against.  A scheduler session's end state is large (mostly the Kubernet
 summary — the binds Kubernetes saw and the failed-scheduling count — and a SHA-256 fingerprint of the whole
 canonical JSON (``fingerprint``), so a failing comparison still names the first bind that differs.
 
-    NHD_REFERENCE_ROOT=<checkout of the reference> python tests/golden/make_live_golden.py
+    NHD_REFERENCE_ROOT=<checkout of the reference> python tests/golden/make_live_golden.py [oracle sched codec ingest rpc]
 """
 import contextlib
 import gzip
@@ -129,6 +129,7 @@ def make_oracle():
     ref = ref_loader.load()
     doc = {f: [_records(s) for s in oracle_scenarios(f)] for f in ('mixed', 'wild', 'vf', 'big')}
     doc['near_limits'] = [_records(s) for s in near_limit_scenarios()]
+    doc['nic_fp64'] = [_records(s) for s in scenarios.nic_bandwidth_scenarios()]
     doc['node_descriptions'] = [{name: node_description(n) for name, n in scenarios.build_nodes(s, ref.node).items()}
                                 for s in ingest_node_scenarios()]
     _save('oracle', doc)
@@ -231,16 +232,16 @@ def make_rpc():
     _save('rpc', {'proto': proto, 'responses': responses, 'fractional_gbps': fractional_gbps})
 
 
-def main():
+MAKERS = {'oracle': make_oracle, 'sched': make_sched, 'codec': make_codec, 'ingest': make_ingest, 'rpc': make_rpc}
+
+
+def main(names):
     from oracle import ref_loader
     if not ref_loader.available():
         raise SystemExit('set NHD_REFERENCE_ROOT to a checkout of the reference')
-    make_oracle()
-    make_sched()
-    make_codec()
-    make_ingest()
-    make_rpc()
+    for name in names or MAKERS:
+        MAKERS[name]()
 
 
 if __name__ == '__main__':
-    main()
+    main(sys.argv[1:])

@@ -46,13 +46,15 @@ def _run_gpu_tests(lib, extra_env=None, select=None):
 def test_gpu_suite_passes_on_the_emulated_device(emu_cuda_lib, lane_order):
     """Between two collectives the lanes of a warp run in a fixed order: both orders must give the oracle's answers
     (a lane-0 update of a word the other lanes still have to read shows up as a divergence in one of them)."""
-    # ascending: the whole -m gpu suite; descending: the parity tests proper (keeps the CPU suite to a few minutes)
+    # ascending: the whole -m gpu suite; descending: the parity tests proper and the limit cases (keeps the CPU suite
+    # to a few minutes)
     res = _run_gpu_tests(emu_cuda_lib, extra_env={'EMU_LANE_ORDER': lane_order},
-                         select=None if lane_order == 'a' else 'random_scenarios or constant_clock or clock_changes or edge_cases')
+                         select=None if lane_order == 'a' else
+                         'random_scenarios or constant_clock or clock_changes or edge_cases or gpu_limits')
     tail = (res.stdout + res.stderr)[-3000:]
     assert res.returncode == 0, tail
     last = [ln for ln in res.stdout.strip().splitlines() if 'passed' in ln][-1]
-    assert 'failed' not in last and int(last.split()[0]) >= (60 if lane_order == 'a' else 6), last
+    assert 'failed' not in last and int(last.split()[0]) >= (90 if lane_order == 'a' else 35), last
 
 
 @pytest.mark.parametrize('sched_seed', ['', '1', '2'], ids=['round_robin', 'shuffled1', 'shuffled2'])

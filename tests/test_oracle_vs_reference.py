@@ -62,3 +62,16 @@ def test_oracle_matches_live_reference_near_the_limits(oracle_lib):
         attempts += a
         placed += p
     assert attempts == 42 and placed > 20
+
+
+def test_oracle_matches_live_reference_on_non_dyadic_nic_bandwidth(oracle_lib):
+    """Group Gb/s such as 0.1, 0.3, 12.7 and 33.3, summed per group in core order and taken off a NIC in group order,
+    leave remainders of exactly 0 or an ulp either side of it (tests/scenarios.py, nic_bandwidth_scenarios): the
+    per-group sums of the packing and the oracle's subtraction order against the reference's."""
+    attempts = placed = 0
+    golden = live.load('oracle')['nic_fp64']
+    for seed, (scn, want) in enumerate(zip(scenarios.nic_bandwidth_scenarios(), golden, strict=True)):
+        a, p = _compare(oracle_lib, scn, want, scn['id'])
+        attempts += a
+        placed += p
+    assert attempts == 96 and placed > 40
