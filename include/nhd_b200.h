@@ -59,6 +59,20 @@ extern "C" {
 #define NHD_REF_WOULD_CRASH     3   /* unwind hit the buggy NIC rollback (Node.py:831-835); state as IndexError  */
 #define NHD_BAD_MAP_TYPE        4   /* map_type not NUMA/PCI -> (None,) (Matcher.py:45-47)                       */
 
+/* Why a node could not take a NO_CANDIDATE pod (nhd_explain_batch / nhd_explain_pod): the FIRST stage of the
+ * reference, in this order, that drops the node, evaluated on the cluster as that pod saw it. */
+#define NHD_WHY_GROUP           0   /* no node-group in common with the pod   (NHDScheduler.py:240)          */
+#define NHD_WHY_INACTIVE        1   /* node not active                        (NHDScheduler.py:241)          */
+#define NHD_WHY_MAINTENANCE     2   /* node in maintenance                    (Matcher.py:73)                */
+#define NHD_WHY_HUGEPAGES       3   /* pod's hugepages_gb > node's free        (Matcher.py:78)                */
+#define NHD_WHY_BUSY            4   /* GPU pod inside the node's busy window   (Matcher.py:107-111)           */
+#define NHD_WHY_GPU             5   /* no NUMA tuple of free GPUs              (Matcher.py:132)               */
+#define NHD_WHY_CPU             6   /* no NUMA tuple of free CPU cores         (Matcher.py:214)               */
+#define NHD_WHY_NIC             7   /* no NIC combination with the bandwidth   (Matcher.py:270)               */
+#define NHD_WHY_INTERSECT       8   /* PCI pruning and/or empty GPU/CPU/NIC intersection (Matcher.py:295-359) */
+#define NHD_WHY_COUNT           9
+#define NHD_WHY_NONE            0xFF /* nhd_explain_pod: the pod's status is not NHD_NO_CANDIDATE            */
+
 /* CfgTopology.TopologyMapType values (CfgTopology.py:41-45) */
 #define NHD_MAP_INVALID         0
 #define NHD_MAP_NUMA            1
@@ -250,6 +264,24 @@ int32_t nhd_sync(nhd_handle* h);
 int32_t nhd_run_filter_only(nhd_handle* h);
 
 int32_t nhd_last_timing(const nhd_handle* h, nhd_timing* out);
+
+/*
+ * Why the pods of the last solved batch that got NHD_NO_CANDIDATE found no node.  For such a pod i every loaded
+ * node n gets a reason NHD_WHY_*: the first stage of the reference that drops n, on the cluster as pod i saw it —
+ * the batch-start records plus what pods 0..i-1 of the batch did (cores, GPUs, NICs, hugepages and the busy stamp
+ * now[j] of a placement; the busy stamp of a failed assignment), at clock now[i].
+ *   nhd_explain_batch  counts[i * NHD_WHY_COUNT + r] = nodes with reason r for pod i; a NO_CANDIDATE row sums to
+ *                      n_nodes, every other row is zero.  counts holds n_pods * NHD_WHY_COUNT entries.
+ *   nhd_explain_pod    node_reason[n] for one pod (n_nodes bytes); NHD_WHY_NONE everywhere when the pod's status
+ *                      is not NHD_NO_CANDIDATE.
+ * The batch-start state is read from the handle's snapshot, so both need the sequence
+ *     nhd_snapshot -> nhd_stage_batch -> nhd_solve_staged (or nhd_solve_batch)
+ * with nothing else changing the mirror in between or since (no load / update / restore / other stage or solve);
+ * otherwise they return NHD_ERR_STATE.  Neither changes the mirror, the bindings or the filter bitmaps, and neither
+ * enters a collective (every rank holds all records).  They wait for the device before returning.
+ */
+int32_t nhd_explain_batch(nhd_handle* h, uint32_t* counts);
+int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_reason);
 
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */

@@ -192,6 +192,13 @@ class DeviceCluster:
         self._last = (pods, np.full(len(tops), now, dtype='<f8'))
         return self._solver.solve_batch(*self._last)
 
+    def explain(self):
+        """Per-reason node counts ((pods, wire.WHY_COUNT) array) of the NO_CANDIDATE pods of the last ``solve``,
+        each at the state that pod saw; valid right after ``solve`` (before any ``rewind``).  None when the solver
+        in use cannot explain (a stand-in without ``explain_batch``)."""
+        fn = getattr(self._solver, 'explain_batch', None)
+        return fn() if fn is not None else None
+
     def rewind(self, k: int):
         """Put the device back to the state right after pod ``k`` of the last batch (restore the
         snapshot taken before it, solve pods ``0..k`` again: the solver is deterministic)."""
@@ -240,6 +247,9 @@ class NHDScheduler:
         self.pods_solved = 0
         self.assign_failed_nodes = set()
         self.unsupported_pods = []                   # (ns, pod, why): requests beyond the packed layout's limits
+        # (ns, pod) -> {reason name: nodes}: why the pod's last attempt found no node (NHD_WHY_*, wire.WHY_NAMES),
+        # until the pod is scheduled or deleted
+        self.unschedulable_reasons: Dict[tuple, Dict[str, int]] = {}
         self.stats_from_device = stats_from_device
 
     # ---- small helpers --------------------------------------------------------------------
@@ -476,7 +486,7 @@ class NHDScheduler:
                     self._prepare(e)
             now = float(self._clock())
             solvable = [e for e in run if e.top is not None and e.unsupported is None]
-            bindings = {}
+            bindings, why = {}, None
             if solvable and self.nodes:
                 self.cluster.sync(self.nodes, self._dirty)
                 self._dirty.clear()
@@ -495,9 +505,15 @@ class NHDScheduler:
                         solvable.pop(int(m.group(1))).unsupported = str(err)
                 self.pods_solved += len(solvable)
                 bindings = {e.pos: out[i] for i, e in enumerate(solvable)}
+                # why the NO_CANDIDATE pods found no node: read before a rewind replaces the solved batch
+                why = self.cluster.explain() if any(int(b['status']) == wire.NO_CANDIDATE for b in out) else None
+                if why is not None:
+                    why = {e.pos: why[i] for i, e in enumerate(solvable)}
             cut = None
             for e in run:
                 b = bindings.get(e.pos)
+                if b is not None and int(b['status']) == wire.NO_CANDIDATE and why is not None:
+                    self._explain(e, why[e.pos])
                 rewound = False
                 if b is not None and int(b['status']) in (wire.ASSIGN_FAILED, wire.REF_WOULD_CRASH):
                     # what a failed assignment leaves on its node is read back from the solver (see _finish);
@@ -519,9 +535,19 @@ class NHDScheduler:
             pos = cut.pos + 1
         return results
 
+    def _explain(self, e: _Pending, counts):
+        """Remember and log why pod ``e`` found no node: per reason, the nodes whose first failing stage it was."""
+        ns, podname = e.key[0], e.key[1]
+        reasons = {name: int(c) for name, c in zip(wire.WHY_NAMES, counts) if int(c)}
+        self.unschedulable_reasons[(ns, podname)] = reasons
+        total = int(sum(int(c) for c in counts))
+        detail = ', '.join(f'{c} {name}' for name, c in sorted(reasons.items(), key=lambda kv: -kv[1]))
+        self._info(f'Pod {ns}.{podname}: 0/{total} nodes are available: {detail}')
+
     def _record(self, key, ok: bool):                 # the two branches of CheckPendingPods (:431-436)
         podkey = (key[0], key[1])
         if ok:
+            self.unschedulable_reasons.pop(podkey, None)
             self.pod_state[podkey] = {'state': PodStatus.POD_STATUS_SCHEDULED, 'time': self._wall(), 'uid': key[2]}
         else:
             self._error(f'Failed scheduling pod {key[0]}.{key[1]} [{key[2]}]')
@@ -595,6 +621,7 @@ class NHDScheduler:
             if t == 'NHD_WATCH_TYPE_TRIAD_POD_DELETE':
                 self.ReleasePodResources(pn, ns)
                 self.pod_state.pop((ns, pn), None)
+                self.unschedulable_reasons.pop((ns, pn), None)
             else:
                 if ((ns, pn) in self.pod_state) and \
                         (self.pod_state[(ns, pn)]['state'] == PodStatus.POD_STATUS_SCHEDULED):

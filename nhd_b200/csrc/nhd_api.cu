@@ -117,6 +117,18 @@ struct nhd_handle {
     uint64_t* d_pod_groups = nullptr; size_t pod_groups_cap = 0;
     std::vector<int32_t> pod_type_host;
 
+    /* Generation of the device mirror: every call that changes it (or the staged batch) takes a new value.  The
+     * explanations need the snapshot to be the batch's starting state and the mirror to hold exactly that batch's
+     * commit, i.e. snapshot, stage and solve as three consecutive generations. */
+    uint64_t gen = 1, snap_gen = 0, stage_gen = 0, explain_gen = 0;
+    bool batch_on_snapshot = false;
+    /* explanation scratch: per-node placement lists (CSR), the failed pods, per-pod counts, one pod's node reasons */
+    int32_t* d_xnode = nullptr;   size_t xnode_cap = 0;      /* node_cnt | node_start | cursor */
+    int32_t* d_xpod = nullptr;    size_t xpod_cap = 0;       /* node_pods | failed */
+    uint32_t* d_xcounts = nullptr; size_t xcounts_cap = 0;
+    uint8_t* d_xreasons = nullptr; size_t xreasons_cap = 0;
+    uint32_t* d_xsmall = nullptr;                             /* n_failed, survivors */
+
     nhd_timing timing;
     std::string err;
 };
@@ -301,6 +313,7 @@ extern "C" int32_t nhd_destroy(nhd_handle* h)
     cudaFree(h->d_prof);
 #endif
     cudaFree(h->d_pend); cudaFree(h->d_vresult); cudaFree(h->d_pod_groups);
+    cudaFree(h->d_xnode); cudaFree(h->d_xpod); cudaFree(h->d_xcounts); cudaFree(h->d_xreasons); cudaFree(h->d_xsmall);
     if (h->h_stage) cudaFreeHost(h->h_stage);
     if (h->h_batch) cudaFreeHost(h->h_batch);
     if (h->h_out) cudaFreeHost(h->h_out);
@@ -449,6 +462,7 @@ static int32_t upload_records(nhd_handle* h, int n, const nhd_node_rec* recs, co
 extern "C" int32_t nhd_load_nodes(nhd_handle* h, int32_t n_nodes, const nhd_node_rec* recs)
 {
     if (!h || n_nodes < 0 || (n_nodes > 0 && !recs)) return NHD_ERR_INVALID;
+    h->gen++;
     CK(cudaSetDevice(h->params.device));
     const int n_super = std::max(1, (n_nodes + SUPER_NODES - 1) / SUPER_NODES);
     const size_t bytes = (size_t)n_super * SUPER_BYTES;
@@ -499,6 +513,7 @@ extern "C" int32_t nhd_update_nodes(nhd_handle* h, int32_t n, const int32_t* idx
         }
     }
     if (n == 0) return NHD_OK;
+    h->gen++;
     int mx = 1;
     const int32_t rc = upload_records(h, n, recs, idx, &mx);
     if (rc == NHD_OK) track_numa(h, n, recs, idx);
@@ -527,15 +542,18 @@ extern "C" int32_t nhd_snapshot(nhd_handle* h)
 {
     if (!h || !h->loaded) return NHD_ERR_STATE;
     CK(cudaSetDevice(h->params.device));
+    h->gen++;
     CK(cudaMemcpyAsync(h->d_snapshot, h->d_nodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     h->have_snapshot = true;
+    h->snap_gen = h->gen;
     return NHD_OK;
 }
 
 extern "C" int32_t nhd_restore(nhd_handle* h)
 {
     if (!h || !h->loaded || !h->have_snapshot) return NHD_ERR_STATE;
+    h->gen++;
     CK(cudaSetDevice(h->params.device));
     CK(cudaMemcpyAsync(h->d_nodes, h->d_snapshot, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
     return NHD_OK;
@@ -582,6 +600,8 @@ extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod*
 {
     if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now))) return NHD_ERR_INVALID;
     if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_stage_batch before nhd_load_nodes");
+    const bool on_snapshot = h->gen == h->snap_gen;
+    h->gen++;
     CK(cudaSetDevice(h->params.device));
     h->staged = h->solved = false;
 
@@ -680,6 +700,8 @@ extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod*
     h->const_clock = true;
     for (int i = 1; i < n_pods; i++) if (now[i] != now[0]) { h->const_clock = false; break; }
     h->staged = true;
+    h->batch_on_snapshot = on_snapshot;
+    h->stage_gen = h->gen;
     return NHD_OK;
 }
 
@@ -696,6 +718,9 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
 {
     if (!h) return NHD_ERR_INVALID;
     if (!h->staged) return fail(h, NHD_ERR_STATE, "nhd_solve_staged without a staged batch");
+    const bool explainable = !filter_only && h->batch_on_snapshot && h->gen == h->stage_gen;
+    h->gen++;
+    h->explain_gen = explainable ? h->gen : 0;
     CK(cudaSetDevice(h->params.device));
     const int T = h->n_types, W = h->words;
     int launches = 0;
@@ -887,6 +912,127 @@ extern "C" int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* wor
         memcpy(pod_type, h->pod_type_host.data(), (size_t)h->n_pods * 4);
     }
     return NHD_OK;
+}
+
+/* ------------------------------------------------------------------ explanations */
+
+static int32_t explain_ready(nhd_handle* h)
+{
+    if (!h->solved || h->explain_gen == 0 || h->gen != h->explain_gen)
+        return fail(h, NHD_ERR_STATE, "explanations need nhd_snapshot -> nhd_stage_batch -> solve, with nothing changing "
+                                      "the device mirror in between or since");
+    return NHD_OK;
+}
+
+/* The pods bound to each node, in pod order (CSR over the batch's bindings), and the list of NO_CANDIDATE pods.
+ * Returns the number of NO_CANDIDATE pods in *n_failed. */
+static int32_t explain_prepare(nhd_handle* h, int* n_failed)
+{
+    const int N = h->n_nodes, P = h->n_pods;
+    CK(grow_dev(h->d_xnode, h->xnode_cap, ((size_t)3 * N + 2) * 4));
+    CK(grow_dev(h->d_xpod, h->xpod_cap, ((size_t)2 * P + 1) * 4));
+    if (!h->d_xsmall) CK(cudaMalloc((void**)&h->d_xsmall, 16));
+    int32_t* node_cnt = h->d_xnode;
+    int32_t* node_start = h->d_xnode + N;            /* N + 1 entries */
+    int32_t* cursor = h->d_xnode + 2 * N + 1;
+    int32_t* node_pods = h->d_xpod;
+    int32_t* failed = h->d_xpod + P;
+    CK(cudaMemsetAsync(node_cnt, 0, (size_t)N * 4, h->stream));
+    CK(cudaMemsetAsync(h->d_xsmall, 0, 16, h->stream));
+    const int threads = 256;
+    if (P > 0) {
+        explain_count_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(h->d_out, P, node_cnt, failed,
+                                                                                     (int32_t*)h->d_xsmall);
+        CK(cudaGetLastError());
+    }
+    explain_scan_kernel<<<1, EXPLAIN_SCAN_THREADS, 0, h->stream>>>(node_cnt, N, node_start, cursor);
+    CK(cudaGetLastError());
+    if (P > 0) {
+        explain_fill_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(h->d_out, P, cursor, node_pods);
+        CK(cudaGetLastError());
+    }
+    if (N > 0) {
+        explain_sort_kernel<<<(N + threads - 1) / threads, threads, 0, h->stream>>>(node_start, N, node_pods);
+        CK(cudaGetLastError());
+    }
+    int32_t nf = 0;
+    CK(cudaMemcpyAsync(&nf, h->d_xsmall, 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    *n_failed = nf;
+    return NHD_OK;
+}
+
+/* one (failed pod x node) pass; counts and/or reasons may be null */
+static int32_t explain_launch(nhd_handle* h, int n_failed, uint32_t* d_counts, uint8_t* d_reasons)
+{
+    const int N = h->n_nodes, P = h->n_pods;
+    if (n_failed == 0 || N == 0) return NHD_OK;
+    ExplainArgs xa;
+    xa.snapshot = h->d_snapshot; xa.types = h->d_types; xa.pod_type = h->d_pod_type; xa.now = h->d_now; xa.out = h->d_out;
+    xa.pod_groups = h->n_names ? h->d_pod_groups : nullptr;
+    xa.node_start = h->d_xnode + N; xa.node_pods = h->d_xpod; xa.failed = h->d_xpod + P;
+    xa.n_failed = (const int32_t*)h->d_xsmall;
+    xa.n_nodes = N; xa.min_busy = h->params.min_busy_secs;
+    memcpy(xa.cap, h->cap, sizeof(xa.cap));
+    xa.counts = d_counts; xa.reasons = d_reasons; xa.survivors = h->d_xsmall + 1;
+    const dim3 grid((unsigned)((N + EXPLAIN_THREADS - 1) / EXPLAIN_THREADS), (unsigned)std::min(n_failed, 65535));
+    explain_kernel<<<grid, EXPLAIN_THREADS, 0, h->stream>>>(xa);
+    CK(cudaGetLastError());
+    return NHD_OK;
+}
+
+/* every NO_CANDIDATE pod's nodes must all be dropped by some stage: a node passing them all means the state was
+ * not rebuilt as the pod saw it */
+static int32_t explain_survivors(nhd_handle* h, const char* what)
+{
+    uint32_t surv = 0;
+    CK(cudaMemcpyAsync(&surv, h->d_xsmall + 1, 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (surv) return fail(h, NHD_ERR_STATE, "%s: %u (pod, node) pairs of NO_CANDIDATE pods pass every stage", what, surv);
+    return NHD_OK;
+}
+
+extern "C" int32_t nhd_explain_batch(nhd_handle* h, uint32_t* counts)
+{
+    if (!h || (h->n_pods > 0 && !counts)) return NHD_ERR_INVALID;
+    int32_t rc = explain_ready(h);
+    if (rc != NHD_OK) return rc;
+    CK(cudaSetDevice(h->params.device));
+    const size_t bytes = (size_t)h->n_pods * NHD_WHY_COUNT * 4;
+    if (bytes == 0) return NHD_OK;
+    int nf = 0;
+    if ((rc = explain_prepare(h, &nf)) != NHD_OK) return rc;
+    CK(grow_dev(h->d_xcounts, h->xcounts_cap, bytes));
+    CK(cudaMemsetAsync(h->d_xcounts, 0, bytes, h->stream));
+    if ((rc = explain_launch(h, nf, h->d_xcounts, nullptr)) != NHD_OK) return rc;
+    CK(cudaMemcpyAsync(counts, h->d_xcounts, bytes, cudaMemcpyDeviceToHost, h->stream));
+    return explain_survivors(h, "nhd_explain_batch");
+}
+
+extern "C" int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_reason)
+{
+    if (!h || (h->n_nodes > 0 && !node_reason)) return NHD_ERR_INVALID;
+    int32_t rc = explain_ready(h);
+    if (rc != NHD_OK) return rc;
+    if (pod < 0 || pod >= h->n_pods) return fail(h, NHD_ERR_INVALID, "pod %d outside the batch of %d", pod, h->n_pods);
+    CK(cudaSetDevice(h->params.device));
+    int32_t status = 0;
+    CK(cudaMemcpyAsync(&status, &h->d_out[pod].status, 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (status != NHD_NO_CANDIDATE) {
+        memset(node_reason, NHD_WHY_NONE, (size_t)h->n_nodes);
+        return NHD_OK;
+    }
+    int nf = 0;
+    if ((rc = explain_prepare(h, &nf)) != NHD_OK) return rc;
+    const int32_t one[1] = {pod};                    /* explain just this pod: failed[0] = pod, n_failed = 1 */
+    const int32_t n1 = 1;
+    CK(cudaMemcpyAsync(h->d_xpod + h->n_pods, one, 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_xsmall, &n1, 4, cudaMemcpyHostToDevice, h->stream));
+    CK(grow_dev(h->d_xreasons, h->xreasons_cap, (size_t)h->n_nodes));
+    if ((rc = explain_launch(h, 1, nullptr, h->d_xreasons)) != NHD_OK) return rc;
+    CK(cudaMemcpyAsync(node_reason, h->d_xreasons, (size_t)h->n_nodes, cudaMemcpyDeviceToHost, h->stream));
+    return explain_survivors(h, "nhd_explain_pod");
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

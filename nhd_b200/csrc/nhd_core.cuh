@@ -1231,4 +1231,124 @@ NHD_HDN M256 assign_cores_from_snapshot(const nhd_node_rec& snap, const PodType&
     return m_andnot(rec_used(r), before);
 }
 
+/* ================================================================================== */
+/* Explanations: why a NO_CANDIDATE pod found no node                                  */
+/* ================================================================================== */
+
+/*
+ * One binding of the batch folded into its node's record, as the reference leaves the node after that pod
+ * (NHDScheduler.py:289-304): a placed pod's cores, GPUs, claimed NICs and hugepages, and for every pod that
+ * reached the node — placed or not — the busy stamp.  A failed assignment unwinds everything else (Node.py:825-837;
+ * its only raise points come before the hugepage decrement, see assign_resources).  Plain stores: the caller owns r.
+ */
+NHD_HD void apply_binding(nhd_node_rec& r, const nhd_binding& b, int32_t hugepages_gb, double now)
+{
+    if (b.status == NHD_PLACED) {
+        for (int k = 0; k < b.n_cores && k < NHD_MAX_POD_CORES; k++) mark_used(r, b.cores[k]);
+        for (int k = 0; k < b.n_gpus && k < NHD_MAX_POD_GPUS; k++) r.gpu_used |= (uint16_t)(1u << b.gpu_index[k]);
+        for (int k = 0; k < b.n_claimed && k < NHD_MAX_GROUPS; k++) r.nic_inuse |= 1u << b.claimed_nics[k];
+        if (hugepages_gb > 0) r.free_hugepages_gb -= hugepages_gb;
+    }
+    r.busy_time = now;
+}
+
+/*
+ * nic_first_fit as an existence test with the PCI pruning as a parameter: FilterNumaTopology's NIC stage keeps
+ * its entries before the pruning (Matcher.py:224-276), IntersectResources prunes them (:295-335).  Same search,
+ * same fp64 subtraction order; kept separate so that the solver's own NIC search is not touched.
+ */
+NHD_HD bool nic_entry_exists(const nhd_node_rec& r, const PodType& t, const uint8_t* p, int K, const double* cap,
+                             uint64_t gsw, bool pci)
+{
+    const int G = t.G;
+    int ord[NHD_MAX_GROUPS];
+    int n = 0;
+    for (int k = 0; k < K; k++)
+        for (int g = 0; g < G; g++)
+            if (p[g] == k) {
+                if (r.nic_numa_mask[k] == 0) return false;
+                ord[n++] = g;
+            }
+    int choice[NHD_MAX_GROUPS], li[NHD_MAX_GROUPS];
+    double rrx[NHD_MAX_GROUPS], rtx[NHD_MAX_GROUPS];
+    int d = 0;
+    choice[0] = 0;
+    for (;;) {
+        const int g = ord[d];
+        const int l = nth_bit32(r.nic_numa_mask[p[g]], choice[d]);
+        if (l < 0) {
+            if (d == 0) return false;
+            d--;
+            choice[d]++;
+            continue;
+        }
+        double rx = nic_free_bw(r, l, cap), tx = rx;
+        for (int e = d - 1; e >= 0; e--)
+            if (li[e] == l) { rx = rrx[e]; tx = rtx[e]; break; }
+        rx -= t.pod.groups[g].rx_gbps;
+        tx -= t.pod.groups[g].tx_gbps;
+        bool ok = !(rx < 0) && !(tx < 0);
+        if (ok && pci) {
+            const int s = nic_switch(r, l);
+            int cnt = 1;
+            for (int e = 0; e < d; e++) cnt += (nic_switch(r, li[e]) == s);
+            ok = cnt <= (int)((gsw >> (4 * s)) & 0xF);
+        }
+        if (!ok) { choice[d]++; continue; }
+        li[d] = l; rrx[d] = rx; rtx[d] = tx;
+        if (d == G - 1) return true;
+        d++;
+        choice[d] = 0;
+    }
+}
+
+/*
+ * The first stage of the reference that drops node r for pod type t (NHD_WHY_*), or NHD_WHY_COUNT when r passes
+ * them all.  pod_groups is the pod's own node-group list (the batch's pod types drop it when a batch mixes lists).
+ *   InitialNodeFilter (NHDScheduler.py:240-241), FilterPodResources (Matcher.py:73,78), the three stages of
+ *   FilterNumaTopology (:107-111 busy, :118-132 GPU, :203-214 CPU, :242-270 NIC over every NUMA tuple), and
+ *   IntersectResources (:295-359): the NUMA tuples passing all three stages, the NIC stage after the PCI pruning.
+ * Only whether a stage leaves something matters, so each stage stops at its first surviving tuple.
+ */
+NHD_HDN int explain_node(const nhd_node_rec& r, const PodType& t, uint64_t pod_groups, double now, double min_busy,
+                         const double* cap)
+{
+    if ((r.group_mask & pod_groups) == 0) return NHD_WHY_GROUP;
+    if (!(r.flags & NHD_NODE_ACTIVE)) return NHD_WHY_INACTIVE;
+    if (r.flags & NHD_NODE_MAINTENANCE) return NHD_WHY_MAINTENANCE;
+    if (t.pod.hugepages_gb > r.free_hugepages_gb) return NHD_WHY_HUGEPAGES;
+    if (t.needs_gpu && node_busy(r, now, min_busy)) return NHD_WHY_BUSY;
+    const int K = r.n_numa, G = t.G;
+    const int np = ipow(K, G);                              /* <= 64: checked when the batch was staged */
+    int fg[NHD_MAX_NUMA], fc[NHD_MAX_NUMA];
+    free_gpus(r, fg);
+    free_cores(r, fc);
+    const bool smt = rec_smt(r);
+    uint8_t p[NHD_MAX_GROUPS];
+    uint64_t ma = 0, mb = 0;
+    for (int pi = 0; pi < np; pi++) {
+        tuple_digits(pi, K, G, p);
+        if (gpu_ok(t, p, K, fg)) ma |= 1ULL << pi;
+    }
+    if (!ma) return NHD_WHY_GPU;
+    for (int pi = 0; pi < np; pi++) {
+        tuple_digits(pi, K, G, p);
+        for (int m = 0; m < K; m++)
+            if (cpu_ok(t, p, m, K, fc, smt)) { mb |= 1ULL << pi; break; }
+    }
+    if (!mb) return NHD_WHY_CPU;
+    bool nic = false;
+    for (int pi = 0; pi < np && !nic; pi++) {
+        tuple_digits(pi, K, G, p);
+        nic = nic_entry_exists(r, t, p, K, cap, 0, false);
+    }
+    if (!nic) return NHD_WHY_NIC;
+    const uint64_t gsw = t.pci ? free_gpus_per_switch(r) : 0;
+    for (uint64_t both = ma & mb; both; both &= both - 1) {
+        tuple_digits(ctz64(both), K, G, p);
+        if (nic_entry_exists(r, t, p, K, cap, gsw, t.pci != 0)) return NHD_WHY_COUNT;
+    }
+    return NHD_WHY_INTERSECT;
+}
+
 } // namespace nhd

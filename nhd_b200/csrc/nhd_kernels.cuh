@@ -2491,4 +2491,131 @@ __global__ void commit_kernel(const FinishArgs a)
     *reinterpret_cast<double*>(a.nodes + chunk_off(node, 3)) = d.busy_time;
 }
 
+/* ------------------------------------------------------------------ explanations (nhd_explain_batch / _pod) */
+
+/*
+ * Not part of a solve: these run only when a caller asks why pods found no node, after the batch is done.
+ * The state pod i saw on node n is the snapshot record of n plus the bindings of the pods j < i bound to n, so the
+ * batch's bindings are first sorted by node (a counting sort, pod order kept inside a node).  Then one thread per
+ * (failed pod, node) rebuilds that record and reports the first stage that drops the node.
+ */
+
+/* per pod: count it on its node, and list the NO_CANDIDATE pods (in any order: each gets its own row) */
+__global__ void explain_count_kernel(const nhd_binding* __restrict__ out, int n_pods, int32_t* node_cnt,
+                                     int32_t* failed, int32_t* n_failed)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_pods) return;
+    const int node = out[i].node, st = out[i].status;
+    if (node >= 0) atomicAdd(&node_cnt[node], 1);
+    if (st == NHD_NO_CANDIDATE) failed[atomicAdd(n_failed, 1)] = i;
+}
+
+/* exclusive prefix sum of node_cnt[0..n) into start[0..n] (start[n] = total) and cursor[0..n); one CTA */
+constexpr int EXPLAIN_SCAN_THREADS = 1024;
+__global__ void __launch_bounds__(EXPLAIN_SCAN_THREADS) explain_scan_kernel(const int32_t* __restrict__ node_cnt, int n,
+                                                                             int32_t* start, int32_t* cursor)
+{
+    __shared__ int32_t part[EXPLAIN_SCAN_THREADS];
+    const int tid = threadIdx.x;
+    const int per = (n + EXPLAIN_SCAN_THREADS - 1) / EXPLAIN_SCAN_THREADS;
+    const int lo = tid * per < n ? tid * per : n, hi = lo + per < n ? lo + per : n;
+    int32_t s = 0;
+    for (int k = lo; k < hi; k++) s += node_cnt[k];
+    part[tid] = s;
+    __syncthreads();
+    for (int off = 1; off < EXPLAIN_SCAN_THREADS; off <<= 1) {      /* inclusive scan of the chunk sums */
+        const int32_t v = tid >= off ? part[tid - off] : 0;
+        __syncthreads();
+        part[tid] += v;
+        __syncthreads();
+    }
+    int32_t run = part[tid] - s;
+    for (int k = lo; k < hi; k++) { start[k] = run; cursor[k] = run; run += node_cnt[k]; }
+    if (tid == EXPLAIN_SCAN_THREADS - 1) start[n] = part[tid];
+}
+
+__global__ void explain_fill_kernel(const nhd_binding* __restrict__ out, int n_pods, int32_t* cursor, int32_t* node_pods)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_pods) return;
+    const int node = out[i].node;
+    if (node >= 0) node_pods[atomicAdd(&cursor[node], 1)] = i;
+}
+
+/* pod order inside each node's list (the lists are short: the pods one batch bound to one node) */
+__global__ void explain_sort_kernel(const int32_t* __restrict__ start, int n, int32_t* node_pods)
+{
+    const int node = blockIdx.x * blockDim.x + threadIdx.x;
+    if (node >= n) return;
+    const int lo = start[node], hi = start[node + 1];
+    for (int k = lo + 1; k < hi; k++) {
+        const int32_t v = node_pods[k];
+        int q = k - 1;
+        for (; q >= lo && node_pods[q] > v; q--) node_pods[q + 1] = node_pods[q];
+        node_pods[q + 1] = v;
+    }
+}
+
+struct ExplainArgs {
+    const uint8_t* snapshot;       /* batch-start records (tiled layout) */
+    const PodType* types;
+    const int32_t* pod_type;
+    const double* now;
+    const nhd_binding* out;
+    const uint64_t* pod_groups;    /* per-pod node-group lists of a batch that mixes them, else null */
+    const int32_t* node_start;     /* pods bound to node n: node_pods[node_start[n] .. node_start[n + 1]), in pod order */
+    const int32_t* node_pods;
+    const int32_t* failed;         /* the pods to explain */
+    const int32_t* n_failed;
+    int n_nodes;
+    double min_busy;
+    double cap[NHD_MAX_SPEED_CLASSES];
+    uint32_t* counts;              /* [pod][NHD_WHY_COUNT], or null */
+    uint8_t* reasons;              /* [node] of the single pod failed[0], or null */
+    uint32_t* survivors;           /* (pod, node) pairs that pass every stage: a NO_CANDIDATE pod has none */
+};
+
+constexpr int EXPLAIN_THREADS = 256;
+
+/* grid: x over nodes, y over failed pods (strided).  Warp ballots count each reason: one atomic per warp and reason. */
+__global__ void __launch_bounds__(EXPLAIN_THREADS) explain_kernel(const __grid_constant__ ExplainArgs a)
+{
+    __shared__ PodType st;
+    __shared__ double scap[NHD_MAX_SPEED_CLASSES];
+    const int tid = threadIdx.x, lane = tid & 31;
+    const int n = blockIdx.x * EXPLAIN_THREADS + tid;
+    if (tid < NHD_MAX_SPEED_CLASSES) scap[tid] = a.cap[tid];
+    const int nf = *a.n_failed;
+    for (int f = blockIdx.y; f < nf; f += gridDim.y) {
+        const int i = a.failed[f];
+        const PodType* gt = &a.types[a.pod_type[i]];
+        __syncthreads();                                             /* the previous pod's type is no longer read */
+        for (int w = tid; w < (int)(sizeof(PodType) / 4); w += EXPLAIN_THREADS)
+            reinterpret_cast<uint32_t*>(&st)[w] = reinterpret_cast<const uint32_t*>(gt)[w];
+        __syncthreads();
+        int reason = -1;
+        if (n < a.n_nodes) {
+            RecU u;
+            load_rec(a.snapshot, n, u);
+            const int hi = a.node_start[n + 1];
+            for (int k = a.node_start[n]; k < hi; k++) {
+                const int j = a.node_pods[k];
+                if (j >= i) break;
+                apply_binding(u.r, a.out[j], a.types[a.pod_type[j]].pod.hugepages_gb, a.now[j]);
+            }
+            const uint64_t groups = a.pod_groups ? a.pod_groups[i] : st.pod.group_mask;
+            reason = explain_node(u.r, st, groups, a.now[i], a.min_busy, scap);
+            if (a.reasons) a.reasons[n] = (uint8_t)reason;
+        }
+        for (int r = 0; r <= NHD_WHY_COUNT; r++) {
+            const unsigned m = __ballot_sync(0xFFFFFFFFu, reason == r);
+            if (lane == 0 && m) {
+                if (r == NHD_WHY_COUNT) atomicAdd(a.survivors, (uint32_t)__popc(m));
+                else if (a.counts) atomicAdd(&a.counts[(size_t)i * NHD_WHY_COUNT + r], (uint32_t)__popc(m));
+            }
+        }
+    }
+}
+
 } // namespace nhd

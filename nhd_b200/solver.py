@@ -167,6 +167,22 @@ class Solver:
         self._ck(self._L.nhd_debug_counters(self._h, out.ctypes.data))
         return out
 
+    # ---- explanations ---------------------------------------------------------------
+    def explain_batch(self):
+        """(n_pods, WHY_COUNT) uint32: for every NO_CANDIDATE pod of the last solved batch, how many nodes each
+        reference stage (``wire.WHY_NAMES``, first stage that drops the node) ruled out, at the state that pod saw;
+        zero rows for the other pods.  Needs ``snapshot()`` right before the batch was staged."""
+        out = np.zeros((self.n_pods, wire.WHY_COUNT), dtype='<u4')
+        self._ck(self._L.nhd_explain_batch(self._h, out.ctypes.data))
+        return out
+
+    def explain_pod(self, i):
+        """(n_nodes,) uint8: the reason code of every node for pod ``i`` of the last solved batch
+        (``wire.WHY_NONE`` everywhere when that pod is not NO_CANDIDATE)."""
+        out = np.zeros(self.n_nodes, dtype=np.uint8)
+        self._ck(self._L.nhd_explain_pod(self._h, int(i), out.ctypes.data))
+        return out
+
     def filter_bitmaps(self):
         """Runs only the snapshot predicate kernel on the staged batch; returns
         (feas[type, node] bool, nogpu[node], busy[node], pod_type[pod])."""

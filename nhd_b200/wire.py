@@ -22,6 +22,12 @@ PLACED, NO_CANDIDATE, ASSIGN_FAILED, REF_WOULD_CRASH, BAD_MAP_TYPE = 0, 1, 2, 3,
 STATUS_NAMES = {PLACED: 'placed', NO_CANDIDATE: 'none', ASSIGN_FAILED: 'assign_failed',
                 REF_WOULD_CRASH: 'ref_would_crash', BAD_MAP_TYPE: 'bad_map_type'}
 
+# why a node could not take a NO_CANDIDATE pod (NHD_WHY_*): the first reference stage that drops it
+WHY_GROUP, WHY_INACTIVE, WHY_MAINTENANCE, WHY_HUGEPAGES, WHY_BUSY, WHY_GPU, WHY_CPU, WHY_NIC, WHY_INTERSECT = range(9)
+WHY_COUNT = 9
+WHY_NONE = 0xFF
+WHY_NAMES = ('group', 'inactive', 'maintenance', 'hugepages', 'busy', 'gpu', 'cpu', 'nic', 'intersect')
+
 MAP_INVALID, MAP_NUMA, MAP_PCI, MAP_NONE = 0, 1, 2, 3
 NODE_SMT, NODE_ACTIVE, NODE_MAINTENANCE = 1, 2, 4
 GRP_PROC_SMT, GRP_HELPER_SMT, GRP_HAS_NIC_CORES = 1, 2, 4
