@@ -283,6 +283,25 @@ int32_t nhd_last_timing(const nhd_handle* h, nhd_timing* out);
 int32_t nhd_explain_batch(nhd_handle* h, uint32_t* counts);
 int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_reason);
 
+/*
+ * Where each pod would go on its own, without placing anything: the reference's Matcher.FindNode (Matcher.py:27-63),
+ * which has no side effects, plus what SetPhysicalIdsFromMapping would take on that node.
+ *   NHD_QUERY_MIRROR    the records as they are now
+ *   NHD_QUERY_SNAPSHOT  the records of the last nhd_snapshot
+ * out[i] is byte for byte the binding nhd_solve_batch(h, 1, &pods[i], &now[i], ...) would return on the chosen
+ * records: status, node, mapping, core ids, GPU indices, NIC indices and claim order of pod i ALONE.  Pods do not
+ * see each other.  Nothing is written: not the mirror, the snapshot, the staged batch or its bindings, the filter
+ * bitmaps or the explanation state; nhd_explain_* and nhd_fetch_bindings of the last batch stay valid across a
+ * query.  NHD_QUERY_SNAPSHOT needs a snapshot with no nhd_load_nodes / nhd_update_nodes since it (solves, stages and
+ * restores are fine), otherwise NHD_ERR_STATE.  Pods are validated as by nhd_stage_batch (NHD_ERR_INVALID /
+ * NHD_ERR_UNSUPPORTED naming the pod index, tuple limits included).  No collective: every rank holds all records and
+ * may call alone.  Waits for the device before returning.
+ */
+#define NHD_QUERY_MIRROR        0
+#define NHD_QUERY_SNAPSHOT      1
+int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods, const nhd_pod* pods,
+                        const double* now, nhd_binding* out);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

@@ -218,6 +218,36 @@ class Matcher:
         mapping['_nhd_binding'] = b
         return names[int(b['node'])], mapping
 
+    def FindNodes(self, nl, tops: Sequence, pod_groups: Sequence[Iterable[str]] = None, now=None):
+        """Per pod, what ``FindNode(nl, top)`` would return for that pod ALONE: ``(nodename, mapping)`` or ``(None,)``
+        (``mapping`` again carries the device binding under ``'_nhd_binding'``).  One GPU query for all pods; the pods
+        do not see each other and nothing is committed: the device records, the ``Node`` objects and the nodes the
+        next call re-sends stay as they are.  ``pod_groups``: one group list per pod, or None when ``nl`` is already
+        narrowed by ``InitialNodeFilter`` (as for ``FindNode``).  ``now``: one clock for all pods or one per pod."""
+        n = len(tops)
+        if n == 0:
+            return []
+        if len(nl) == 0:
+            return [(None,)] * n
+        names, nodes, solver = self._load(nl)
+        pods = np.zeros(n, dtype=wire.POD_DTYPE)
+        for i, top in enumerate(tops):
+            packing.pack_pod(top, [], self._layout, out=pods[i])
+            pods[i]['group_mask'] = np.uint64(0xFFFFFFFFFFFFFFFF) if pod_groups is None else \
+                self._layout.groups_mask(pod_groups[i], create=False)
+        if now is None:
+            now = time.monotonic()
+        nows = np.full(n, now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
+        results = []
+        for b in solver.query_batch(pods, nows):
+            if int(b['node']) < 0:
+                results.append((None,))
+                continue
+            mapping = packing.binding_to_mapping(b)
+            mapping['_nhd_binding'] = b
+            results.append((names[int(b['node'])], mapping))
+        return results
+
     def FindNodesBatch(self, nl, tops: Sequence, pod_groups: Sequence[Iterable[str]] = None,
                        now=None, apply: bool = True):
         """Schedule ``tops`` in order on ``nl`` (all nodes of the cluster, NOT pre-filtered:

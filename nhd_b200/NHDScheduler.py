@@ -176,10 +176,7 @@ class DeviceCluster:
             self._solver.update_nodes(idx, recs)
             self.delta_nodes += len(idx)
 
-    def solve(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now: float, packed: Sequence = None):
-        """Bindings of ``tops`` scheduled in order on the synced cluster (one GPU call).  ``packed``: records
-        ``pack_pod`` already made of them; only the node-group mask is worked out again (``sync`` may have met new
-        group names since)."""
+    def _pods(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], packed: Sequence = None) -> np.ndarray:
         pods = np.zeros(len(tops), dtype=wire.POD_DTYPE)
         for i, top in enumerate(tops):
             if packed is not None and packed[i] is not None:
@@ -187,6 +184,13 @@ class DeviceCluster:
                 pods[i]['group_mask'] = self._layout.groups_mask(pod_groups[i], create=False)
             else:
                 packing.pack_pod(top, pod_groups[i], self._layout, out=pods[i])
+        return pods
+
+    def solve(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now: float, packed: Sequence = None):
+        """Bindings of ``tops`` scheduled in order on the synced cluster (one GPU call).  ``packed``: records
+        ``pack_pod`` already made of them; only the node-group mask is worked out again (``sync`` may have met new
+        group names since)."""
+        pods = self._pods(tops, pod_groups, packed)
         self.batches += 1
         self._solver.snapshot()                       # so that rewind() can step back inside this batch
         self._last = (pods, np.full(len(tops), now, dtype='<f8'))
@@ -198,6 +202,18 @@ class DeviceCluster:
         in use cannot explain (a stand-in without ``explain_batch``)."""
         fn = getattr(self._solver, 'explain_batch', None)
         return fn() if fn is not None else None
+
+    def query(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now, source: str = 'mirror',
+              packed: Sequence = None):
+        """Per pod, the binding it would get on its own (one GPU query, nothing placed): on the synced cluster
+        (``source='mirror'``) or on the state the last ``solve`` started from (``'snapshot'``, valid until the next
+        ``sync`` that uploads records).  ``now``: one clock or one per pod.  None when the solver in use cannot
+        answer queries (a stand-in without ``query_batch``)."""
+        fn = getattr(self._solver, 'query_batch', None)
+        if fn is None:
+            return None
+        nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
+        return fn(self._pods(tops, pod_groups, packed), nows, source=source)
 
     def rewind(self, k: int):
         """Put the device back to the state right after pod ``k`` of the last batch (restore the
@@ -231,7 +247,7 @@ class NHDScheduler:
     def __init__(self, k8s, cfg_parser: Callable, rpcq: Queue = None, solver_factory: Callable = None,
                  device: int = 0, clock: Callable[[], float] = time.monotonic,
                  wall: Callable[[], float] = time.time, node_cls=Node, logger=None,
-                 stats_from_device: bool = False):
+                 stats_from_device: bool = False, diagnose_contention: bool = False):
         self.nodes: Dict[str, Node] = {}
         self.k8s = k8s
         self.sched_name = NHD_SCHED_NAME
@@ -251,6 +267,11 @@ class NHDScheduler:
         # until the pod is scheduled or deleted
         self.unschedulable_reasons: Dict[tuple, Dict[str, int]] = {}
         self.stats_from_device = stats_from_device
+        # opt-in: for a pod that found no node, ask whether it would have fit alone at the start of its batch
+        # (nhd_query_batch on the batch-start snapshot); (ns, pod) -> that node, i.e. earlier pods of the same batch
+        # took the capacity.  Kept until the pod is scheduled or deleted.
+        self.diagnose_contention = diagnose_contention
+        self.contended_pods: Dict[tuple, str] = {}
 
     # ---- small helpers --------------------------------------------------------------------
     def _info(self, msg):
@@ -369,23 +390,26 @@ class NHDScheduler:
         ngroups = self.k8s.GetPodNodeGroups(podname, ns)
         return {n: v for n, v in self.nodes.items() if len(set(v.groups) & set(ngroups)) > 0 and v.active}
 
-    def _prepare(self, e: _Pending):
-        """The Kubernetes reads of ``AttemptScheduling`` up to ``FindNode`` (``:254-275``)."""
+    def _prepare(self, e: _Pending, events: bool = True):
+        """The Kubernetes reads of ``AttemptScheduling`` up to ``FindNode`` (``:254-275``); ``events=False`` only
+        reads (no pod event is generated)."""
         ns, podname = e.key[0], e.key[1]
         e.ready = True
         e.pobj = self.k8s.GetPodObj(podname, ns)
         if e.pobj is None:
             self._error(f'Could not get pod object for pod {ns}.{podname}')
             return
-        self.k8s.GeneratePodEvent(e.pobj, podname, ns, 'StartedScheduling', K8SEventType.EVENT_TYPE_NORMAL,
-                                  f'Started scheduling {ns}/{podname}')
+        if events:
+            self.k8s.GeneratePodEvent(e.pobj, podname, ns, 'StartedScheduling', K8SEventType.EVENT_TYPE_NORMAL,
+                                      f'Started scheduling {ns}/{podname}')
         _, cfgstr = self.k8s.GetCfgMap(podname, ns)
         cfgtype = self.k8s.GetCfgType(podname, ns)
         e.tcfg = self.GetCfgParser(cfgtype, cfgstr)
         e.top = e.tcfg.CfgToTopology(False)
         if e.top is None:
-            self.k8s.GeneratePodEvent(e.pobj, podname, ns, 'FailedCfgParse', K8SEventType.EVENT_TYPE_WARNING,
-                                      f'Error while processing config for pod {podname}')
+            if events:
+                self.k8s.GeneratePodEvent(e.pobj, podname, ns, 'FailedCfgParse', K8SEventType.EVENT_TYPE_WARNING,
+                                          f'Error while processing config for pod {podname}')
             return
         e.groups = self.k8s.GetPodNodeGroups(podname, ns)
         try:                                         # a request beyond the packed layout (include/nhd_b200.h, NHD_MAX_*)
@@ -486,7 +510,7 @@ class NHDScheduler:
                     self._prepare(e)
             now = float(self._clock())
             solvable = [e for e in run if e.top is not None and e.unsupported is None]
-            bindings, why = {}, None
+            bindings, why, contended = {}, None, None
             if solvable and self.nodes:
                 self.cluster.sync(self.nodes, self._dirty)
                 self._dirty.clear()
@@ -509,11 +533,15 @@ class NHDScheduler:
                 why = self.cluster.explain() if any(int(b['status']) == wire.NO_CANDIDATE for b in out) else None
                 if why is not None:
                     why = {e.pos: why[i] for i, e in enumerate(solvable)}
+                if self.diagnose_contention and any(int(b['status']) == wire.NO_CANDIDATE for b in out):
+                    contended = self._contention(solvable, out, now)
             cut = None
             for e in run:
                 b = bindings.get(e.pos)
                 if b is not None and int(b['status']) == wire.NO_CANDIDATE and why is not None:
                     self._explain(e, why[e.pos])
+                if b is not None and int(b['status']) == wire.NO_CANDIDATE and contended is not None:
+                    self._contended(e, contended[e.pos])
                 rewound = False
                 if b is not None and int(b['status']) in (wire.ASSIGN_FAILED, wire.REF_WOULD_CRASH):
                     # what a failed assignment leaves on its node is read back from the solver (see _finish);
@@ -544,9 +572,33 @@ class NHDScheduler:
         detail = ', '.join(f'{c} {name}' for name, c in sorted(reasons.items(), key=lambda kv: -kv[1]))
         self._info(f'Pod {ns}.{podname}: 0/{total} nodes are available: {detail}')
 
+    def _contention(self, solvable, out, now):
+        """{pos: node name or None} for the NO_CANDIDATE pods of the batch just solved: the node each would have been
+        placed on alone, at the state the batch started from (a query of the snapshot ``solve`` took).  None when the
+        solver in use cannot answer queries."""
+        failed = [i for i, b in enumerate(out) if int(b['status']) == wire.NO_CANDIDATE]
+        q = self.cluster.query([solvable[i].top for i in failed], [solvable[i].groups for i in failed], now,
+                               source='snapshot', packed=[solvable[i].rec for i in failed])
+        if q is None:
+            return None
+        return {solvable[i].pos: self.cluster.name_of(int(b['node'])) if int(b['status']) == wire.PLACED else None
+                for i, b in zip(failed, q)}
+
+    def _contended(self, e: _Pending, nodename):
+        """Remember and log that pod ``e`` found no node although it would have fit alone on ``nodename`` at the start
+        of its batch (earlier pods of the batch took the capacity); forget it when it would not have fit either."""
+        key = (e.key[0], e.key[1])
+        if nodename is None:
+            self.contended_pods.pop(key, None)
+            return
+        self.contended_pods[key] = nodename
+        self._info(f'Pod {key[0]}.{key[1]}: would have fit on node {nodename} alone; earlier pods of the same batch '
+                   f'took the capacity')
+
     def _record(self, key, ok: bool):                 # the two branches of CheckPendingPods (:431-436)
         podkey = (key[0], key[1])
         if ok:
+            self.contended_pods.pop(podkey, None)
             self.unschedulable_reasons.pop(podkey, None)
             self.pod_state[podkey] = {'state': PodStatus.POD_STATUS_SCHEDULED, 'time': self._wall(), 'uid': key[2]}
         else:
@@ -563,6 +615,42 @@ class NHDScheduler:
         else:
             self.pod_state[(ns, podname)] = saved
         return ok
+
+    def PreviewPods(self, keys: Sequence) -> Dict:
+        """Where each pod of ``keys`` (``(ns, name[, uid])``) would be placed right now on its own, without scheduling
+        anything: ``{(ns, name): node name}``, or None for a pod that would not be placed (no node, a failed
+        assignment on the chosen node, a config that does not parse, a request beyond the solver's limits).  The
+        pods do not see each other.  Only the Kubernetes reads of a scheduling attempt happen: no event, no write;
+        ``pod_state`` and the ``Node`` objects stay as they are.  Nodes the host changed are synced first, as for a
+        batch."""
+        entries = [_Pending(i, k) for i, k in enumerate(keys)]
+        for e in entries:
+            self._prepare(e, events=False)
+        result = {(e.key[0], e.key[1]): None for e in entries}
+        ok = [e for e in entries if e.top is not None and e.unsupported is None]
+        if not ok or not self.nodes:
+            return result
+        self.cluster.sync(self.nodes, self._dirty)
+        self._dirty.clear()
+        now = float(self._clock())
+        while ok:
+            try:
+                out = self.cluster.query([e.top for e in ok], [e.groups for e in ok], now,
+                                         packed=[e.rec for e in ok])
+                break
+            except Exception as err:                  # a pod beyond the tuple limits: it gets None, the rest goes on
+                m = re.search(r'pod (\d+)', str(err)) if getattr(err, 'code', None) == wire.ERR_UNSUPPORTED else None
+                if m is None or int(m.group(1)) >= len(ok):
+                    raise
+                ok.pop(int(m.group(1)))
+        else:
+            return result
+        if out is None:
+            raise RuntimeError('the solver in use cannot answer placement queries (no query_batch)')
+        for e, b in zip(ok, out):
+            if int(b['status']) == wire.PLACED:
+                result[(e.key[0], e.key[1])] = self.cluster.name_of(int(b['node']))
+        return result
 
     def CheckPendingPods(self):
         """``NHDScheduler.py:425-441`` with the pending set solved as one batch."""
@@ -622,6 +710,7 @@ class NHDScheduler:
                 self.ReleasePodResources(pn, ns)
                 self.pod_state.pop((ns, pn), None)
                 self.unschedulable_reasons.pop((ns, pn), None)
+                self.contended_pods.pop((ns, pn), None)
             else:
                 if ((ns, pn) in self.pod_state) and \
                         (self.pod_state[(ns, pn)]['state'] == PodStatus.POD_STATUS_SCHEDULED):

@@ -129,6 +129,20 @@ struct nhd_handle {
     uint8_t* d_xreasons = nullptr; size_t xreasons_cap = 0;
     uint32_t* d_xsmall = nullptr;                             /* n_failed, survivors */
 
+    /* Records generation: load and update change it, snapshot remembers it.  A query of the snapshot needs the two
+     * equal, so that the nodes' hardware classes (d_class, d_cls_fast, d_sigs: the mirror's) describe the snapshot. */
+    uint64_t rec_gen = 1, snap_rec_gen = 0;
+    /* query scratch (nhd_query_batch): its own pod types, per-pod arrays, bitmaps, summaries and tables, so that a
+     * query leaves the staged batch, its bindings and its filter output alone */
+    PodType* d_qtypes = nullptr;    size_t qtypes_cap = 0;
+    uint8_t* d_qpods = nullptr;     size_t qpods_cap = 0;        /* pod_type | now | group masks */
+    nhd_binding* d_qout = nullptr;  size_t qout_cap = 0;
+    uint8_t* h_q = nullptr;         size_t h_q_cap = 0;           /* pinned: types | pod_type | now | group masks */
+    nhd_binding* h_qout = nullptr;  size_t h_qout_cap = 0;        /* pinned */
+    uint64_t* d_qbitmaps = nullptr; size_t qbitmaps_cap = 0;
+    uint4* d_qdyn = nullptr;        size_t qdyn_cap = 0;
+    uint8_t* d_qftab = nullptr;
+
     nhd_timing timing;
     std::string err;
 };
@@ -314,6 +328,9 @@ extern "C" int32_t nhd_destroy(nhd_handle* h)
 #endif
     cudaFree(h->d_pend); cudaFree(h->d_vresult); cudaFree(h->d_pod_groups);
     cudaFree(h->d_xnode); cudaFree(h->d_xpod); cudaFree(h->d_xcounts); cudaFree(h->d_xreasons); cudaFree(h->d_xsmall);
+    cudaFree(h->d_qtypes); cudaFree(h->d_qpods); cudaFree(h->d_qout); cudaFree(h->d_qbitmaps); cudaFree(h->d_qdyn); cudaFree(h->d_qftab);
+    if (h->h_q) cudaFreeHost(h->h_q);
+    if (h->h_qout) cudaFreeHost(h->h_qout);
     if (h->h_stage) cudaFreeHost(h->h_stage);
     if (h->h_batch) cudaFreeHost(h->h_batch);
     if (h->h_out) cudaFreeHost(h->h_out);
@@ -463,6 +480,7 @@ extern "C" int32_t nhd_load_nodes(nhd_handle* h, int32_t n_nodes, const nhd_node
 {
     if (!h || n_nodes < 0 || (n_nodes > 0 && !recs)) return NHD_ERR_INVALID;
     h->gen++;
+    h->rec_gen++;
     CK(cudaSetDevice(h->params.device));
     const int n_super = std::max(1, (n_nodes + SUPER_NODES - 1) / SUPER_NODES);
     const size_t bytes = (size_t)n_super * SUPER_BYTES;
@@ -514,6 +532,7 @@ extern "C" int32_t nhd_update_nodes(nhd_handle* h, int32_t n, const int32_t* idx
     }
     if (n == 0) return NHD_OK;
     h->gen++;
+    h->rec_gen++;
     int mx = 1;
     const int32_t rc = upload_records(h, n, recs, idx, &mx);
     if (rc == NHD_OK) track_numa(h, n, recs, idx);
@@ -547,6 +566,7 @@ extern "C" int32_t nhd_snapshot(nhd_handle* h)
     CK(cudaStreamSynchronize(h->stream));
     h->have_snapshot = true;
     h->snap_gen = h->gen;
+    h->snap_rec_gen = h->rec_gen;
     return NHD_OK;
 }
 
@@ -596,34 +616,29 @@ static nhd_pod canonical_pod(const nhd_pod& in)
     return p;
 }
 
-extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod* pods, const double* now)
+/* node-group gate (NHDScheduler.py:235-247): one distinct pod group list -> folded into the pod types; several ->
+ * types are group-agnostic and the per-name node bitmaps apply the gate.  Returns whether the pods mix lists. */
+static bool group_lists(int n_pods, const nhd_pod* pods, uint64_t* names_used)
 {
-    if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now))) return NHD_ERR_INVALID;
-    if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_stage_batch before nhd_load_nodes");
-    const bool on_snapshot = h->gen == h->snap_gen;
-    h->gen++;
-    CK(cudaSetDevice(h->params.device));
-    h->staged = h->solved = false;
-
-    /* node-group gate (NHDScheduler.py:235-247): one distinct pod group list -> folded into the pod
-     * types; several -> types are group-agnostic and the sweep applies per-name node bitmaps */
     bool multi_group = false;
-    uint64_t names_used = 0;
+    uint64_t used = 0;
     for (int i = 0; i < n_pods; i++) {
-        names_used |= pods[i].group_mask;
+        used |= pods[i].group_mask;
         if (pods[i].group_mask != pods[0].group_mask) multi_group = true;
     }
-    h->n_names = 0;
-    h->names_used = 0;
-    if (multi_group) {
-        h->names_used = names_used;
-        h->n_names = __builtin_popcountll(names_used);
-    }
-    /* pod types = distinct descriptors (the reference re-derives everything per pod) */
+    *names_used = used;
+    return multi_group;
+}
+
+/* Validate the pods and de-duplicate them into pod types (distinct descriptors: the reference re-derives everything
+ * per pod): types[] and pod_type[i].  Refusals name the pod.  Touches nothing of the handle but its error text. */
+static int32_t make_pod_types(nhd_handle* h, int n_pods, const nhd_pod* pods, const double* now, bool multi_group,
+                              std::vector<PodType>& types, std::vector<int32_t>& pod_type)
+{
     std::unordered_map<PodKey, int32_t, PodKeyHash> index;
     index.reserve(64);
-    std::vector<PodType> types;
-    h->pod_type_host.resize(n_pods);
+    types.clear();
+    pod_type.resize(n_pods);
     /* pending sets repeat a few descriptors thousands of times: a descriptor seen before (byte for byte) skips
      * validation, normalisation and the map */
     struct RawSlot { uint64_t hash; int32_t type; nhd_pod raw; };
@@ -638,7 +653,7 @@ extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod*
         RawSlot& rs = raw_cache[rh & 255];
         if (rs.type >= 0 && rs.hash == rh && memcmp(&rs.raw, &pods[i], sizeof(nhd_pod)) == 0) {
             if (!std::isfinite(now[i])) return fail(h, NHD_ERR_INVALID, "pod %d: non-finite clock", i);
-            h->pod_type_host[i] = rs.type;
+            pod_type[i] = rs.type;
             continue;
         }
         int32_t v = nhd_validate_pod(&pods[i]);
@@ -657,9 +672,32 @@ extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod*
             it = index.emplace(k, (int32_t)types.size()).first;
             types.push_back(t);
         }
-        h->pod_type_host[i] = it->second;
+        pod_type[i] = it->second;
         rs.hash = rh; rs.type = it->second; rs.raw = pods[i];
     }
+    return NHD_OK;
+}
+
+extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod* pods, const double* now)
+{
+    if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now))) return NHD_ERR_INVALID;
+    if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_stage_batch before nhd_load_nodes");
+    const bool on_snapshot = h->gen == h->snap_gen;
+    h->gen++;
+    CK(cudaSetDevice(h->params.device));
+    h->staged = h->solved = false;
+
+    uint64_t names_used = 0;
+    const bool multi_group = group_lists(n_pods, pods, &names_used);
+    h->n_names = 0;
+    h->names_used = 0;
+    if (multi_group) {
+        h->names_used = names_used;
+        h->n_names = __builtin_popcountll(names_used);
+    }
+    std::vector<PodType> types;
+    const int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, types, h->pod_type_host);
+    if (rc != NHD_OK) return rc;
     const int T = (int)types.size();
     const size_t types_bytes = (size_t)T * sizeof(PodType);
     const size_t off_pt = (types_bytes + 15) & ~(size_t)15;
@@ -1033,6 +1071,104 @@ extern "C" int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_rea
     if ((rc = explain_launch(h, 1, nullptr, h->d_xreasons)) != NHD_OK) return rc;
     CK(cudaMemcpyAsync(node_reason, h->d_xreasons, (size_t)h->n_nodes, cudaMemcpyDeviceToHost, h->stream));
     return explain_survivors(h, "nhd_explain_pod");
+}
+
+/* ------------------------------------------------------------------ placement queries */
+
+/*
+ * Where each pod would go on its own, on the mirror or on the snapshot, with nothing written but the query's own
+ * scratch: de-duplicate into pod types (as nhd_stage_batch), filter the whole cluster into the query's bitmaps and
+ * summaries (fast_tables_kernel + filter_kernel, no sharding, no exchange), one warp per pod picks the node
+ * (query_select_kernel), one thread per placed pod works out the mapping and the assignment (query_assign_kernel).
+ */
+extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods, const nhd_pod* pods, const double* now,
+                                   nhd_binding* out)
+{
+    if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now || !out))) return NHD_ERR_INVALID;
+    if (source != NHD_QUERY_MIRROR && source != NHD_QUERY_SNAPSHOT)
+        return fail(h, NHD_ERR_INVALID, "query source %d is neither NHD_QUERY_MIRROR nor NHD_QUERY_SNAPSHOT", source);
+    if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_query_batch before nhd_load_nodes");
+    if (source == NHD_QUERY_SNAPSHOT && (!h->have_snapshot || h->snap_rec_gen != h->rec_gen))
+        return fail(h, NHD_ERR_STATE, "a snapshot query needs nhd_snapshot with no nhd_load_nodes / nhd_update_nodes since");
+    uint64_t names_used = 0;
+    const bool multi_group = group_lists(n_pods, pods, &names_used);
+    std::vector<PodType> types;
+    std::vector<int32_t> pod_type;
+    int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, types, pod_type);
+    if (rc != NHD_OK) return rc;
+    if (n_pods == 0) return NHD_OK;
+    CK(cudaSetDevice(h->params.device));
+    const int T = (int)types.size(), W = h->words;
+    const int n_names = multi_group ? __builtin_popcountll(names_used) : 0;
+    const uint8_t* nodes = source == NHD_QUERY_SNAPSHOT ? h->d_snapshot : h->d_nodes;
+
+    /* host -> device: types | pod_type | now | group masks, one pinned buffer */
+    const size_t types_bytes = (size_t)T * sizeof(PodType);
+    const size_t off_pt = 0, off_now = ((size_t)n_pods * 4 + 15) & ~(size_t)15;
+    const size_t off_gm = off_now + (size_t)n_pods * 8, pods_bytes = off_gm + (multi_group ? (size_t)n_pods * 8 : 0);
+    CK(grow_pinned(h->h_q, h->h_q_cap, types_bytes + pods_bytes));
+    memcpy(h->h_q, types.data(), types_bytes);
+    uint8_t* hp = h->h_q + types_bytes;
+    memcpy(hp + off_pt, pod_type.data(), (size_t)n_pods * 4);
+    memcpy(hp + off_now, now, (size_t)n_pods * 8);
+    if (multi_group)
+        for (int i = 0; i < n_pods; i++) memcpy(hp + off_gm + (size_t)i * 8, &pods[i].group_mask, 8);
+    CK(grow_dev(h->d_qtypes, h->qtypes_cap, types_bytes));
+    CK(grow_dev(h->d_qpods, h->qpods_cap, pods_bytes));
+    CK(grow_dev(h->d_qout, h->qout_cap, (size_t)n_pods * sizeof(nhd_binding)));
+    CK(grow_dev(h->d_qbitmaps, h->qbitmaps_cap, (size_t)(T + 2 + n_names) * W * 8));
+    CK(grow_dev(h->d_qdyn, h->qdyn_cap, (size_t)W * 64 * sizeof(NodeDyn)));
+    CK(cudaMemcpyAsync(h->d_qtypes, h->h_q, types_bytes, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_qpods, hp, pods_bytes, cudaMemcpyHostToDevice, h->stream));
+
+    /* the candidate bitmaps of the query's pod types on the chosen records */
+    const bool have_ftab = T <= FAST_MAX_TYPES;
+    if (have_ftab) {
+        if (!h->d_qftab) CK(cudaMalloc((void**)&h->d_qftab, ftab_bytes(FAST_MAX_TYPES)));
+        TablesArgs ta;
+        ta.types = h->d_qtypes; ta.n_types = T; ta.sigs = h->d_sigs; ta.out = h->d_qftab;
+        memcpy(ta.cap, h->cap, sizeof(ta.cap));
+        fast_tables_kernel<<<dim3(T, FAST_NSIG * 16 / 256), 256, 0, h->stream>>>(ta);
+        CK(cudaGetLastError());
+    }
+    FilterArgs fa;
+    fa.ftab = have_ftab ? h->d_qftab : nullptr; fa.mapt = h->d_mapt; fa.cls = h->d_cls_fast;
+    fa.nodes = nodes; fa.types = h->d_qtypes; fa.n_types = T; fa.n_nodes = h->n_nodes;
+    fa.super_lo = 0; fa.super_hi = h->n_super;
+    fa.dyn = h->d_qdyn; fa.bitmaps = h->d_qbitmaps; fa.words = W; fa.word_base = 0;
+    fa.class_id = h->d_class; fa.names_used = multi_group ? names_used : 0;
+    fa.now0 = now[0]; fa.min_busy = h->params.min_busy_secs;
+    memcpy(fa.cap, h->cap, sizeof(fa.cap));
+    fa.type_split = std::max(1, std::min(T, (h->sm_count * 2) / h->n_super));
+    const int fgrid = std::min(h->n_super, h->sm_count * 2) * fa.type_split;
+    const size_t fsmem = FILTER_STAGES * SUPER_BYTES + (T <= TYPES_SMEM_MAX ? (size_t)T * sizeof(PodType) : 0);
+    filter_kernel<<<fgrid, FILTER_THREADS, fsmem, h->stream>>>(fa);
+    CK(cudaGetLastError());
+
+    /* each pod on its own: the node, then the mapping and the assignment on a copy of its record */
+    QueryArgs qa;
+    qa.nodes = nodes; qa.types = h->d_qtypes;
+    qa.pod_type = reinterpret_cast<const int32_t*>(h->d_qpods + off_pt);
+    qa.now = reinterpret_cast<const double*>(h->d_qpods + off_now);
+    qa.bitmaps = h->d_qbitmaps;
+    qa.pod_groups = multi_group ? reinterpret_cast<const uint64_t*>(h->d_qpods + off_gm) : nullptr;
+    qa.names_used = multi_group ? names_used : 0;
+    qa.out = h->d_qout; qa.n_pods = n_pods; qa.n_types = T; qa.words = W;
+    qa.min_busy = h->params.min_busy_secs;
+    memcpy(qa.cap, h->cap, sizeof(qa.cap));
+    const int warps_per_cta = QUERY_SELECT_THREADS / 32;
+    query_select_kernel<<<(n_pods + warps_per_cta - 1) / warps_per_cta, QUERY_SELECT_THREADS, 0, h->stream>>>(qa);
+    CK(cudaGetLastError());
+    query_assign_kernel<<<(n_pods + 63) / 64, 64, 0, h->stream>>>(qa);
+    CK(cudaGetLastError());
+
+    const size_t out_bytes = (size_t)n_pods * sizeof(nhd_binding);
+    const bool direct = is_pinned_host(out);
+    if (!direct) CK(grow_pinned(h->h_qout, h->h_qout_cap, out_bytes));
+    CK(cudaMemcpyAsync(direct ? (void*)out : (void*)h->h_qout, h->d_qout, out_bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (!direct) memcpy(out, h->h_qout, out_bytes);
+    return NHD_OK;
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

@@ -21,6 +21,8 @@
  *   assign_cores_kernel   Node.GetFreeCpuBatch (nhd/Node.py:502-519) for every placed pod, in
  *                   parallel, from the snapshot core masks and per-socket prefix offsets
  *   commit_kernel   folds the batch into the node records
+ * Outside a solve: explain_* (why a pod found no node) and query_select / query_assign_kernel (where each pod
+ * of a query would go on its own, nhd_query_batch).
  *
  * Device layout of the node array ("tiled AoSoA"): tiles of 32 nodes, 4 KB each:
  *     byte offset(node n, 16-byte chunk c) = (n / 32) * 4096 + c * 512 + (n % 32) * 16
@@ -2616,6 +2618,110 @@ __global__ void __launch_bounds__(EXPLAIN_THREADS) explain_kernel(const __grid_c
             }
         }
     }
+}
+
+/* ------------------------------------------------------------------ placement queries (nhd_query_batch) */
+
+/*
+ * Not part of a solve: where each pod of a query would go on its own.  The query's pod types were filtered on the
+ * chosen record array into the query's own bitmaps (filter_kernel), so F[type] is exactly FindNode's candidate set on
+ * those records apart from the busy window.  Every pod is independent: one warp picks its node, then one thread works
+ * out the mapping and the assignment on a private copy of that node's record.
+ */
+struct QueryArgs {
+    const uint8_t* nodes;          /* the records queried (mirror or snapshot, tiled layout) */
+    const PodType* types;
+    const int32_t* pod_type;
+    const double* now;
+    const uint64_t* bitmaps;       /* [n_types + 2 + n_names][words]: F[0..T), NOGPU, BUSY (unused), per group name */
+    const uint64_t* pod_groups;    /* per-pod node-group lists of a query that mixes them, else null */
+    uint64_t names_used;
+    nhd_binding* out;
+    int n_pods, n_types, words;
+    double min_busy;
+    double cap[NHD_MAX_SPEED_CLASSES];
+};
+
+constexpr int QUERY_SELECT_THREADS = 128;
+
+/* One warp per pod: the first node in load order of F[type] & the pod's node-group gate, GPU-less nodes first for a
+ * pod without GPUs (SelectNode, Matcher.py:393-421), busy nodes skipped for a GPU pod at that pod's own clock
+ * (Matcher.py:107-111).  Writes the final binding of a pod without a node, and (node, NHD_PENDING) otherwise. */
+__global__ void __launch_bounds__(QUERY_SELECT_THREADS) query_select_kernel(const __grid_constant__ QueryArgs a)
+{
+    const int i = (int)((blockIdx.x * (unsigned)QUERY_SELECT_THREADS + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+    if (i >= a.n_pods) return;                                     /* whole warps */
+    const int ti = a.pod_type[i], W = a.words;
+    const PodType& t = a.types[ti];
+    uint4* bout = reinterpret_cast<uint4*>(&a.out[i]);
+    if (!t.valid_map) {                                            /* Matcher.py:45-47 */
+        if (lane < 8) bout[lane] = make_uint4(lane == 0 ? NHD_BAD_MAP_TYPE : 0, lane == 0 ? 0xFFFFFFFFu : 0, lane == 0 ? t.G : 0, 0);
+        return;
+    }
+    const uint64_t* F = a.bitmaps + (size_t)ti * W;
+    const uint64_t* NOGPU = a.bitmaps + (size_t)a.n_types * W;
+    const uint64_t* GB = a.bitmaps + (size_t)(a.n_types + 2) * W;
+    const uint64_t gm = a.pod_groups ? a.pod_groups[i] : 0;
+    const double now = a.now[i];
+    int chosen = -1;
+    for (int pass = t.needs_gpu ? 1 : 0; pass < 2 && chosen < 0; pass++) {
+        for (int base = 0; base < W && chosen < 0; base += 32) {
+            const int w = base + lane;
+            int mine = -1;
+            if (w < W) {
+                uint64_t word = F[w] & (pass == 0 ? NOGPU[w] : ~0ULL);
+                if (a.pod_groups && word) {                        /* InitialNodeFilter per group name (NHDScheduler.py:241) */
+                    uint64_t e = 0;
+                    for (uint64_t g = gm; g; g &= g - 1)
+                        e |= GB[(size_t)popc64(a.names_used & ((1ULL << ctz64(g)) - 1)) * W + w];
+                    word &= e;
+                }
+                for (; word; word &= word - 1) {
+                    const int node = w * 64 + ctz64(word);
+                    if (t.needs_gpu) {
+                        nhd_node_rec r;
+                        r.busy_time = *reinterpret_cast<const double*>(a.nodes + chunk_off(node, 3));
+                        if (node_busy(r, now, a.min_busy)) continue;
+                    }
+                    mine = node;
+                    break;
+                }
+            }
+            const unsigned m = __ballot_sync(0xFFFFFFFFu, mine >= 0);
+            if (m) chosen = __shfl_sync(0xFFFFFFFFu, mine, ctz32(m));
+        }
+    }
+    if (lane < 8) {
+        uint4 v = make_uint4(0, 0, 0, 0);
+        if (lane == 0) v = chosen < 0 ? make_uint4(NHD_NO_CANDIDATE, 0xFFFFFFFFu, t.G, 0) : make_uint4(NHD_PENDING, (uint32_t)chosen, 0, 0);
+        bout[lane] = v;
+    }
+}
+
+/* One thread per pod with a node: GetNumaGroupIdx + SetBusy + SetPhysicalIdsFromMapping + ClaimPodNICResources
+ * (evaluate_mapping, assign_pod) on a private copy of the node's record, which is not written back. */
+__global__ void query_assign_kernel(const __grid_constant__ QueryArgs a)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= a.n_pods) return;
+    const uint2 hd = *reinterpret_cast<const uint2*>(&a.out[i]);
+    if ((int)hd.x != NHD_PENDING) return;
+    const int node = (int)hd.y;
+    const PodType& t = a.types[a.pod_type[i]];
+    RecU u;
+    load_rec(a.nodes, node, u);
+    union { nhd_binding b; uint4 q[8]; } bu;
+    for (int c = 0; c < 8; c++) bu.q[c] = make_uint4(0, 0, 0, 0);
+    Mapping m;
+    if (evaluate_mapping(u.r, t, a.cap, &m)) {
+        bu.b.node = node;
+        assign_pod(u.r, t, m, a.now[i], &bu.b);
+    } else {
+        bu.b.status = NHD_NO_CANDIDATE;          /* cannot happen: the filter bit said feasible */
+        bu.b.node = -1;
+        bu.b.n_groups = t.G;
+    }
+    for (int c = 0; c < 8; c++) reinterpret_cast<uint4*>(&a.out[i])[c] = bu.q[c];
 }
 
 } // namespace nhd

@@ -183,6 +183,22 @@ class Solver:
         self._ck(self._L.nhd_explain_pod(self._h, int(i), out.ctypes.data))
         return out
 
+    # ---- placement queries ----------------------------------------------------------
+    def query_batch(self, pods, now, source='mirror', out=None):
+        """Where each pod would go on its own (``nhd_query_batch``): per pod the binding ``solve_batch`` would return
+        for that pod alone, on the current records (``source='mirror'``) or on those of the last ``snapshot()``
+        (``'snapshot'``).  Nothing is placed: records, snapshot, the last batch and its explanations stay as they are."""
+        src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
+        if src is None:
+            raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
+        pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
+        now = np.ascontiguousarray(now, dtype='<f8')
+        assert len(pods) == len(now)
+        if out is None:
+            out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
+        self._ck(self._L.nhd_query_batch(self._h, src, len(pods), pods.ctypes.data, now.ctypes.data, out.ctypes.data))
+        return out
+
     def filter_bitmaps(self):
         """Runs only the snapshot predicate kernel on the staged batch; returns
         (feas[type, node] bool, nogpu[node], busy[node], pod_type[pod])."""

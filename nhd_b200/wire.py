@@ -28,6 +28,9 @@ WHY_COUNT = 9
 WHY_NONE = 0xFF
 WHY_NAMES = ('group', 'inactive', 'maintenance', 'hugepages', 'busy', 'gpu', 'cpu', 'nic', 'intersect')
 
+# nhd_query_batch sources (NHD_QUERY_*)
+QUERY_MIRROR, QUERY_SNAPSHOT = 0, 1
+
 MAP_INVALID, MAP_NUMA, MAP_PCI, MAP_NONE = 0, 1, 2, 3
 NODE_SMT, NODE_ACTIVE, NODE_MAINTENANCE = 1, 2, 4
 GRP_PROC_SMT, GRP_HELPER_SMT, GRP_HAS_NIC_CORES = 1, 2, 4
