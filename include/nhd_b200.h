@@ -302,6 +302,25 @@ int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_reason);
 int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods, const nhd_pod* pods,
                         const double* now, nhd_binding* out);
 
+/*
+ * A dry run of a batch: where the pods would go scheduled in order, each seeing the ones before it, with nothing
+ * placed.  source is NHD_QUERY_MIRROR or NHD_QUERY_SNAPSHOT, under the same rule as nhd_query_batch.  The nodes
+ * excluded[0..n_excluded) are taken as if NHD_NODE_MAINTENANCE were set on their records (Matcher.py:73: what a
+ * maintenance start does); an index outside [0, n_nodes) is NHD_ERR_INVALID, a duplicate counts once.
+ *   out[i]         byte for byte what nhd_solve_batch(h, n_pods, pods, now, out) would return on the chosen records
+ *                  with the excluded nodes so marked;
+ *   why_counts     (may be NULL) n_pods * NHD_WHY_COUNT entries: what nhd_explain_batch would return after that solve
+ *                  (an excluded node that passes the group and active stages counts as NHD_WHY_MAINTENANCE).
+ * Pods are validated and refused as by nhd_stage_batch, naming the pod index; the tuple limits are judged as that solve
+ * would judge them, without the excluded nodes.  Nothing is written that a caller can observe: not the mirror, the
+ * snapshot, the staged batch, its bindings, filter bitmaps or explanations, nhd_last_timing or nhd_debug_counters.  No
+ * collective: every rank holds all records, filters the whole cluster and may call alone (the bindings do not depend
+ * on sharding).  Waits for the device before returning.
+ */
+int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                       int32_t n_pods, const nhd_pod* pods, const double* now,
+                       nhd_binding* out, uint32_t* why_counts);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

@@ -215,6 +215,23 @@ class DeviceCluster:
         nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
         return fn(self._pods(tops, pod_groups, packed), nows, source=source)
 
+    def plan(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now, source: str = 'mirror',
+             exclude: Iterable[str] = (), packed: Sequence = None, explain: bool = False):
+        """The bindings of ``tops`` scheduled in order, each seeing the ones before it, with nothing placed (one GPU
+        dry run): on the synced cluster (``source='mirror'``) or on the state the last ``solve`` started from
+        (``'snapshot'``), with the nodes named in ``exclude`` taken as in maintenance.  ``explain=True``: also the
+        per-reason node counts of the NO_CANDIDATE pods, as ``explain`` gives them after a ``solve``.  None when the
+        solver in use cannot plan (a stand-in without ``plan_batch``)."""
+        fn = getattr(self._solver, 'plan_batch', None)
+        if fn is None:
+            return None
+        missing = [n for n in exclude if n not in self._index]
+        if missing:
+            raise ValueError(f'cannot exclude unknown node(s) {missing}')
+        idx = np.asarray([self._index[n] for n in exclude], dtype='<i4')
+        nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
+        return fn(self._pods(tops, pod_groups, packed), nows, source=source, exclude=idx, explain=explain)
+
     def rewind(self, k: int):
         """Put the device back to the state right after pod ``k`` of the last batch (restore the
         snapshot taken before it, solve pods ``0..k`` again: the solver is deterministic)."""
@@ -651,6 +668,62 @@ class NHDScheduler:
             if int(b['status']) == wire.PLACED:
                 result[(e.key[0], e.key[1])] = self.cluster.name_of(int(b['node']))
         return result
+
+    def PlanPods(self, keys: Sequence):
+        """Would the pods of ``keys`` (``(ns, name[, uid])``) all be placed if they were scheduled now, in this order?
+        A dry run of the batch on the synced cluster: each pod sees the ones before it, nothing is placed.  Returns
+        ``(placement, reasons)``: ``placement[(ns, name)]`` is the node the pod would be bound to, or None (no node, a
+        failed assignment, a config that does not parse, a request beyond the solver's limits); ``reasons[(ns, name)]``
+        is ``{reason name: nodes}`` (``wire.WHY_NAMES``) for each pod that would find no node, as
+        ``unschedulable_reasons`` would hold it.  Only the Kubernetes reads of a scheduling attempt happen: no event,
+        no write; ``pod_state``, the ``Node`` objects and the counters stay as they are."""
+        return self._plan(keys, ())
+
+    def PlanDrain(self, node_names: Sequence[str]):
+        """Can these nodes be taken down?  Where the pods now on them (nodes in the given order, pods in
+        ``Node.pod_info`` order) would go if they were re-created, read as a scheduling attempt reads them, with those
+        nodes in maintenance.  Same dry run and the same ``(placement, reasons)`` as ``PlanPods``."""
+        names = list(node_names)
+        missing = [n for n in names if n not in self.nodes]
+        if missing:
+            raise ValueError(f'unknown node(s) {missing}')
+        keys = [(ns, pod) for n in names for (pod, ns) in self.nodes[n].pod_info]
+        return self._plan(keys, names)
+
+    def _plan(self, keys: Sequence, exclude: Sequence[str]):
+        entries = [_Pending(i, k) for i, k in enumerate(keys)]
+        for e in entries:
+            self._prepare(e, events=False)
+        placement = {(e.key[0], e.key[1]): None for e in entries}
+        reasons = {}
+        ok = [e for e in entries if e.top is not None and e.unsupported is None]
+        if not ok or not self.nodes:
+            return placement, reasons
+        self.cluster.sync(self.nodes, self._dirty)
+        self._dirty.clear()
+        now = float(self._clock())
+        while ok:
+            try:
+                res = self.cluster.plan([e.top for e in ok], [e.groups for e in ok], now, exclude=exclude,
+                                        packed=[e.rec for e in ok], explain=True)
+                break
+            except Exception as err:                  # a pod beyond the tuple limits: it gets None, the rest goes on
+                m = re.search(r'pod (\d+)', str(err)) if getattr(err, 'code', None) == wire.ERR_UNSUPPORTED else None
+                if m is None or int(m.group(1)) >= len(ok):
+                    raise
+                ok.pop(int(m.group(1)))
+        else:
+            return placement, reasons
+        if res is None:
+            raise RuntimeError('the solver in use cannot plan batches (no plan_batch)')
+        out, counts = res
+        for e, b, c in zip(ok, out, counts):
+            key = (e.key[0], e.key[1])
+            if int(b['status']) == wire.PLACED:
+                placement[key] = self.cluster.name_of(int(b['node']))
+            elif int(b['status']) == wire.NO_CANDIDATE:
+                reasons[key] = {name: int(n) for name, n in zip(wire.WHY_NAMES, c) if int(n)}
+        return placement, reasons
 
     def CheckPendingPods(self):
         """``NHDScheduler.py:425-441`` with the pending set solved as one batch."""

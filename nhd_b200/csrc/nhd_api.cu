@@ -14,6 +14,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdarg>
+#include <cstddef>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -58,6 +59,8 @@ struct NcclApi {
     }
 };
 static NcclApi g_nccl;
+
+static_assert(offsetof(nhd_node_rec, flags) == 2 * 16 + REC_FLAGS_BYTE, "exclude_nodes_kernel's flags byte");
 
 /* ------------------------------------------------------------------ handle */
 
@@ -142,6 +145,14 @@ struct nhd_handle {
     uint64_t* d_qbitmaps = nullptr; size_t qbitmaps_cap = 0;
     uint4* d_qdyn = nullptr;        size_t qdyn_cap = 0;
     uint8_t* d_qftab = nullptr;
+    /* plan scratch (nhd_plan_batch), on top of the query's: the sweep's cursors, busy list and pend, its debug
+     * counters, and the copy of the records the excluded nodes are flagged in */
+    int32_t* d_pcursors = nullptr;  size_t pcursors_cap = 0;
+    int32_t* d_pbusy = nullptr;     size_t pbusy_cap = 0;
+    int32_t* d_ppend = nullptr;     size_t ppend_cap = 0;
+    unsigned long long* d_pprof = nullptr;
+    uint8_t* d_pnodes = nullptr;    size_t pnodes_cap = 0;
+    int32_t* d_pidx = nullptr;      size_t pidx_cap = 0;
 
     nhd_timing timing;
     std::string err;
@@ -329,6 +340,7 @@ extern "C" int32_t nhd_destroy(nhd_handle* h)
     cudaFree(h->d_pend); cudaFree(h->d_vresult); cudaFree(h->d_pod_groups);
     cudaFree(h->d_xnode); cudaFree(h->d_xpod); cudaFree(h->d_xcounts); cudaFree(h->d_xreasons); cudaFree(h->d_xsmall);
     cudaFree(h->d_qtypes); cudaFree(h->d_qpods); cudaFree(h->d_qout); cudaFree(h->d_qbitmaps); cudaFree(h->d_qdyn); cudaFree(h->d_qftab);
+    cudaFree(h->d_pcursors); cudaFree(h->d_pbusy); cudaFree(h->d_ppend); cudaFree(h->d_pprof); cudaFree(h->d_pnodes); cudaFree(h->d_pidx);
     if (h->h_q) cudaFreeHost(h->h_q);
     if (h->h_qout) cudaFreeHost(h->h_qout);
     if (h->h_stage) cudaFreeHost(h->h_stage);
@@ -631,9 +643,10 @@ static bool group_lists(int n_pods, const nhd_pod* pods, uint64_t* names_used)
 }
 
 /* Validate the pods and de-duplicate them into pod types (distinct descriptors: the reference re-derives everything
- * per pod): types[] and pod_type[i].  Refusals name the pod.  Touches nothing of the handle but its error text. */
+ * per pod): types[] and pod_type[i].  Refusals name the pod; the tuple limits are judged against max_numa.  Touches
+ * nothing of the handle but its error text. */
 static int32_t make_pod_types(nhd_handle* h, int n_pods, const nhd_pod* pods, const double* now, bool multi_group,
-                              std::vector<PodType>& types, std::vector<int32_t>& pod_type)
+                              int max_numa, std::vector<PodType>& types, std::vector<int32_t>& pod_type)
 {
     std::unordered_map<PodKey, int32_t, PodKeyHash> index;
     index.reserve(64);
@@ -659,9 +672,9 @@ static int32_t make_pod_types(nhd_handle* h, int n_pods, const nhd_pod* pods, co
         int32_t v = nhd_validate_pod(&pods[i]);
         if (v != NHD_OK) return fail(h, v, "pod %d: descriptor rejected by nhd_validate_pod", i);
         if (!std::isfinite(now[i])) return fail(h, NHD_ERR_INVALID, "pod %d: non-finite clock", i);
-        if (!tuple_limits_ok(h->max_numa, pods[i].n_groups))
+        if (!tuple_limits_ok(max_numa, pods[i].n_groups))
             return fail(h, NHD_ERR_UNSUPPORTED, "pod %d: %d groups on %d-NUMA nodes exceeds the tuple limits", i,
-                        (int)pods[i].n_groups, h->max_numa);
+                        (int)pods[i].n_groups, max_numa);
         PodKey k{canonical_pod(pods[i])};
         if (multi_group) k.p.group_mask = ~0ULL;
         auto it = index.find(k);
@@ -696,7 +709,7 @@ extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod*
         h->n_names = __builtin_popcountll(names_used);
     }
     std::vector<PodType> types;
-    const int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, types, h->pod_type_host);
+    const int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, h->max_numa, types, h->pod_type_host);
     if (rc != NHD_OK) return rc;
     const int T = (int)types.size();
     const size_t types_bytes = (size_t)T * sizeof(PodType);
@@ -752,17 +765,52 @@ extern "C" int32_t nhd_run_filter_only(nhd_handle* h)
     return nhd_sync(h);
 }
 
-static int32_t solve_staged(nhd_handle* h, bool filter_only)
+/* One solve's inputs and outputs on the device: the records it starts from, the pod set, and every buffer its kernels
+ * write.  A batch runs on the handle's own buffers (batch_work); a plan on the query scratch plus its own sweep buffers
+ * (nhd_plan_batch), so that it leaves the staged batch, its bindings and its filter output alone. */
+struct SolveWork {
+    uint8_t* nodes;                   /* records at the start of the solve (tiled); only a batch's commit writes them */
+    const PodType* types;
+    const int32_t* pod_type;
+    const double* now;
+    const uint64_t* pod_groups;       /* per-pod node-group masks when n_names > 0, else null */
+    int n_pods, n_types, n_names;
+    uint64_t names_used;
+    double now0;                      /* clock of the first pod (the filter's BUSY row) */
+    bool const_clock;
+    uint64_t* bitmaps;                /* [n_types + 2 + n_names][words] */
+    uint4* dyn;                       /* NodeDyn summaries */
+    int32_t* cursors;                 /* [max(n_types, 1)][3] */
+    int32_t* busy_list;               /* n_super * SUPER_NODES + 64 */
+    int32_t* pend;                    /* n_super * SUPER_NODES */
+    uint8_t* ftab;                    /* ftab_bytes(FAST_MAX_TYPES) */
+    nhd_binding* out;                 /* n_pods + 8 (spare records for check builds) */
+    unsigned long long* prof;         /* the sweep's debug counters (nhd_debug_counters reads the batch's) */
+};
+
+static SolveWork batch_work(nhd_handle* h, uint8_t* records)
 {
-    if (!h) return NHD_ERR_INVALID;
-    if (!h->staged) return fail(h, NHD_ERR_STATE, "nhd_solve_staged without a staged batch");
-    const bool explainable = !filter_only && h->batch_on_snapshot && h->gen == h->stage_gen;
-    h->gen++;
-    h->explain_gen = explainable ? h->gen : 0;
-    CK(cudaSetDevice(h->params.device));
-    const int T = h->n_types, W = h->words;
+    SolveWork w;
+    w.nodes = records; w.types = h->d_types; w.pod_type = h->d_pod_type; w.now = h->d_now;
+    w.pod_groups = h->n_names ? h->d_pod_groups : nullptr;
+    w.n_pods = h->n_pods; w.n_types = h->n_types; w.n_names = h->n_names; w.names_used = h->names_used;
+    w.now0 = h->now0; w.const_clock = h->const_clock;
+    w.bitmaps = h->d_bitmaps; w.dyn = h->d_dyn; w.cursors = h->d_cursors; w.busy_list = h->d_busy_list; w.pend = h->d_pend;
+    w.ftab = h->d_ftab; w.out = h->d_out; w.prof = h->d_prof;
+    return w;
+}
+
+/*
+ * The launches of a solve on one workspace: direct-path tables, filter, sweep, resolve, core ids.  batch = the handle's
+ * staged batch: its timing events, the node-sharded filter + exchange when world_size > 1, and commit_kernel, which
+ * folds the bindings into w.nodes.  Without it (a plan, or a query's filter) none of the three: every rank filters the
+ * whole cluster and the records are only read.  filter_only stops after the filter.
+ */
+static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool filter_only)
+{
+    const int T = w.n_types, W = h->words;
     int launches = 0;
-    CK(cudaEventRecord(h->ev[0], h->stream));
+    if (batch) CK(cudaEventRecord(h->ev[0], h->stream));
 
     /* 1. snapshot predicate kernel over this rank's node shard.  With several ranks every rank filters the nodes
      * of S consecutive super-tiles into its slot of an exchange buffer (their NodeDyn summaries, then their
@@ -770,28 +818,28 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
      * as the arrays the (replicated) sweep reads.  Clusters too small for that to pay (nhd_shard_min_pairs) are
      * filtered whole by every rank, without any exchange. */
     const int ws = h->params.world_size, rk = h->params.rank;
-    const int rows = T + 2 + h->n_names;
+    const int rows = T + 2 + w.n_names;
     const size_t bm_bytes = (size_t)rows * W * 8;
-    const bool sharded = ws > 1 && h->n_pods > 0 && (long long)h->n_nodes * T >= h->shard_min_pairs;
+    const bool sharded = batch && ws > 1 && w.n_pods > 0 && (long long)h->n_nodes * T >= h->shard_min_pairs;
     const int S = sharded ? (h->n_super + ws - 1) / ws : h->n_super;
     const int super_lo = sharded ? std::min(rk * S, h->n_super) : 0;
     const int super_hi = sharded ? std::min(super_lo + S, h->n_super) : h->n_super;
     const size_t slot_bytes = (size_t)S * 32 * (SUPER_NODES + rows);
     if (sharded) CK(grow_dev(h->d_xchg, h->xchg_cap, slot_bytes * ws));
     const bool have_ftab = T > 0 && T <= FAST_MAX_TYPES;
-    if (h->n_pods > 0 && have_ftab) {
+    if (w.n_pods > 0 && have_ftab) {
         /* 0. the direct-path tables of this batch's pod types (filter and sweep both read them) */
         TablesArgs ta;
-        ta.types = h->d_types; ta.n_types = T; ta.sigs = h->d_sigs; ta.out = h->d_ftab;
+        ta.types = w.types; ta.n_types = T; ta.sigs = h->d_sigs; ta.out = w.ftab;
         memcpy(ta.cap, h->cap, sizeof(ta.cap));
         fast_tables_kernel<<<dim3(T, FAST_NSIG * 16 / 256), 256, 0, h->stream>>>(ta);
         CK(cudaGetLastError());
         launches++;
     }
-    if (h->n_pods > 0 && super_hi > super_lo) {
+    if (w.n_pods > 0 && super_hi > super_lo) {
         FilterArgs fa;
-        fa.ftab = have_ftab ? h->d_ftab : nullptr; fa.mapt = h->d_mapt; fa.cls = h->d_cls_fast;
-        fa.nodes = h->d_nodes; fa.types = h->d_types; fa.n_types = T; fa.n_nodes = h->n_nodes;
+        fa.ftab = have_ftab ? w.ftab : nullptr; fa.mapt = h->d_mapt; fa.cls = h->d_cls_fast;
+        fa.nodes = w.nodes; fa.types = w.types; fa.n_types = T; fa.n_nodes = h->n_nodes;
         fa.super_lo = super_lo; fa.super_hi = super_hi;
         if (sharded) {
             uint8_t* slot = h->d_xchg + slot_bytes * rk;
@@ -799,10 +847,10 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
             fa.bitmaps = reinterpret_cast<uint64_t*>(slot + (size_t)S * SUPER_NODES * 32);
             fa.words = S * 4; fa.word_base = super_lo * 4;
         } else {
-            fa.dyn = h->d_dyn; fa.bitmaps = h->d_bitmaps; fa.words = W; fa.word_base = 0;
+            fa.dyn = w.dyn; fa.bitmaps = w.bitmaps; fa.words = W; fa.word_base = 0;
         }
-        fa.class_id = h->d_class; fa.names_used = h->names_used;
-        fa.now0 = h->now0; fa.min_busy = h->params.min_busy_secs;
+        fa.class_id = h->d_class; fa.names_used = w.names_used;
+        fa.now0 = w.now0; fa.min_busy = h->params.min_busy_secs;
         memcpy(fa.cap, h->cap, sizeof(fa.cap));
         /* few super-tiles (small cluster, or a rank's shard): deal the pod types over several CTAs per super-tile */
         const int n_sh = super_hi - super_lo;
@@ -813,7 +861,7 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
         CK(cudaGetLastError());
         launches++;
     }
-    CK(cudaEventRecord(h->ev[1], h->stream));
+    if (batch) CK(cudaEventRecord(h->ev[1], h->stream));
 
     /* 2. one collective per batch: every rank contributes its slot */
     if (sharded) {
@@ -821,27 +869,29 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
         if (r != 0) return fail(h, NHD_ERR_NCCL, "ncclAllGather: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
         const size_t n16 = slot_bytes / 16 * ws;
         unpack_slots_kernel<<<(unsigned)((n16 + 255) / 256), 256, 0, h->stream>>>(reinterpret_cast<const uint4*>(h->d_xchg), ws, S, h->n_super,
-                                                                              rows, W, h->d_dyn, h->d_bitmaps);
+                                                                              rows, W, w.dyn, w.bitmaps);
         CK(cudaGetLastError());
         launches += 2;
     }
-    CK(cudaEventRecord(h->ev[2], h->stream));
+    if (batch) CK(cudaEventRecord(h->ev[2], h->stream));
 
     /* 3. sequential select + assign sweep (replicated on every rank) */
-    if (h->n_pods > 0 && !filter_only) {
+    if (w.n_pods > 0 && !filter_only) {
         SweepArgs sa;
-        sa.nodes = h->d_nodes; sa.types = h->d_types; sa.pod_type = h->d_pod_type; sa.now = h->d_now; sa.out = h->d_out;
-        sa.n_pods = h->n_pods; sa.n_types = T; sa.n_nodes = h->n_nodes; sa.words = W;
-        sa.n_names = h->n_names; sa.names_used = h->names_used; sa.pod_groups = h->d_pod_groups;
+        sa.nodes = w.nodes; sa.types = w.types; sa.pod_type = w.pod_type; sa.now = w.now; sa.out = w.out;
+        sa.n_pods = w.n_pods; sa.n_types = T; sa.n_nodes = h->n_nodes; sa.words = W;
+        sa.n_names = w.n_names; sa.names_used = w.names_used; sa.pod_groups = w.pod_groups;
         /* reserved_ (test knobs; every setting gives the same bindings): low byte 0 = default, 1 = the general one-warp
          * sweep only (no standing decisions), 2 = standing decisions but never the two pod classes side by side;
          * bits 8.. = debug switches of sweep_kernel */
-        sa.dual = (h->const_clock && (h->params.reserved_ & 0xFF) != 1) ? 1 : 0;
+        sa.dual = (w.const_clock && (h->params.reserved_ & 0xFF) != 1) ? 1 : 0;
         sa.sweep_flags = ((h->params.reserved_ & 0xFF) == 2 ? 1 : 0) | ((h->params.reserved_ >> 8) << 8);
-        sa.bitmaps = h->d_bitmaps; sa.dyn = h->d_dyn; sa.cursors = h->d_cursors; sa.busy_list = h->d_busy_list;
-        sa.memo = h->d_memo; sa.prof = h->d_prof; sa.pend_pod = h->d_pend;
+        sa.bitmaps = w.bitmaps; sa.dyn = w.dyn; sa.cursors = w.cursors; sa.busy_list = w.busy_list;
+        /* the mapping memo is a pure cache of choose_mapping (its key holds every input: K, G and the three stage
+         * masks), so every workspace shares the handle's */
+        sa.memo = h->d_memo; sa.prof = w.prof; sa.pend_pod = w.pend;
         sa.mapt = h->d_mapt; sa.mapt2 = h->d_mapt2; sa.sigs = h->d_sigs; sa.cls_fast = h->d_cls_fast;
-        sa.ftab = (T > 0 && T <= FAST_MAX_TYPES) ? h->d_ftab : nullptr;
+        sa.ftab = (T > 0 && T <= FAST_MAX_TYPES) ? w.ftab : nullptr;
         sa.min_busy = h->params.min_busy_secs;
         memcpy(sa.cap, h->cap, sizeof(sa.cap));
         /* shared memory: memo front | pod types | cursors | (bitmaps when they fit) */
@@ -862,20 +912,38 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
         }
         CK(cudaGetLastError());
         FinishArgs fin;
-        fin.nodes = h->d_nodes; fin.types = h->d_types; fin.pod_type = h->d_pod_type; fin.out = h->d_out;
-        fin.dyn = h->d_dyn; fin.n_pods = h->n_pods;
-        const int fthreads = 128, fgrid = (h->n_pods + fthreads - 1) / fthreads;
-        resolve_kernel<<<(h->n_pods + 63) / 64, 64, 0, h->stream>>>(sa);
+        fin.nodes = w.nodes; fin.types = w.types; fin.pod_type = w.pod_type; fin.out = w.out;
+        fin.dyn = w.dyn; fin.n_pods = w.n_pods;
+        const int fthreads = 128, fgrid = (w.n_pods + fthreads - 1) / fthreads;
+        resolve_kernel<<<(w.n_pods + 63) / 64, 64, 0, h->stream>>>(sa);
         CK(cudaGetLastError());
         assign_cores_kernel<<<fgrid, fthreads, 0, h->stream>>>(fin);
         CK(cudaGetLastError());
-        commit_kernel<<<fgrid, fthreads, 0, h->stream>>>(fin);
-        CK(cudaGetLastError());
-        launches += 4;
+        launches += 3;
+        if (batch) {
+            commit_kernel<<<fgrid, fthreads, 0, h->stream>>>(fin);
+            CK(cudaGetLastError());
+            launches++;
+        }
     }
-    CK(cudaEventRecord(h->ev[3], h->stream));
-    h->timing.n_launches = launches;
-    h->timing.n_types = T;
+    if (batch) {
+        CK(cudaEventRecord(h->ev[3], h->stream));
+        h->timing.n_launches = launches;
+        h->timing.n_types = T;
+    }
+    return NHD_OK;
+}
+
+static int32_t solve_staged(nhd_handle* h, bool filter_only)
+{
+    if (!h) return NHD_ERR_INVALID;
+    if (!h->staged) return fail(h, NHD_ERR_STATE, "nhd_solve_staged without a staged batch");
+    const bool explainable = !filter_only && h->batch_on_snapshot && h->gen == h->stage_gen;
+    h->gen++;
+    h->explain_gen = explainable ? h->gen : 0;
+    CK(cudaSetDevice(h->params.device));
+    const int32_t rc = launch_solve(h, batch_work(h, h->d_nodes), true, filter_only);
+    if (rc != NHD_OK) return rc;
     h->solved = true;
     return NHD_OK;
 }
@@ -962,11 +1030,11 @@ static int32_t explain_ready(nhd_handle* h)
     return NHD_OK;
 }
 
-/* The pods bound to each node, in pod order (CSR over the batch's bindings), and the list of NO_CANDIDATE pods.
+/* The pods of a solve bound to each node, in pod order (CSR over w.out), and the list of NO_CANDIDATE pods.
  * Returns the number of NO_CANDIDATE pods in *n_failed. */
-static int32_t explain_prepare(nhd_handle* h, int* n_failed)
+static int32_t explain_prepare(nhd_handle* h, const SolveWork& w, int* n_failed)
 {
-    const int N = h->n_nodes, P = h->n_pods;
+    const int N = h->n_nodes, P = w.n_pods;
     CK(grow_dev(h->d_xnode, h->xnode_cap, ((size_t)3 * N + 2) * 4));
     CK(grow_dev(h->d_xpod, h->xpod_cap, ((size_t)2 * P + 1) * 4));
     if (!h->d_xsmall) CK(cudaMalloc((void**)&h->d_xsmall, 16));
@@ -979,14 +1047,14 @@ static int32_t explain_prepare(nhd_handle* h, int* n_failed)
     CK(cudaMemsetAsync(h->d_xsmall, 0, 16, h->stream));
     const int threads = 256;
     if (P > 0) {
-        explain_count_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(h->d_out, P, node_cnt, failed,
+        explain_count_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(w.out, P, node_cnt, failed,
                                                                                      (int32_t*)h->d_xsmall);
         CK(cudaGetLastError());
     }
     explain_scan_kernel<<<1, EXPLAIN_SCAN_THREADS, 0, h->stream>>>(node_cnt, N, node_start, cursor);
     CK(cudaGetLastError());
     if (P > 0) {
-        explain_fill_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(h->d_out, P, cursor, node_pods);
+        explain_fill_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(w.out, P, cursor, node_pods);
         CK(cudaGetLastError());
     }
     if (N > 0) {
@@ -1000,14 +1068,14 @@ static int32_t explain_prepare(nhd_handle* h, int* n_failed)
     return NHD_OK;
 }
 
-/* one (failed pod x node) pass; counts and/or reasons may be null */
-static int32_t explain_launch(nhd_handle* h, int n_failed, uint32_t* d_counts, uint8_t* d_reasons)
+/* one (failed pod x node) pass over a solve whose start records are w.nodes; counts and/or reasons may be null */
+static int32_t explain_launch(nhd_handle* h, const SolveWork& w, int n_failed, uint32_t* d_counts, uint8_t* d_reasons)
 {
-    const int N = h->n_nodes, P = h->n_pods;
+    const int N = h->n_nodes, P = w.n_pods;
     if (n_failed == 0 || N == 0) return NHD_OK;
     ExplainArgs xa;
-    xa.snapshot = h->d_snapshot; xa.types = h->d_types; xa.pod_type = h->d_pod_type; xa.now = h->d_now; xa.out = h->d_out;
-    xa.pod_groups = h->n_names ? h->d_pod_groups : nullptr;
+    xa.snapshot = w.nodes; xa.types = w.types; xa.pod_type = w.pod_type; xa.now = w.now; xa.out = w.out;
+    xa.pod_groups = w.pod_groups;
     xa.node_start = h->d_xnode + N; xa.node_pods = h->d_xpod; xa.failed = h->d_xpod + P;
     xa.n_failed = (const int32_t*)h->d_xsmall;
     xa.n_nodes = N; xa.min_busy = h->params.min_busy_secs;
@@ -1030,21 +1098,28 @@ static int32_t explain_survivors(nhd_handle* h, const char* what)
     return NHD_OK;
 }
 
+/* per-reason node counts of every NO_CANDIDATE pod of the solve w into the host array counts (n_pods * NHD_WHY_COUNT) */
+static int32_t explain_counts(nhd_handle* h, const SolveWork& w, uint32_t* counts, const char* what)
+{
+    const size_t bytes = (size_t)w.n_pods * NHD_WHY_COUNT * 4;
+    if (bytes == 0) return NHD_OK;
+    int nf = 0;
+    int32_t rc;
+    if ((rc = explain_prepare(h, w, &nf)) != NHD_OK) return rc;
+    CK(grow_dev(h->d_xcounts, h->xcounts_cap, bytes));
+    CK(cudaMemsetAsync(h->d_xcounts, 0, bytes, h->stream));
+    if ((rc = explain_launch(h, w, nf, h->d_xcounts, nullptr)) != NHD_OK) return rc;
+    CK(cudaMemcpyAsync(counts, h->d_xcounts, bytes, cudaMemcpyDeviceToHost, h->stream));
+    return explain_survivors(h, what);
+}
+
 extern "C" int32_t nhd_explain_batch(nhd_handle* h, uint32_t* counts)
 {
     if (!h || (h->n_pods > 0 && !counts)) return NHD_ERR_INVALID;
     int32_t rc = explain_ready(h);
     if (rc != NHD_OK) return rc;
     CK(cudaSetDevice(h->params.device));
-    const size_t bytes = (size_t)h->n_pods * NHD_WHY_COUNT * 4;
-    if (bytes == 0) return NHD_OK;
-    int nf = 0;
-    if ((rc = explain_prepare(h, &nf)) != NHD_OK) return rc;
-    CK(grow_dev(h->d_xcounts, h->xcounts_cap, bytes));
-    CK(cudaMemsetAsync(h->d_xcounts, 0, bytes, h->stream));
-    if ((rc = explain_launch(h, nf, h->d_xcounts, nullptr)) != NHD_OK) return rc;
-    CK(cudaMemcpyAsync(counts, h->d_xcounts, bytes, cudaMemcpyDeviceToHost, h->stream));
-    return explain_survivors(h, "nhd_explain_batch");
+    return explain_counts(h, batch_work(h, h->d_snapshot), counts, "nhd_explain_batch");
 }
 
 extern "C" int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_reason)
@@ -1061,46 +1136,51 @@ extern "C" int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_rea
         memset(node_reason, NHD_WHY_NONE, (size_t)h->n_nodes);
         return NHD_OK;
     }
+    const SolveWork w = batch_work(h, h->d_snapshot);
     int nf = 0;
-    if ((rc = explain_prepare(h, &nf)) != NHD_OK) return rc;
+    if ((rc = explain_prepare(h, w, &nf)) != NHD_OK) return rc;
     const int32_t one[1] = {pod};                    /* explain just this pod: failed[0] = pod, n_failed = 1 */
     const int32_t n1 = 1;
     CK(cudaMemcpyAsync(h->d_xpod + h->n_pods, one, 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xsmall, &n1, 4, cudaMemcpyHostToDevice, h->stream));
     CK(grow_dev(h->d_xreasons, h->xreasons_cap, (size_t)h->n_nodes));
-    if ((rc = explain_launch(h, 1, nullptr, h->d_xreasons)) != NHD_OK) return rc;
+    if ((rc = explain_launch(h, w, 1, nullptr, h->d_xreasons)) != NHD_OK) return rc;
     CK(cudaMemcpyAsync(node_reason, h->d_xreasons, (size_t)h->n_nodes, cudaMemcpyDeviceToHost, h->stream));
     return explain_survivors(h, "nhd_explain_pod");
 }
 
-/* ------------------------------------------------------------------ placement queries */
+/* ------------------------------------------------------------------ placement queries and plans */
+
+/* the records a query or a plan reads: NHD_QUERY_MIRROR or NHD_QUERY_SNAPSHOT, the latter only while the hardware
+ * classes (d_class, d_cls_fast, d_sigs: the mirror's) describe it, i.e. no load or update since the snapshot */
+static int32_t source_records(nhd_handle* h, int32_t source, const char* what, uint8_t** records)
+{
+    if (source != NHD_QUERY_MIRROR && source != NHD_QUERY_SNAPSHOT)
+        return fail(h, NHD_ERR_INVALID, "%s source %d is neither NHD_QUERY_MIRROR nor NHD_QUERY_SNAPSHOT", what, source);
+    if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_%s_batch before nhd_load_nodes", what);
+    if (source == NHD_QUERY_SNAPSHOT && (!h->have_snapshot || h->snap_rec_gen != h->rec_gen))
+        return fail(h, NHD_ERR_STATE, "a snapshot %s needs nhd_snapshot with no nhd_load_nodes / nhd_update_nodes since", what);
+    *records = source == NHD_QUERY_SNAPSHOT ? h->d_snapshot : h->d_nodes;
+    return NHD_OK;
+}
 
 /*
- * Where each pod would go on its own, on the mirror or on the snapshot, with nothing written but the query's own
- * scratch: de-duplicate into pod types (as nhd_stage_batch), filter the whole cluster into the query's bitmaps and
- * summaries (fast_tables_kernel + filter_kernel, no sharding, no exchange), one warp per pod picks the node
- * (query_select_kernel), one thread per placed pod works out the mapping and the assignment (query_assign_kernel).
+ * A query's or a plan's pods: validated and de-duplicated into pod types as by nhd_stage_batch (tuple limits judged
+ * against max_numa), then copied into the query scratch with room for their filter output and bindings.  Fills the
+ * pod-set and filter fields of w (n_pods > 0); the sweep's own buffers are the plan's business.
  */
-extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods, const nhd_pod* pods, const double* now,
-                                   nhd_binding* out)
+static int32_t upload_pod_set(nhd_handle* h, int n_pods, const nhd_pod* pods, const double* now, int max_numa,
+                              SolveWork& w)
 {
-    if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now || !out))) return NHD_ERR_INVALID;
-    if (source != NHD_QUERY_MIRROR && source != NHD_QUERY_SNAPSHOT)
-        return fail(h, NHD_ERR_INVALID, "query source %d is neither NHD_QUERY_MIRROR nor NHD_QUERY_SNAPSHOT", source);
-    if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_query_batch before nhd_load_nodes");
-    if (source == NHD_QUERY_SNAPSHOT && (!h->have_snapshot || h->snap_rec_gen != h->rec_gen))
-        return fail(h, NHD_ERR_STATE, "a snapshot query needs nhd_snapshot with no nhd_load_nodes / nhd_update_nodes since");
     uint64_t names_used = 0;
     const bool multi_group = group_lists(n_pods, pods, &names_used);
     std::vector<PodType> types;
     std::vector<int32_t> pod_type;
-    int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, types, pod_type);
+    const int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, max_numa, types, pod_type);
     if (rc != NHD_OK) return rc;
-    if (n_pods == 0) return NHD_OK;
     CK(cudaSetDevice(h->params.device));
     const int T = (int)types.size(), W = h->words;
     const int n_names = multi_group ? __builtin_popcountll(names_used) : 0;
-    const uint8_t* nodes = source == NHD_QUERY_SNAPSHOT ? h->d_snapshot : h->d_nodes;
 
     /* host -> device: types | pod_type | now | group masks, one pinned buffer */
     const size_t types_bytes = (size_t)T * sizeof(PodType);
@@ -1115,53 +1195,29 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
         for (int i = 0; i < n_pods; i++) memcpy(hp + off_gm + (size_t)i * 8, &pods[i].group_mask, 8);
     CK(grow_dev(h->d_qtypes, h->qtypes_cap, types_bytes));
     CK(grow_dev(h->d_qpods, h->qpods_cap, pods_bytes));
-    CK(grow_dev(h->d_qout, h->qout_cap, (size_t)n_pods * sizeof(nhd_binding)));
+    CK(grow_dev(h->d_qout, h->qout_cap, ((size_t)n_pods + 8) * sizeof(nhd_binding)));
     CK(grow_dev(h->d_qbitmaps, h->qbitmaps_cap, (size_t)(T + 2 + n_names) * W * 8));
     CK(grow_dev(h->d_qdyn, h->qdyn_cap, (size_t)W * 64 * sizeof(NodeDyn)));
+    if (!h->d_qftab) CK(cudaMalloc((void**)&h->d_qftab, ftab_bytes(FAST_MAX_TYPES)));
     CK(cudaMemcpyAsync(h->d_qtypes, h->h_q, types_bytes, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_qpods, hp, pods_bytes, cudaMemcpyHostToDevice, h->stream));
 
-    /* the candidate bitmaps of the query's pod types on the chosen records */
-    const bool have_ftab = T <= FAST_MAX_TYPES;
-    if (have_ftab) {
-        if (!h->d_qftab) CK(cudaMalloc((void**)&h->d_qftab, ftab_bytes(FAST_MAX_TYPES)));
-        TablesArgs ta;
-        ta.types = h->d_qtypes; ta.n_types = T; ta.sigs = h->d_sigs; ta.out = h->d_qftab;
-        memcpy(ta.cap, h->cap, sizeof(ta.cap));
-        fast_tables_kernel<<<dim3(T, FAST_NSIG * 16 / 256), 256, 0, h->stream>>>(ta);
-        CK(cudaGetLastError());
-    }
-    FilterArgs fa;
-    fa.ftab = have_ftab ? h->d_qftab : nullptr; fa.mapt = h->d_mapt; fa.cls = h->d_cls_fast;
-    fa.nodes = nodes; fa.types = h->d_qtypes; fa.n_types = T; fa.n_nodes = h->n_nodes;
-    fa.super_lo = 0; fa.super_hi = h->n_super;
-    fa.dyn = h->d_qdyn; fa.bitmaps = h->d_qbitmaps; fa.words = W; fa.word_base = 0;
-    fa.class_id = h->d_class; fa.names_used = multi_group ? names_used : 0;
-    fa.now0 = now[0]; fa.min_busy = h->params.min_busy_secs;
-    memcpy(fa.cap, h->cap, sizeof(fa.cap));
-    fa.type_split = std::max(1, std::min(T, (h->sm_count * 2) / h->n_super));
-    const int fgrid = std::min(h->n_super, h->sm_count * 2) * fa.type_split;
-    const size_t fsmem = FILTER_STAGES * SUPER_BYTES + (T <= TYPES_SMEM_MAX ? (size_t)T * sizeof(PodType) : 0);
-    filter_kernel<<<fgrid, FILTER_THREADS, fsmem, h->stream>>>(fa);
-    CK(cudaGetLastError());
+    w.types = h->d_qtypes;
+    w.pod_type = reinterpret_cast<const int32_t*>(h->d_qpods + off_pt);
+    w.now = reinterpret_cast<const double*>(h->d_qpods + off_now);
+    w.pod_groups = multi_group ? reinterpret_cast<const uint64_t*>(h->d_qpods + off_gm) : nullptr;
+    w.n_pods = n_pods; w.n_types = T; w.n_names = n_names; w.names_used = multi_group ? names_used : 0;
+    w.now0 = now[0];
+    w.const_clock = true;
+    for (int i = 1; i < n_pods; i++) if (now[i] != now[0]) { w.const_clock = false; break; }
+    w.bitmaps = h->d_qbitmaps; w.dyn = h->d_qdyn; w.ftab = h->d_qftab; w.out = h->d_qout;
+    w.cursors = nullptr; w.busy_list = nullptr; w.pend = nullptr; w.prof = nullptr;
+    return NHD_OK;
+}
 
-    /* each pod on its own: the node, then the mapping and the assignment on a copy of its record */
-    QueryArgs qa;
-    qa.nodes = nodes; qa.types = h->d_qtypes;
-    qa.pod_type = reinterpret_cast<const int32_t*>(h->d_qpods + off_pt);
-    qa.now = reinterpret_cast<const double*>(h->d_qpods + off_now);
-    qa.bitmaps = h->d_qbitmaps;
-    qa.pod_groups = multi_group ? reinterpret_cast<const uint64_t*>(h->d_qpods + off_gm) : nullptr;
-    qa.names_used = multi_group ? names_used : 0;
-    qa.out = h->d_qout; qa.n_pods = n_pods; qa.n_types = T; qa.words = W;
-    qa.min_busy = h->params.min_busy_secs;
-    memcpy(qa.cap, h->cap, sizeof(qa.cap));
-    const int warps_per_cta = QUERY_SELECT_THREADS / 32;
-    query_select_kernel<<<(n_pods + warps_per_cta - 1) / warps_per_cta, QUERY_SELECT_THREADS, 0, h->stream>>>(qa);
-    CK(cudaGetLastError());
-    query_assign_kernel<<<(n_pods + 63) / 64, 64, 0, h->stream>>>(qa);
-    CK(cudaGetLastError());
-
+/* device -> host: the first n_pods bindings of the scratch, waiting for the device */
+static int32_t fetch_scratch_bindings(nhd_handle* h, int n_pods, nhd_binding* out)
+{
     const size_t out_bytes = (size_t)n_pods * sizeof(nhd_binding);
     const bool direct = is_pinned_host(out);
     if (!direct) CK(grow_pinned(h->h_qout, h->h_qout_cap, out_bytes));
@@ -1169,6 +1225,104 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
     CK(cudaStreamSynchronize(h->stream));
     if (!direct) memcpy(out, h->h_qout, out_bytes);
     return NHD_OK;
+}
+
+/*
+ * Where each pod would go on its own, on the mirror or on the snapshot, with nothing written but the query's own
+ * scratch: de-duplicate into pod types (as nhd_stage_batch), filter the whole cluster into the query's bitmaps and
+ * summaries (fast_tables_kernel + filter_kernel, no sharding, no exchange), one warp per pod picks the node
+ * (query_select_kernel), one thread per placed pod works out the mapping and the assignment (query_assign_kernel).
+ */
+extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods, const nhd_pod* pods, const double* now,
+                                   nhd_binding* out)
+{
+    if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now || !out))) return NHD_ERR_INVALID;
+    uint8_t* nodes = nullptr;
+    int32_t rc = source_records(h, source, "query", &nodes);
+    if (rc != NHD_OK) return rc;
+    if (n_pods == 0) return NHD_OK;
+    SolveWork w;
+    w.nodes = nodes;
+    if ((rc = upload_pod_set(h, n_pods, pods, now, h->max_numa, w)) != NHD_OK) return rc;
+
+    /* the candidate bitmaps of the query's pod types on the chosen records */
+    if ((rc = launch_solve(h, w, false, true)) != NHD_OK) return rc;
+
+    /* each pod on its own: the node, then the mapping and the assignment on a copy of its record */
+    QueryArgs qa;
+    qa.nodes = nodes; qa.types = w.types; qa.pod_type = w.pod_type; qa.now = w.now;
+    qa.bitmaps = w.bitmaps; qa.pod_groups = w.pod_groups; qa.names_used = w.names_used;
+    qa.out = w.out; qa.n_pods = n_pods; qa.n_types = w.n_types; qa.words = h->words;
+    qa.min_busy = h->params.min_busy_secs;
+    memcpy(qa.cap, h->cap, sizeof(qa.cap));
+    const int warps_per_cta = QUERY_SELECT_THREADS / 32;
+    query_select_kernel<<<(n_pods + warps_per_cta - 1) / warps_per_cta, QUERY_SELECT_THREADS, 0, h->stream>>>(qa);
+    CK(cudaGetLastError());
+    query_assign_kernel<<<(n_pods + 63) / 64, 64, 0, h->stream>>>(qa);
+    CK(cudaGetLastError());
+    return fetch_scratch_bindings(h, n_pods, out);
+}
+
+/*
+ * The bindings nhd_solve_batch would return on the chosen records with the excluded nodes in maintenance, and
+ * optionally nhd_explain_batch's counts after it, with nothing written but the plan's own scratch: the solve's own
+ * launches (launch_solve) on a workspace of the query scratch plus the plan's cursors, busy list and pend, without the
+ * commit and without sharding.  With exclusions the records are first copied into a plan-owned array and the excluded
+ * nodes flagged there (exclude_nodes_kernel); without, the source records are read in place.
+ */
+extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                                  int32_t n_pods, const nhd_pod* pods, const double* now, nhd_binding* out,
+                                  uint32_t* why_counts)
+{
+    if (!h || n_pods < 0 || n_excluded < 0 || (n_excluded > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)))
+        return NHD_ERR_INVALID;
+    uint8_t* records = nullptr;
+    int32_t rc = source_records(h, source, "plan", &records);
+    if (rc != NHD_OK) return rc;
+
+    /* the excluded nodes, each once; the tuple limits are judged as the equivalent solve would, on the largest NUMA
+     * count among the nodes the filter could accept once they are in maintenance */
+    std::vector<int32_t> ex;
+    int hist[NHD_MAX_NUMA + 1];
+    memcpy(hist, h->numa_hist, sizeof(hist));
+    {
+        std::vector<uint8_t> seen((size_t)h->n_nodes, 0);
+        for (int i = 0; i < n_excluded; i++) {
+            const int32_t n = excluded[i];
+            if (n < 0 || n >= h->n_nodes)
+                return fail(h, NHD_ERR_INVALID, "excluded node %d outside the %d loaded nodes", n, h->n_nodes);
+            if (seen[n]) continue;
+            seen[n] = 1;
+            ex.push_back(n);
+            hist[h->node_numa[n]]--;
+            hist[0]++;
+        }
+    }
+    int max_numa = 1;
+    for (int k = 2; k <= NHD_MAX_NUMA; k++) if (hist[k] > 0) max_numa = k;
+    if (n_pods == 0) return NHD_OK;
+    SolveWork w;
+    if ((rc = upload_pod_set(h, n_pods, pods, now, max_numa, w)) != NHD_OK) return rc;
+
+    const size_t n_slots = (size_t)h->n_super * SUPER_NODES;
+    CK(grow_dev(h->d_pcursors, h->pcursors_cap, (size_t)std::max(w.n_types, 1) * 3 * 4));
+    CK(grow_dev(h->d_pbusy, h->pbusy_cap, (n_slots + 64) * 4));
+    CK(grow_dev(h->d_ppend, h->ppend_cap, n_slots * 4));
+    if (!h->d_pprof) CK(cudaMalloc((void**)&h->d_pprof, 64 * 8));
+    w.cursors = h->d_pcursors; w.busy_list = h->d_pbusy; w.pend = h->d_ppend; w.prof = h->d_pprof;
+    w.nodes = records;
+    if (!ex.empty()) {
+        CK(grow_dev(h->d_pnodes, h->pnodes_cap, h->nodes_bytes));
+        CK(grow_dev(h->d_pidx, h->pidx_cap, ex.size() * 4));
+        CK(cudaMemcpyAsync(h->d_pnodes, records, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
+        CK(cudaMemcpyAsync(h->d_pidx, ex.data(), ex.size() * 4, cudaMemcpyHostToDevice, h->stream));
+        exclude_nodes_kernel<<<(unsigned)((ex.size() + 255) / 256), 256, 0, h->stream>>>(h->d_pnodes, h->d_pidx, (int)ex.size());
+        CK(cudaGetLastError());
+        w.nodes = h->d_pnodes;
+    }
+    if ((rc = launch_solve(h, w, false, false)) != NHD_OK) return rc;
+    if (why_counts && (rc = explain_counts(h, w, why_counts, "nhd_plan_batch")) != NHD_OK) return rc;
+    return fetch_scratch_bindings(h, n_pods, out);
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

@@ -21,8 +21,8 @@
  *   assign_cores_kernel   Node.GetFreeCpuBatch (nhd/Node.py:502-519) for every placed pod, in
  *                   parallel, from the snapshot core masks and per-socket prefix offsets
  *   commit_kernel   folds the batch into the node records
- * Outside a solve: explain_* (why a pod found no node) and query_select / query_assign_kernel (where each pod
- * of a query would go on its own, nhd_query_batch).
+ * Outside a solve: explain_* (why a pod found no node), query_select / query_assign_kernel (where each pod
+ * of a query would go on its own, nhd_query_batch) and exclude_nodes_kernel (a plan's excluded nodes, nhd_plan_batch).
  *
  * Device layout of the node array ("tiled AoSoA"): tiles of 32 nodes, 4 KB each:
  *     byte offset(node n, 16-byte chunk c) = (n / 32) * 4096 + c * 512 + (n % 32) * 16
@@ -2722,6 +2722,22 @@ __global__ void query_assign_kernel(const __grid_constant__ QueryArgs a)
         bu.b.n_groups = t.G;
     }
     for (int c = 0; c < 8; c++) reinterpret_cast<uint4*>(&a.out[i])[c] = bu.q[c];
+}
+
+/* ------------------------------------------------------------------ plans (nhd_plan_batch) */
+
+/* byte offset of nhd_node_rec.flags inside chunk 2 (the record's bytes 32..47) */
+constexpr int REC_FLAGS_BYTE = 13;
+
+/* A plan's excluded nodes, on the plan's own copy of the records: NHD_NODE_MAINTENANCE set, as the reference's
+ * maintenance event does (Matcher.py:73).  The flag is not part of a node's hardware class (static_key takes only the
+ * SMT bit of the flags byte), so the mirror's d_class / d_cls_fast / d_sigs describe the copy as well; the filter reads
+ * the flag from the record on every path (node_gates, node_feasible_k2, node_feasible). */
+__global__ void exclude_nodes_kernel(uint8_t* nodes, const int32_t* __restrict__ idx, int n)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n) return;
+    nodes[chunk_off(idx[i], 2) + REC_FLAGS_BYTE] |= (uint8_t)NHD_NODE_MAINTENANCE;
 }
 
 } // namespace nhd

@@ -199,6 +199,27 @@ class Solver:
         self._ck(self._L.nhd_query_batch(self._h, src, len(pods), pods.ctypes.data, now.ctypes.data, out.ctypes.data))
         return out
 
+    def plan_batch(self, pods, now, source='mirror', exclude=(), explain=False, out=None):
+        """A dry run of ``solve_batch`` (``nhd_plan_batch``): the bindings the pods would get scheduled in order, each
+        seeing the ones before it, on the current records (``source='mirror'``) or on those of the last ``snapshot()``
+        (``'snapshot'``), with the node indices ``exclude`` taken as in maintenance.  With ``explain=True`` returns
+        ``(bindings, counts)``, counts being what ``explain_batch`` would return after that solve.  Nothing is placed:
+        records, snapshot, the last batch and its explanations stay as they are."""
+        src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
+        if src is None:
+            raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
+        pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
+        now = np.ascontiguousarray(now, dtype='<f8')
+        assert len(pods) == len(now)
+        ex = np.ascontiguousarray(exclude, dtype='<i4').reshape(-1)
+        if out is None:
+            out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
+        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
+        self._ck(self._L.nhd_plan_batch(self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods),
+                                        pods.ctypes.data, now.ctypes.data, out.ctypes.data,
+                                        counts.ctypes.data if explain else None))
+        return (out, counts) if explain else out
+
     def filter_bitmaps(self):
         """Runs only the snapshot predicate kernel on the staged batch; returns
         (feas[type, node] bool, nogpu[node], busy[node], pod_type[pod])."""
