@@ -321,6 +321,34 @@ int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_excluded, const 
                        int32_t n_pods, const nhd_pod* pods, const double* now,
                        nhd_binding* out, uint32_t* why_counts);
 
+/*
+ * Many independent dry runs in one call: "which of these nodes (or racks) could be taken down, each on its own?".
+ * Scenario s excludes excluded[excl_start[s] .. excl_start[s+1]) and plans pods[pod_start[s] .. pod_start[s+1]) with
+ * now[] of the same rows; both offset arrays hold n_scenarios + 1 entries, start at 0 and never go down.
+ *   out[pod_start[s] .. pod_start[s+1])  when scenario_status[s] == NHD_OK: byte for byte what
+ *                  nhd_plan_batch(h, source, n_excl_s, excl_s, n_pods_s, pods_s, now_s, out_s, NULL) would return.
+ *                  Scenarios do not see each other; the pods inside one see the earlier ones, in order.
+ *   scenario_status[s], scenario_pod[s]  NHD_OK and -1, or the refusal nhd_plan_batch would give that scenario
+ *                  (NHD_ERR_INVALID / NHD_ERR_UNSUPPORTED: a descriptor nhd_validate_pod rejects, a non-finite clock,
+ *                  the tuple limits) and the index inside the scenario of the pod it names.  The out rows of a refused
+ *                  scenario are not written.
+ * source is NHD_QUERY_MIRROR or NHD_QUERY_SNAPSHOT, under the same rule as nhd_query_batch.  Unlike nhd_plan_batch the
+ * tuple limits are judged against every schedulable node of the cluster, the excluded ones included: one filter on the
+ * unchanged records serves every scenario, and it enumerates the NUMA tuples of the excluded nodes too.  Exclusions can
+ * only lower the largest NUMA count, so this refuses only scenarios that nhd_plan_batch accepts because of their
+ * exclusions; plan such a scenario with nhd_plan_batch.
+ * Malformed arguments make the whole call NHD_ERR_INVALID: a null pointer, offsets that do not start at 0 or go down,
+ * an excluded index outside [0, n_nodes); a duplicate exclusion counts once.  Nothing is written that a caller can
+ * observe (the same list as nhd_plan_batch), no collective is entered (any rank may call alone), and the call waits
+ * for the device before returning.  Explanations are not part of it: nhd_plan_batch gives a scenario's why_counts.
+ * Meant for many small scenarios (the pods of one node or one rack): one warp runs each, and a pod's cost grows with
+ * the number of nodes its scenario's earlier pods reached.  A large single batch belongs to nhd_plan_batch.
+ */
+int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                           const int32_t* excl_start, const int32_t* excluded,
+                           const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                           nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

@@ -232,6 +232,27 @@ class DeviceCluster:
         nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
         return fn(self._pods(tops, pod_groups, packed), nows, source=source, exclude=idx, explain=explain)
 
+    def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror'):
+        """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
+        of ``(exclude, tops, pod_groups, now[, packed])`` with ``exclude`` node names.  Returns one ``(code, pod,
+        bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None when the scenario is refused, ``code``
+        and ``pod`` saying why and for which of its pods.  None when the solver in use cannot plan scenarios (a stand-in
+        without ``plan_scenarios``)."""
+        fn = getattr(self._solver, 'plan_scenarios', None)
+        if fn is None:
+            return None
+        missing = sorted({n for sc in scenarios for n in sc[0] if n not in self._index})
+        if missing:
+            raise ValueError(f'cannot exclude unknown node(s) {missing}')
+        args = []
+        for sc in scenarios:
+            exclude, tops, pod_groups, now = sc[:4]
+            packed = sc[4] if len(sc) > 4 else None
+            idx = np.asarray([self._index[n] for n in exclude], dtype='<i4')
+            nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
+            args.append((idx, self._pods(tops, pod_groups, packed), nows))
+        return fn(args, source=source)
+
     def rewind(self, k: int):
         """Put the device back to the state right after pod ``k`` of the last batch (restore the
         snapshot taken before it, solve pods ``0..k`` again: the solver is deterministic)."""
@@ -690,18 +711,74 @@ class NHDScheduler:
         keys = [(ns, pod) for n in names for (pod, ns) in self.nodes[n].pod_info]
         return self._plan(keys, names)
 
+    def PlanDrains(self, node_groups: Sequence[Sequence[str]] = None) -> Dict:
+        """Which nodes (or groups of nodes) could be taken down, each group on its own?  ``{tuple(group): placement}``
+        with ``placement`` what ``PlanDrain(list(group))[0]`` returns from the same state; by default every node that
+        holds pods is its own group, in node order.  All groups are planned side by side in one GPU call; the groups
+        do not see each other.  Each pod is read from Kubernetes once, as a scheduling attempt reads it: no event, no
+        write; ``pod_state``, the ``Node`` objects and the counters stay as they are.  Reasons are not returned:
+        ``PlanDrain(group)`` gives them for the groups that do not drain."""
+        if node_groups is None:
+            node_groups = [[n] for n, v in self.nodes.items() if v.pod_info]
+        groups = [tuple(g) for g in node_groups]
+        missing = sorted({n for g in groups for n in g if n not in self.nodes})
+        if missing:
+            raise ValueError(f'unknown node(s) {missing}')
+        prepared = {}
+        group_entries = []
+        for g in groups:
+            entries = []
+            for n in g:
+                for (pod, ns) in self.nodes[n].pod_info:
+                    if (ns, pod) not in prepared:
+                        e = _Pending(len(prepared), (ns, pod))
+                        self._prepare(e, events=False)
+                        prepared[(ns, pod)] = e
+                    entries.append(prepared[(ns, pod)])
+            group_entries.append(entries)
+        result = {}
+        todo = []
+        for g, entries in zip(groups, group_entries):
+            result[g] = {(e.key[0], e.key[1]): None for e in entries}
+            ok = [e for e in entries if e.top is not None and e.unsupported is None]
+            if ok and self.nodes:
+                todo.append((g, entries, ok))
+        if not todo:
+            return result
+        self.cluster.sync(self.nodes, self._dirty)
+        self._dirty.clear()
+        now = float(self._clock())
+        res = self.cluster.plan_scenarios([(g, [e.top for e in ok], [e.groups for e in ok], now, [e.rec for e in ok])
+                                           for g, _, ok in todo])
+        if res is None:
+            raise RuntimeError('the solver in use cannot plan scenarios (no plan_scenarios)')
+        for (g, entries, ok), (code, _, out) in zip(todo, res):
+            if out is None:
+                # refused (the tuple limits are judged with the group's own nodes counted): the single plan judges
+                # them without, and drops a pod beyond them, or raises, as PlanDrain does
+                result[g] = self._plan_prepared(entries, list(g), now)[0]
+                continue
+            for e, b in zip(ok, out):
+                if int(b['status']) == wire.PLACED:
+                    result[g][(e.key[0], e.key[1])] = self.cluster.name_of(int(b['node']))
+        return result
+
     def _plan(self, keys: Sequence, exclude: Sequence[str]):
         entries = [_Pending(i, k) for i, k in enumerate(keys)]
         for e in entries:
             self._prepare(e, events=False)
+        ok = [e for e in entries if e.top is not None and e.unsupported is None]
+        if not ok or not self.nodes:
+            return {(e.key[0], e.key[1]): None for e in entries}, {}
+        self.cluster.sync(self.nodes, self._dirty)
+        self._dirty.clear()
+        return self._plan_prepared(entries, exclude, float(self._clock()))
+
+    def _plan_prepared(self, entries: Sequence, exclude: Sequence[str], now: float):
+        """``_plan`` from pods already read from Kubernetes, on the synced cluster at clock ``now``."""
         placement = {(e.key[0], e.key[1]): None for e in entries}
         reasons = {}
         ok = [e for e in entries if e.top is not None and e.unsupported is None]
-        if not ok or not self.nodes:
-            return placement, reasons
-        self.cluster.sync(self.nodes, self._dirty)
-        self._dirty.clear()
-        now = float(self._clock())
         while ok:
             try:
                 res = self.cluster.plan([e.top for e in ok], [e.groups for e in ok], now, exclude=exclude,

@@ -153,6 +153,10 @@ struct nhd_handle {
     unsigned long long* d_pprof = nullptr;
     uint8_t* d_pnodes = nullptr;    size_t pnodes_cap = 0;
     int32_t* d_pidx = nullptr;      size_t pidx_cap = 0;
+    /* scenario scratch (nhd_plan_scenarios), on top of the query's: pod offsets | exclusion offsets | exclusions |
+     * slot nodes | the failed-mapping word, and one working record per pod */
+    int32_t* d_sidx = nullptr;      size_t sidx_cap = 0;
+    uint4* d_swork = nullptr;       size_t swork_cap = 0;
 
     nhd_timing timing;
     std::string err;
@@ -341,6 +345,7 @@ extern "C" int32_t nhd_destroy(nhd_handle* h)
     cudaFree(h->d_xnode); cudaFree(h->d_xpod); cudaFree(h->d_xcounts); cudaFree(h->d_xreasons); cudaFree(h->d_xsmall);
     cudaFree(h->d_qtypes); cudaFree(h->d_qpods); cudaFree(h->d_qout); cudaFree(h->d_qbitmaps); cudaFree(h->d_qdyn); cudaFree(h->d_qftab);
     cudaFree(h->d_pcursors); cudaFree(h->d_pbusy); cudaFree(h->d_ppend); cudaFree(h->d_pprof); cudaFree(h->d_pnodes); cudaFree(h->d_pidx);
+    cudaFree(h->d_sidx); cudaFree(h->d_swork);
     if (h->h_q) cudaFreeHost(h->h_q);
     if (h->h_qout) cudaFreeHost(h->h_qout);
     if (h->h_stage) cudaFreeHost(h->h_stage);
@@ -642,6 +647,19 @@ static bool group_lists(int n_pods, const nhd_pod* pods, uint64_t* names_used)
     return multi_group;
 }
 
+/* The staging checks of one pod, in order: the descriptor (nhd_validate_pod), a finite clock, the tuple limits against
+ * max_numa.  The refusal names the pod as index i; h may be null (the code alone). */
+static int32_t check_pod(nhd_handle* h, int i, const nhd_pod& p, double now, int max_numa)
+{
+    const int32_t v = nhd_validate_pod(&p);
+    if (v != NHD_OK) return fail(h, v, "pod %d: descriptor rejected by nhd_validate_pod", i);
+    if (!std::isfinite(now)) return fail(h, NHD_ERR_INVALID, "pod %d: non-finite clock", i);
+    if (!tuple_limits_ok(max_numa, p.n_groups))
+        return fail(h, NHD_ERR_UNSUPPORTED, "pod %d: %d groups on %d-NUMA nodes exceeds the tuple limits", i,
+                    (int)p.n_groups, max_numa);
+    return NHD_OK;
+}
+
 /* Validate the pods and de-duplicate them into pod types (distinct descriptors: the reference re-derives everything
  * per pod): types[] and pod_type[i].  Refusals name the pod; the tuple limits are judged against max_numa.  Touches
  * nothing of the handle but its error text. */
@@ -669,12 +687,8 @@ static int32_t make_pod_types(nhd_handle* h, int n_pods, const nhd_pod* pods, co
             pod_type[i] = rs.type;
             continue;
         }
-        int32_t v = nhd_validate_pod(&pods[i]);
-        if (v != NHD_OK) return fail(h, v, "pod %d: descriptor rejected by nhd_validate_pod", i);
-        if (!std::isfinite(now[i])) return fail(h, NHD_ERR_INVALID, "pod %d: non-finite clock", i);
-        if (!tuple_limits_ok(max_numa, pods[i].n_groups))
-            return fail(h, NHD_ERR_UNSUPPORTED, "pod %d: %d groups on %d-NUMA nodes exceeds the tuple limits", i,
-                        (int)pods[i].n_groups, max_numa);
+        const int32_t v = check_pod(h, i, pods[i], now[i], max_numa);
+        if (v != NHD_OK) return v;
         PodKey k{canonical_pod(pods[i])};
         if (multi_group) k.p.group_mask = ~0ULL;
         auto it = index.find(k);
@@ -1323,6 +1337,109 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
     if ((rc = launch_solve(h, w, false, false)) != NHD_OK) return rc;
     if (why_counts && (rc = explain_counts(h, w, why_counts, "nhd_plan_batch")) != NHD_OK) return rc;
     return fetch_scratch_bindings(h, n_pods, out);
+}
+
+/*
+ * Many independent plans at once, each on the source records with its own excluded nodes: every scenario's pods are
+ * checked as nhd_stage_batch checks them (a refusal refuses that scenario only), the pods of the accepted scenarios are
+ * de-duplicated into one pod set and filtered once on the unchanged source records (launch_solve's tables + filter, as
+ * a query), then one warp per scenario walks its pods in order (scenario_plan_kernel).  The tuple limits are judged
+ * against the whole cluster's NUMA counts: the shared filter enumerates the tuples of every node, the excluded ones
+ * included.
+ */
+extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_scenarios, const int32_t* excl_start,
+                                      const int32_t* excluded, const int32_t* pod_start, const nhd_pod* pods,
+                                      const double* now, nhd_binding* out, int32_t* scenario_status,
+                                      int32_t* scenario_pod)
+{
+    if (!h || n_scenarios < 0 || !excl_start || !pod_start || (n_scenarios > 0 && (!scenario_status || !scenario_pod)))
+        return NHD_ERR_INVALID;
+    if (excl_start[0] != 0 || pod_start[0] != 0) return fail(h, NHD_ERR_INVALID, "scenario offsets must start at 0");
+    for (int s = 0; s < n_scenarios; s++)
+        if (excl_start[s + 1] < excl_start[s] || pod_start[s + 1] < pod_start[s])
+            return fail(h, NHD_ERR_INVALID, "scenario %d: offsets go down", s);
+    const int n_excl = excl_start[n_scenarios], n_pods = pod_start[n_scenarios];
+    if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out))) return NHD_ERR_INVALID;
+    uint8_t* records = nullptr;
+    int32_t rc = source_records(h, source, "plan", &records);
+    if (rc != NHD_OK) return rc;
+    for (int e = 0; e < n_excl; e++)
+        if (excluded[e] < 0 || excluded[e] >= h->n_nodes)
+            return fail(h, NHD_ERR_INVALID, "excluded node %d outside the %d loaded nodes", excluded[e], h->n_nodes);
+
+    /* per scenario: its refusal, or its place among the accepted ones (pods and exclusions compacted, the exclusions
+     * sorted and each once).  idx = pod offsets | exclusion offsets | exclusions of the accepted scenarios. */
+    std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex;
+    for (int s = 0; s < n_scenarios; s++) {
+        scenario_status[s] = NHD_OK;
+        scenario_pod[s] = -1;
+        for (int i = pod_start[s]; i < pod_start[s + 1]; i++) {
+            const int32_t v = check_pod(nullptr, i - pod_start[s], pods[i], now[i], h->max_numa);
+            if (v != NHD_OK) { scenario_status[s] = v; scenario_pod[s] = i - pod_start[s]; break; }
+        }
+        if (scenario_status[s] != NHD_OK) continue;
+        acc.push_back(s);
+        pod_off.push_back(pod_off.back() + pod_start[s + 1] - pod_start[s]);
+        const size_t e0 = ex.size();
+        ex.insert(ex.end(), excluded + excl_start[s], excluded + excl_start[s + 1]);
+        std::sort(ex.begin() + e0, ex.end());
+        ex.erase(std::unique(ex.begin() + e0, ex.end()), ex.end());
+        ex_off.push_back((int32_t)ex.size());
+    }
+    const int n_acc = (int)acc.size(), n_run = pod_off.back();
+    if (n_run == 0) return NHD_OK;
+    const bool compact = n_run != n_pods;
+    std::vector<nhd_pod> cpods;
+    std::vector<double> cnow;
+    if (compact) {
+        cpods.reserve(n_run);
+        cnow.reserve(n_run);
+        for (int s : acc) {
+            cpods.insert(cpods.end(), pods + pod_start[s], pods + pod_start[s + 1]);
+            cnow.insert(cnow.end(), now + pod_start[s], now + pod_start[s + 1]);
+        }
+    }
+    SolveWork w;
+    w.nodes = records;
+    if ((rc = upload_pod_set(h, n_run, compact ? cpods.data() : pods, compact ? cnow.data() : now, h->max_numa, w)) != NHD_OK)
+        return rc;
+
+    std::vector<int32_t> idx;
+    idx.reserve(pod_off.size() + ex_off.size() + ex.size());
+    idx.insert(idx.end(), pod_off.begin(), pod_off.end());
+    idx.insert(idx.end(), ex_off.begin(), ex_off.end());
+    idx.insert(idx.end(), ex.begin(), ex.end());
+    const size_t off_nodes = idx.size(), off_bad = off_nodes + (size_t)n_run;
+    CK(grow_dev(h->d_sidx, h->sidx_cap, (off_bad + 1) * 4));
+    CK(grow_dev(h->d_swork, h->swork_cap, (size_t)n_run * sizeof(nhd_node_rec)));
+    CK(cudaMemcpyAsync(h->d_sidx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemsetAsync(h->d_sidx + off_bad, 0, 4, h->stream));
+
+    /* the candidate bitmaps of the call's pod types on the unchanged source records */
+    if ((rc = launch_solve(h, w, false, true)) != NHD_OK) return rc;
+
+    ScenarioArgs sa;
+    sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type; sa.now = w.now;
+    sa.bitmaps = w.bitmaps; sa.pod_groups = w.pod_groups; sa.names_used = w.names_used;
+    sa.pod_start = h->d_sidx; sa.excl_start = h->d_sidx + pod_off.size(); sa.excl = sa.excl_start + ex_off.size();
+    sa.work = h->d_swork; sa.work_node = h->d_sidx + off_nodes; sa.out = w.out; sa.bad = (uint32_t*)(h->d_sidx + off_bad);
+    sa.n_scenarios = n_acc; sa.n_types = w.n_types; sa.words = h->words;
+    sa.min_busy = h->params.min_busy_secs;
+    memcpy(sa.cap, h->cap, sizeof(sa.cap));
+    const int warps_per_cta = SCENARIO_THREADS / 32;
+    const int grid = std::min((n_acc + warps_per_cta - 1) / warps_per_cta, h->sm_count * 16);
+    scenario_plan_kernel<<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
+    CK(cudaGetLastError());
+    uint32_t bad = 0;
+    CK(cudaMemcpyAsync(&bad, h->d_sidx + off_bad, 4, cudaMemcpyDeviceToHost, h->stream));
+    std::vector<nhd_binding> run;
+    if (compact) run.resize(n_run);
+    if ((rc = fetch_scratch_bindings(h, n_run, compact ? run.data() : out)) != NHD_OK) return rc;
+    if (bad) return fail(h, NHD_ERR_STATE, "nhd_plan_scenarios: %u chosen nodes without a mapping", bad);
+    if (compact)
+        for (int k = 0; k < n_acc; k++)
+            memcpy(out + pod_start[acc[k]], run.data() + pod_off[k], (size_t)(pod_off[k + 1] - pod_off[k]) * sizeof(nhd_binding));
+    return NHD_OK;
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

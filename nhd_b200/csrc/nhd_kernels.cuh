@@ -22,7 +22,8 @@
  *                   parallel, from the snapshot core masks and per-socket prefix offsets
  *   commit_kernel   folds the batch into the node records
  * Outside a solve: explain_* (why a pod found no node), query_select / query_assign_kernel (where each pod
- * of a query would go on its own, nhd_query_batch) and exclude_nodes_kernel (a plan's excluded nodes, nhd_plan_batch).
+ * of a query would go on its own, nhd_query_batch), exclude_nodes_kernel (a plan's excluded nodes, nhd_plan_batch)
+ * and scenario_plan_kernel (many independent small plans side by side, nhd_plan_scenarios).
  *
  * Device layout of the node array ("tiled AoSoA"): tiles of 32 nodes, 4 KB each:
  *     byte offset(node n, 16-byte chunk c) = (n / 32) * 4096 + c * 512 + (n % 32) * 16
@@ -2738,6 +2739,163 @@ __global__ void exclude_nodes_kernel(uint8_t* nodes, const int32_t* __restrict__
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     nodes[chunk_off(idx[i], 2) + REC_FLAGS_BYTE] |= (uint8_t)NHD_NODE_MAINTENANCE;
+}
+
+/* ------------------------------------------------------------------ independent plans (nhd_plan_scenarios) */
+
+/*
+ * Not part of a solve: many small plans at once, each on the source records with its own nodes in maintenance.  One
+ * filter of the call's pod types on the unchanged source records serves every scenario, because a scenario's records
+ * differ from them only at its excluded nodes (dropped by the maintenance stage, skipped here) and at the nodes its own
+ * earlier pods reached (its touched set, evaluated on working records).  On an untouched node F[type] is FindNode's
+ * candidate set apart from the busy window, as for a query.  So for pod i the first node of
+ *     (untouched, not excluded, F[type], node-group gate, not busy for a GPU pod)  U  (touched, passes every stage)
+ * is the reference's SelectNode at that pod.  One warp per scenario, its pods in order.
+ */
+struct ScenarioArgs {
+    const uint8_t* nodes;          /* the source records (mirror or snapshot, tiled layout), only read */
+    const PodType* types;
+    const int32_t* pod_type;
+    const double* now;
+    const uint64_t* bitmaps;       /* [n_types + 2 + n_names][words]: F[0..T), NOGPU, BUSY (unused), per group name */
+    const uint64_t* pod_groups;    /* per-pod node-group lists of a call that mixes them, else null */
+    uint64_t names_used;
+    const int32_t* pod_start;      /* [n_scenarios + 1]: scenario s owns pods pod_start[s] .. pod_start[s + 1] */
+    const int32_t* excl_start;     /* [n_scenarios + 1] into excl */
+    const int32_t* excl;           /* each scenario's excluded nodes, sorted, without duplicates */
+    uint4* work;                   /* [n_pods][8]: slot pod_start[s] + k = working record of scenario s's k-th touched node */
+    int32_t* work_node;            /* [n_pods]: the node of each slot */
+    nhd_binding* out;
+    uint32_t* bad;                 /* chosen nodes on which no mapping was found: never expected, refused by the host */
+    int n_scenarios, n_types, words;
+    double min_busy;
+    double cap[NHD_MAX_SPEED_CLASSES];
+};
+
+constexpr int SCENARIO_THREADS = 128;
+
+__device__ __forceinline__ bool sorted_contains(const int32_t* v, int n, int x)
+{
+    int lo = 0, hi = n;
+    while (lo < hi) {
+        const int mid = (lo + hi) >> 1;
+        if (v[mid] < x) lo = mid + 1; else hi = mid;
+    }
+    return lo < n && v[lo] == x;
+}
+
+/* One warp per scenario (grid-stride).  For each pod: the first touched node that passes every stage on its working
+ * record (explain_node, lanes over the touched set, warp minimum) and the first untouched candidate (query_select_kernel's
+ * ballot scan, skipping excluded and touched nodes), GPU-less pass first for a pod without GPUs (Matcher.py:412-421);
+ * then lane 0 runs the mapping and the assignment (query_assign_kernel's body) on that node's working record, keeps
+ * the result as the node's working record and writes the binding. */
+__global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const __grid_constant__ ScenarioArgs a)
+{
+    const int lane = threadIdx.x & 31, W = a.words;
+    const int n_warps = (int)((gridDim.x * (unsigned)SCENARIO_THREADS) >> 5);
+    const uint64_t* NOGPU = a.bitmaps + (size_t)a.n_types * W;
+    const uint64_t* GB = a.bitmaps + (size_t)(a.n_types + 2) * W;
+    for (int s = (int)((blockIdx.x * (unsigned)SCENARIO_THREADS + threadIdx.x) >> 5); s < a.n_scenarios; s += n_warps) {
+        const int p0 = a.pod_start[s], p1 = a.pod_start[s + 1];
+        const int32_t* ex = a.excl + a.excl_start[s];
+        const int n_ex = a.excl_start[s + 1] - a.excl_start[s];
+        uint4* work = a.work + (size_t)p0 * REC_CHUNKS;
+        int32_t* work_node = a.work_node + p0;
+        int n_touched = 0;
+        for (int i = p0; i < p1; i++) {
+            const int ti = a.pod_type[i];
+            const PodType& t = a.types[ti];
+            uint4* bout = reinterpret_cast<uint4*>(&a.out[i]);
+            if (!t.valid_map) {                                        /* Matcher.py:45-47 */
+                if (lane < 8) bout[lane] = make_uint4(lane == 0 ? NHD_BAD_MAP_TYPE : 0, lane == 0 ? 0xFFFFFFFFu : 0, lane == 0 ? t.G : 0, 0);
+                continue;
+            }
+            const uint64_t* F = a.bitmaps + (size_t)ti * W;
+            const uint64_t gm = a.pod_groups ? a.pod_groups[i] : 0;
+            const double now = a.now[i];
+            int chosen = -1, slot = -1;
+            for (int pass = t.needs_gpu ? 1 : 0; pass < 2 && chosen < 0; pass++) {
+                /* the first touched node that passes FindNode's stages on its working record */
+                int best = 0x7FFFFFFF, best_k = -1;
+                for (int k = lane; k < n_touched; k += 32) {
+                    RecU u;
+#pragma unroll
+                    for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)k * REC_CHUNKS + c];
+                    const int node = work_node[k];
+                    if (node < best && (pass == 1 || u.r.n_gpus == 0) &&
+                        explain_node(u.r, t, a.pod_groups ? gm : t.pod.group_mask, now, a.min_busy, a.cap) == NHD_WHY_COUNT) {
+                        best = node;
+                        best_k = k;
+                    }
+                }
+                for (int o = 16; o; o >>= 1) {
+                    const int ob = __shfl_sync(0xFFFFFFFFu, best, lane ^ o), ok = __shfl_sync(0xFFFFFFFFu, best_k, lane ^ o);
+                    if (ob < best) { best = ob; best_k = ok; }
+                }
+                /* the first untouched candidate, only where it can come before that node */
+                int first = -1;
+                for (int base = 0; base < W && first < 0 && (long long)base * 64 < best; base += 32) {
+                    const int w = base + lane;
+                    int mine = -1;
+                    if (w < W) {
+                        uint64_t word = F[w] & (pass == 0 ? NOGPU[w] : ~0ULL);
+                        if (a.pod_groups && word) {                    /* InitialNodeFilter per group name (NHDScheduler.py:241) */
+                            uint64_t e = 0;
+                            for (uint64_t g = gm; g; g &= g - 1)
+                                e |= GB[(size_t)popc64(a.names_used & ((1ULL << ctz64(g)) - 1)) * W + w];
+                            word &= e;
+                        }
+                        for (; word; word &= word - 1) {
+                            const int node = w * 64 + ctz64(word);
+                            if (node >= best) break;
+                            if (sorted_contains(ex, n_ex, node)) continue;
+                            bool touched = false;
+                            for (int k = 0; k < n_touched && !touched; k++) touched = work_node[k] == node;
+                            if (touched) continue;
+                            if (t.needs_gpu) {
+                                nhd_node_rec r;
+                                r.busy_time = *reinterpret_cast<const double*>(a.nodes + chunk_off(node, 3));
+                                if (node_busy(r, now, a.min_busy)) continue;
+                            }
+                            mine = node;
+                            break;
+                        }
+                    }
+                    const unsigned m = __ballot_sync(0xFFFFFFFFu, mine >= 0);
+                    if (m) first = __shfl_sync(0xFFFFFFFFu, mine, ctz32(m));
+                }
+                if (first >= 0) { chosen = first; slot = n_touched; }
+                else if (best_k >= 0) { chosen = best; slot = best_k; }
+            }
+            if (lane == 0) {
+                union { nhd_binding b; uint4 q[8]; } bu;
+                for (int c = 0; c < 8; c++) bu.q[c] = make_uint4(0, 0, 0, 0);
+                if (chosen < 0) {
+                    bu.q[0] = make_uint4(NHD_NO_CANDIDATE, 0xFFFFFFFFu, t.G, 0);
+                } else {
+                    RecU u;
+                    if (slot < n_touched) {
+                        for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)slot * REC_CHUNKS + c];
+                    } else {
+                        load_rec(a.nodes, chosen, u);
+                    }
+                    Mapping m;
+                    if (evaluate_mapping(u.r, t, a.cap, &m)) {
+                        bu.b.node = chosen;
+                        assign_pod(u.r, t, m, now, &bu.b);             /* the reference's unwind on a failed assignment */
+                    } else {
+                        atomicAdd(a.bad, 1u);                          /* the candidate test said feasible */
+                        bu.q[0] = make_uint4(NHD_NO_CANDIDATE, 0xFFFFFFFFu, t.G, 0);
+                    }
+                    for (int c = 0; c < REC_CHUNKS; c++) work[(size_t)slot * REC_CHUNKS + c] = u.q[c];
+                    work_node[slot] = chosen;
+                }
+                for (int c = 0; c < 8; c++) bout[c] = bu.q[c];
+            }
+            if (chosen >= 0 && slot == n_touched) n_touched++;
+            __syncwarp();                                              /* the slot is read by every lane from here on */
+        }
+    }
 }
 
 } // namespace nhd

@@ -220,6 +220,46 @@ class Solver:
                                         counts.ctypes.data if explain else None))
         return (out, counts) if explain else out
 
+    def plan_scenarios(self, scenarios, source='mirror'):
+        """Many independent dry runs in one call (``nhd_plan_scenarios``).  ``scenarios``: a sequence of
+        ``(exclude, pods, now)``.  Returns one ``(code, pod, bindings)`` per scenario: ``code`` 0 and ``bindings`` what
+        ``plan_batch(pods, now, source, exclude)`` returns, or the refusal ``plan_batch`` would raise (``wire.ERR_*``),
+        the index of the pod it names and None.  Scenarios do not see each other.  Unlike ``plan_batch`` the tuple
+        limits are judged with the excluded nodes counted; ``plan_batch`` plans a scenario refused for that."""
+        src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
+        if src is None:
+            raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
+        # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
+        # would cost more than the call itself)
+        exs, podb, nowl = [], [], []
+        for exclude, pods, now in scenarios:
+            pods = np.asarray(pods)
+            if pods.dtype != wire.POD_DTYPE:
+                pods = pods.astype(wire.POD_DTYPE)
+            exs.append(np.asarray(exclude, dtype='<i4').reshape(-1))
+            podb.append(np.ascontiguousarray(pods).tobytes())
+            nowl.append(np.asarray(now, dtype='<f8').reshape(-1))
+            assert pods.size == len(nowl[-1])
+        n = len(podb)
+        excl_start = np.zeros(n + 1, dtype='<i4')
+        pod_start = np.zeros(n + 1, dtype='<i4')
+        excl_start[1:] = np.cumsum([len(e) for e in exs])
+        pod_start[1:] = np.cumsum([len(p) for p in nowl])
+        ex = np.ascontiguousarray(np.concatenate(exs) if n else np.zeros(0), dtype='<i4')
+        pods = np.frombuffer(b''.join(podb), dtype=wire.POD_DTYPE)
+        now = np.ascontiguousarray(np.concatenate(nowl) if n else np.zeros(0), dtype='<f8')
+        out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
+        status = np.zeros(n, dtype='<i4')
+        which = np.zeros(n, dtype='<i4')
+        self._ck(self._L.nhd_plan_scenarios(self._h, src, n, excl_start.ctypes.data,
+                                            ex.ctypes.data if len(ex) else None, pod_start.ctypes.data,
+                                            pods.ctypes.data if len(pods) else None,
+                                            now.ctypes.data if len(pods) else None,
+                                            out.ctypes.data if len(pods) else None, status.ctypes.data,
+                                            which.ctypes.data))
+        return [(code, pod, out[a:b] if code == 0 else None)
+                for code, pod, a, b in zip(status.tolist(), which.tolist(), pod_start[:-1].tolist(), pod_start[1:].tolist())]
+
     def filter_bitmaps(self):
         """Runs only the snapshot predicate kernel on the staged batch; returns
         (feas[type, node] bool, nogpu[node], busy[node], pod_type[pod])."""
