@@ -349,6 +349,30 @@ int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_scenarios,
                            const int32_t* pod_start, const nhd_pod* pods, const double* now,
                            nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod);
 
+/*
+ * nhd_plan_scenarios with replaced records and exclusions that end: "if these nodes were drained and put back in
+ * service, would their pods place elsewhere, and would the pending pods then place?".  Scenario s, with its pods
+ * numbered k = 0 .. n_s - 1 inside it:
+ *   - for every e in [edit_start[s], edit_start[s+1]), node edit_node[e] has record edit_rec[e] for the whole scenario;
+ *   - its excluded nodes are in maintenance for its pods k < lift_at[s] and back in service from pod lift_at[s] on,
+ *     each with the flags of its record (the replacement if it has one) plus what the scenario's earlier pods did to it.
+ *   out[pod_start[s] .. pod_start[s+1])  when scenario_status[s] == NHD_OK: byte for byte what nhd_solve_batch would
+ *                  return on a scratch copy of the source records with (1) the edits applied, (2) NHD_NODE_MAINTENANCE
+ *                  set on the excluded nodes, (3) pods [0, lift_at[s]) solved, (4) the excluded nodes' flags put back,
+ *                  (5) pods [lift_at[s], n_s) solved.
+ * lift_at == NULL, or lift_at[s] == n_s, keeps the exclusions to the end; edit_start == NULL means no edits (then
+ * edit_node and edit_rec are not read).  With neither, the call is nhd_plan_scenarios.  Refusals are per scenario as
+ * there, with the tuple limits judged against the larger of the cluster's largest schedulable NUMA count and the
+ * n_numa of every edit record of the call.  Besides nhd_plan_scenarios' malformed arguments, the whole call is
+ * NHD_ERR_INVALID for edit offsets that do not start at 0 or go down, an edit_node outside [0, n_nodes), a node
+ * edited twice in one scenario, an edit record nhd_validate_node rejects, and a lift_at[s] outside [0, n_s].  Side effects, collectives and waiting as for nhd_plan_scenarios.
+ */
+int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                  const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                  const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                                  const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                  nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

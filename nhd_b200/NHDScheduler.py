@@ -33,7 +33,9 @@ any object with ``K8SMgr``'s method surface, ``cfg_parser(cfgtype, cfgstr)`` ret
 ``CfgToTopology / TopologyToCfg / TopologyToGpuMap`` (``TriadCfgParser``).  There is no CPU
 placement path: without the CUDA library ``DeviceCluster`` raises.
 """
+import copy
 import re
+import threading
 import time
 from enum import Enum
 from queue import Queue
@@ -234,23 +236,31 @@ class DeviceCluster:
 
     def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror'):
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
-        of ``(exclude, tops, pod_groups, now[, packed])`` with ``exclude`` node names.  Returns one ``(code, pod,
-        bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None when the scenario is refused, ``code``
-        and ``pod`` saying why and for which of its pods.  None when the solver in use cannot plan scenarios (a stand-in
-        without ``plan_scenarios``)."""
+        of ``(exclude, tops, pod_groups, now[, packed[, lift[, edits]]])`` with ``exclude`` node names.  ``lift`` (None:
+        never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits`` (None: none):
+        ``{node name: Node-like object}``, packed as ``sync`` packs nodes, the records those nodes have for the whole
+        scenario.  Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
+        when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods.  None when the solver
+        in use cannot plan scenarios (a stand-in without ``plan_scenarios``)."""
         fn = getattr(self._solver, 'plan_scenarios', None)
         if fn is None:
             return None
-        missing = sorted({n for sc in scenarios for n in sc[0] if n not in self._index})
+        missing = sorted({n for sc in scenarios for n in list(sc[0]) + list(sc[6] if len(sc) > 6 and sc[6] else ())
+                          if n not in self._index})
         if missing:
-            raise ValueError(f'cannot exclude unknown node(s) {missing}')
+            raise ValueError(f'cannot exclude or edit unknown node(s) {missing}')
         args = []
         for sc in scenarios:
             exclude, tops, pod_groups, now = sc[:4]
             packed = sc[4] if len(sc) > 4 else None
+            lift = sc[5] if len(sc) > 5 else None
+            edits = sc[6] if len(sc) > 6 else None
             idx = np.asarray([self._index[n] for n in exclude], dtype='<i4')
             nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
-            args.append((idx, self._pods(tops, pod_groups, packed), nows))
+            if edits:
+                edits = (np.asarray([self._index[n] for n in edits], dtype='<i4'), self._pack(list(edits.values())))
+            args.append((idx, self._pods(tops, pod_groups, packed), nows) +
+                        ((lift, edits or None) if lift is not None or edits else ()))
         return fn(args, source=source)
 
     def rewind(self, k: int):
@@ -269,6 +279,16 @@ class DeviceCluster:
 
     def name_of(self, index: int) -> str:
         return self._names[index]
+
+
+def _copy_node(node):
+    """A copy of ``node`` that a planned release may change: ``copy.deepcopy`` with a new ``busy_lock`` (a lock cannot
+    be copied) and the pods' topologies shared (a release only reads them)."""
+    memo = {id(top): top for top in node.pod_info.values()}
+    lock = getattr(node, 'busy_lock', None)
+    if lock is not None:
+        memo[id(lock)] = threading.Lock()
+    return copy.deepcopy(node, memo)
 
 
 class _Pending:
@@ -323,9 +343,6 @@ class NHDScheduler:
     def _touch(self, name):
         """The host changed node ``name`` outside the solver: re-send it before the next batch."""
         self._dirty.add(name)
-
-    def _set_busy(self, node):                       # Node.SetBusy, Node.py:843-845, on the scheduler's clock
-        node.busy_time = float(self._clock())
 
     def close(self):
         self.cluster.close()
@@ -394,25 +411,40 @@ class NHDScheduler:
                 self.ClaimPodResources(p[0], p[1], p[2])
 
     def ReleasePodResources(self, podname, ns):
-        cfgstr = self.k8s.GetCfgAnnotations(podname, ns)
-        if cfgstr == False:                          # noqa: E712  never annotated: full re-scan (:178-181)
+        target = self._release_target(podname, ns)
+        if target is None:                           # never annotated: full re-scan (:178-181)
             self.ResetResources()
             return
+        node, top = target
+        if node is not None:
+            self._touch(node)
+            self._give_back(self.nodes[node], podname, ns, top, float(self._clock()))
+
+    def _release_target(self, podname, ns):
+        """The Kubernetes reads of ``ReleasePodResources``: ``(node name, topology)`` of what deleting the pod gives
+        back, ``(None, None)`` when it gives nothing back, None when the pod was never annotated (the release then
+        re-scans every node)."""
+        cfgstr = self.k8s.GetCfgAnnotations(podname, ns)
+        if cfgstr == False:                          # noqa: E712  (the reference's test)
+            return None
         cfgtype = self.k8s.GetCfgType(podname, ns)
         tcfg = self.GetCfgParser(cfgtype, cfgstr)
         top = tcfg.CfgToTopology(True)
-        if top is not None:
-            node = self.k8s.GetPodNode(podname, ns)
-            if not node:                             # annotated but not bound: nothing is given back (:189-191)
-                return
-            if node not in self.nodes:
-                return
-            if not self.nodes[node].PodPresent(podname, ns):
-                return
-            self._touch(node)
-            self.nodes[node].AddResourcesFromTopology(top)
-            self.nodes[node].RemoveScheduledPod(podname, ns)
-            self._set_busy(self.nodes[node])
+        if top is None:
+            return None, None
+        node = self.k8s.GetPodNode(podname, ns)
+        # annotated but not bound (:189-191), an unknown node, a pod the node does not hold: nothing is given back
+        if not node or node not in self.nodes or not self.nodes[node].PodPresent(podname, ns):
+            return None, None
+        return node, top
+
+    @staticmethod
+    def _give_back(node, podname, ns, top, now: float):
+        """The release proper, on ``node``: the pod's resources back, the pod gone, busy from ``now`` (Node.SetBusy,
+        Node.py:843-845, on the scheduler's clock)."""
+        node.AddResourcesFromTopology(top)
+        node.RemoveScheduledPod(podname, ns)
+        node.busy_time = now
 
     def ParsePodResources(self, pod: str, ns: str) -> Dict[str, int]:      # :214-224
         res = self.k8s.GetRequestedPodResources(pod, ns)
@@ -763,6 +795,116 @@ class NHDScheduler:
                     result[g][(e.key[0], e.key[1])] = self.cluster.name_of(int(b['node']))
         return result
 
+    def PlanDefrag(self, keys: Sequence = None, node_groups: Sequence[Sequence[str]] = None,
+                   delay: float = None) -> Dict:
+        """Which nodes (or groups of nodes), drained and put back in service, would let the pending pods place?  For
+        every group, the maintenance workflow planned from the same state, all groups side by side in one GPU call:
+          1. ``NODE_MAINT_START`` on the group's nodes;
+          2. their pods deleted (each released as ``ReleasePodResources`` releases it: resources back, the node busy
+             from now) and re-created, each scheduled at once at the current clock, the group in maintenance;
+          3. ``NODE_MAINT_END`` on the group's nodes (back in service, whatever their maintenance flag was);
+          4. ``delay`` seconds later, the pods of ``keys`` scheduled in order, as the next ``CheckPendingPods`` would.
+        Returns ``{tuple(group): (moved, pending)}``: ``moved[(ns, name)]`` the node each of the group's pods (nodes in
+        the given order, pods in ``Node.pod_info`` order, as ``PlanDrain``) goes to, or None; ``pending[(ns, name)]``
+        the node each pod of ``keys`` goes to, or None.  ``pending`` is None when some moved pod found no node: the
+        next scan would retry that pod too, so the group does not resolve the fragmentation it was planned for.
+        ``keys`` (``(ns, name[, uid])``) defaults to the pods the next ``CheckPendingPods`` would attempt, in its
+        order; ``node_groups`` to every node holding pods on its own, in node order.  ``delay`` defaults to
+        ``MIN_BUSY_SECS``: the first moment the released nodes (busy from the release) take GPU pods again; with less,
+        a GPU pod of ``keys`` does not see them.  A group holding a pod that was never annotated is not planned
+        (its delete would re-scan every node): its pods map to None and ``pending`` is None.
+        Only reads happen, as ``PlanDrains``: each pod is read from Kubernetes once (a scheduling attempt's reads and
+        a release's); the releases run on copies of the ``Node`` objects; ``pod_state``, the ``Node`` objects and the
+        counters stay as they are."""
+        if node_groups is None:
+            node_groups = [[n] for n, v in self.nodes.items() if v.pod_info]
+        groups = [tuple(g) for g in node_groups]
+        missing = sorted({n for g in groups for n in g if n not in self.nodes})
+        if missing:
+            raise ValueError(f'unknown node(s) {missing}')
+        if keys is None:
+            phase = self._service_pods()
+            keys = [k for k in phase if self._wanted(phase)(k)]
+        delay = float(self._node_cls.MIN_BUSY_SECS if delay is None else delay)
+        prepared, targets = {}, {}
+
+        def prepare(key):
+            if key not in prepared:
+                e = _Pending(len(prepared), key)
+                self._prepare(e, events=False)
+                prepared[key] = e
+            return prepared[key]
+        tail = [prepare((k[0], k[1])) for k in keys]
+        tail_ok = [e for e in tail if e.top is not None and e.unsupported is None]
+        group_pods = []
+        for g in groups:
+            pods = [(ns, pod) for n in g for (pod, ns) in self.nodes[n].pod_info]
+            for key in pods:
+                if key not in targets:
+                    targets[key] = self._release_target(key[1], key[0])
+            group_pods.append(pods)
+        entries = [[prepare(key) for key in pods] for pods in group_pods]
+        result = {g: ({key: None for key in pods}, None) for g, pods in zip(groups, group_pods)}
+        if not self.nodes:
+            return result
+        self.cluster.sync(self.nodes, self._dirty)
+        self._dirty.clear()
+        now = float(self._clock())
+        todo = []
+        for g, pods, moved in zip(groups, group_pods, entries):
+            if any(targets[key] is None for key in pods):
+                continue
+            edits = {}
+            for n in g:
+                edits[n] = _copy_node(self.nodes[n])
+                edits[n].maintenance = False                       # NODE_MAINT_END
+            for key in pods:
+                node, top = targets[key]
+                if node is None:
+                    continue
+                if node not in edits:
+                    edits[node] = _copy_node(self.nodes[node])
+                self._give_back(edits[node], key[1], key[0], top, now)
+            ok = [e for e in moved if e.top is not None and e.unsupported is None]
+            todo.append((g, ok, tail_ok, edits))
+        while todo:
+            res = self.cluster.plan_scenarios([self._defrag_scenario(g, ok, tail, edits, now, delay)
+                                               for g, ok, tail, edits in todo])
+            if res is None:
+                raise RuntimeError('the solver in use cannot plan scenarios (no plan_scenarios)')
+            retry = []
+            for (g, ok, tail, edits), (code, pod, out) in zip(todo, res):
+                if out is None:
+                    # a pod beyond the tuple limits (judged with the group's nodes and the edited records counted):
+                    # it gets None, as in PlanDrain, and the group is planned again without it
+                    if code != wire.ERR_UNSUPPORTED:
+                        raise RuntimeError(f'nhd_plan_scenarios_edited refused group {g}: code {code}, pod {pod}')
+                    if pod < len(ok):
+                        ok = ok[:pod] + ok[pod + 1:]
+                    else:
+                        tail = tail[:pod - len(ok)] + tail[pod - len(ok) + 1:]
+                    retry.append((g, ok, tail, edits))
+                    continue
+                moved, _ = result[g]
+                for e, b in zip(ok, out[:len(ok)]):
+                    if int(b['status']) == wire.PLACED:
+                        moved[e.key] = self.cluster.name_of(int(b['node']))
+                if all(v is not None for v in moved.values()):
+                    pending = {(k[0], k[1]): None for k in keys}
+                    for e, b in zip(tail, out[len(ok):]):
+                        if int(b['status']) == wire.PLACED:
+                            pending[e.key] = self.cluster.name_of(int(b['node']))
+                    result[g] = (moved, pending)
+            todo = retry
+        return result
+
+    @staticmethod
+    def _defrag_scenario(g, moved, tail, edits, now, delay):
+        """One ``PlanDefrag`` group as a ``DeviceCluster.plan_scenarios`` scenario."""
+        pods = moved + tail
+        clock = [now] * len(moved) + [now + delay] * len(tail)
+        return (g, [e.top for e in pods], [e.groups for e in pods], clock, [e.rec for e in pods], len(moved), edits)
+
     def _plan(self, keys: Sequence, exclude: Sequence[str]):
         entries = [_Pending(i, k) for i, k in enumerate(keys)]
         for e in entries:
@@ -804,19 +946,26 @@ class NHDScheduler:
 
     def CheckPendingPods(self):
         """``NHDScheduler.py:425-441`` with the pending set solved as one batch."""
-        podlist = self.k8s.ServicePods(self.sched_name)
-        phase = {(k[0], k[1], k[2]): p for k, p in podlist.items()}
+        phase = self._service_pods()
+        self.ScheduleBatch(list(phase), self._wanted(phase))
+        # The reference's second branch (:437-440) compares the pod_state *dict* with an enum member and
+        # therefore never runs; a pod reported 'Failed' keeps its resources until its delete event.
 
+    def _service_pods(self):
+        """``{(ns, name, uid): (phase, node)}`` of every pod of this scheduler, in Kubernetes' order."""
+        podlist = self.k8s.ServicePods(self.sched_name)
+        return {(k[0], k[1], k[2]): p for k, p in podlist.items()}
+
+    def _wanted(self, phase):
+        """The pods of ``phase`` (``_service_pods``) that ``CheckPendingPods`` attempts: pending, unbound and not
+        scheduled here.  Asked again after a cut, since a reset clears ``pod_state``."""
         def wanted(k):
             p = phase[k]
             podkey = (k[0], k[1])
             return (p[0] == 'Pending' and p[1] == None and                     # noqa: E711
                     ((podkey not in self.pod_state) or
                      self.pod_state[podkey]['state'] != PodStatus.POD_STATUS_SCHEDULED))
-
-        self.ScheduleBatch(list(phase), wanted)
-        # The reference's second branch (:437-440) compares the pod_state *dict* with an enum member and
-        # therefore never runs; a pod reported 'Failed' keeps its resources until its delete event.
+        return wanted
 
     # ---- the thread function (NHDScheduler.py:443-577) ------------------------------------------------
     def Startup(self):

@@ -1340,41 +1340,67 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
 }
 
 /*
- * Many independent plans at once, each on the source records with its own excluded nodes: every scenario's pods are
- * checked as nhd_stage_batch checks them (a refusal refuses that scenario only), the pods of the accepted scenarios are
- * de-duplicated into one pod set and filtered once on the unchanged source records (launch_solve's tables + filter, as
- * a query), then one warp per scenario walks its pods in order (scenario_plan_kernel).  The tuple limits are judged
- * against the whole cluster's NUMA counts: the shared filter enumerates the tuples of every node, the excluded ones
- * included.
+ * Many independent plans at once, each on the source records with its own excluded nodes and its own replaced records:
+ * every scenario's pods are checked as nhd_stage_batch checks them (a refusal refuses that scenario only), the pods of
+ * the accepted scenarios are de-duplicated into one pod set and filtered once on the unchanged source records
+ * (launch_solve's tables + filter, as a query), then one warp per scenario walks its pods in order
+ * (scenario_plan_kernel), starting from its edited records and lifting its exclusions at its lift index.  The tuple
+ * limits are judged against the whole cluster's NUMA counts and those of the edit records: the shared filter
+ * enumerates the tuples of every node, the excluded ones included, and an edited node is evaluated on its own record.
  */
-extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_scenarios, const int32_t* excl_start,
-                                      const int32_t* excluded, const int32_t* pod_start, const nhd_pod* pods,
-                                      const double* now, nhd_binding* out, int32_t* scenario_status,
-                                      int32_t* scenario_pod)
+static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, int32_t n_scenarios,
+                              const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                              const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                              const int32_t* pod_start, const nhd_pod* pods, const double* now, nhd_binding* out,
+                              int32_t* scenario_status, int32_t* scenario_pod)
 {
     if (!h || n_scenarios < 0 || !excl_start || !pod_start || (n_scenarios > 0 && (!scenario_status || !scenario_pod)))
         return NHD_ERR_INVALID;
-    if (excl_start[0] != 0 || pod_start[0] != 0) return fail(h, NHD_ERR_INVALID, "scenario offsets must start at 0");
+    if (excl_start[0] != 0 || pod_start[0] != 0 || (edit_start && edit_start[0] != 0))
+        return fail(h, NHD_ERR_INVALID, "scenario offsets must start at 0");
     for (int s = 0; s < n_scenarios; s++)
-        if (excl_start[s + 1] < excl_start[s] || pod_start[s + 1] < pod_start[s])
+        if (excl_start[s + 1] < excl_start[s] || pod_start[s + 1] < pod_start[s] ||
+            (edit_start && edit_start[s + 1] < edit_start[s]))
             return fail(h, NHD_ERR_INVALID, "scenario %d: offsets go down", s);
     const int n_excl = excl_start[n_scenarios], n_pods = pod_start[n_scenarios];
-    if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out))) return NHD_ERR_INVALID;
+    const int n_edit = edit_start ? edit_start[n_scenarios] : 0;
+    if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)) || (n_edit > 0 && (!edit_node || !edit_rec)))
+        return NHD_ERR_INVALID;
     uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
     if (rc != NHD_OK) return rc;
     for (int e = 0; e < n_excl; e++)
         if (excluded[e] < 0 || excluded[e] >= h->n_nodes)
             return fail(h, NHD_ERR_INVALID, "excluded node %d outside the %d loaded nodes", excluded[e], h->n_nodes);
+    int max_numa = h->max_numa;
+    for (int e = 0; e < n_edit; e++) {
+        if (edit_node[e] < 0 || edit_node[e] >= h->n_nodes)
+            return fail(h, NHD_ERR_INVALID, "edited node %d outside the %d loaded nodes", edit_node[e], h->n_nodes);
+        if (nhd_validate_node(&edit_rec[e]) != NHD_OK)
+            return fail(h, NHD_ERR_INVALID, "edit record %d rejected by nhd_validate_node", e);
+        max_numa = std::max(max_numa, (int)edit_rec[e].n_numa);
+    }
+    for (int s = 0; s < n_scenarios && n_edit > 0; s++) {
+        std::vector<int32_t> nodes(edit_node + edit_start[s], edit_node + edit_start[s + 1]);
+        std::sort(nodes.begin(), nodes.end());
+        if (std::adjacent_find(nodes.begin(), nodes.end()) != nodes.end())
+            return fail(h, NHD_ERR_INVALID, "scenario %d: node %d edited twice", s, *std::adjacent_find(nodes.begin(), nodes.end()));
+    }
+    for (int s = 0; s < n_scenarios && lift_at; s++)
+        if (lift_at[s] < 0 || lift_at[s] > pod_start[s + 1] - pod_start[s])
+            return fail(h, NHD_ERR_INVALID, "scenario %d: lift index %d outside [0, %d]", s, lift_at[s],
+                        pod_start[s + 1] - pod_start[s]);
 
-    /* per scenario: its refusal, or its place among the accepted ones (pods and exclusions compacted, the exclusions
-     * sorted and each once).  idx = pod offsets | exclusion offsets | exclusions of the accepted scenarios. */
-    std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex;
+    /* per scenario: its refusal, or its place among the accepted ones (pods, exclusions and edits compacted, the
+     * exclusions sorted and each once).  idx = pod offsets | exclusion offsets | exclusions | edit offsets | edited
+     * nodes | lift indices of the accepted scenarios. */
+    std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex, ed_off{0}, ed_node, lift;
+    std::vector<nhd_node_rec> ed_rec;
     for (int s = 0; s < n_scenarios; s++) {
         scenario_status[s] = NHD_OK;
         scenario_pod[s] = -1;
         for (int i = pod_start[s]; i < pod_start[s + 1]; i++) {
-            const int32_t v = check_pod(nullptr, i - pod_start[s], pods[i], now[i], h->max_numa);
+            const int32_t v = check_pod(nullptr, i - pod_start[s], pods[i], now[i], max_numa);
             if (v != NHD_OK) { scenario_status[s] = v; scenario_pod[s] = i - pod_start[s]; break; }
         }
         if (scenario_status[s] != NHD_OK) continue;
@@ -1385,8 +1411,14 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
         std::sort(ex.begin() + e0, ex.end());
         ex.erase(std::unique(ex.begin() + e0, ex.end()), ex.end());
         ex_off.push_back((int32_t)ex.size());
+        if (n_edit > 0) {
+            ed_node.insert(ed_node.end(), edit_node + edit_start[s], edit_node + edit_start[s + 1]);
+            ed_rec.insert(ed_rec.end(), edit_rec + edit_start[s], edit_rec + edit_start[s + 1]);
+        }
+        ed_off.push_back((int32_t)ed_node.size());
+        lift.push_back(lift_at ? lift_at[s] : pod_start[s + 1] - pod_start[s]);
     }
-    const int n_acc = (int)acc.size(), n_run = pod_off.back();
+    const int n_acc = (int)acc.size(), n_run = pod_off.back(), n_ed = ed_off.back();
     if (n_run == 0) return NHD_OK;
     const bool compact = n_run != n_pods;
     std::vector<nhd_pod> cpods;
@@ -1401,19 +1433,23 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
     }
     SolveWork w;
     w.nodes = records;
-    if ((rc = upload_pod_set(h, n_run, compact ? cpods.data() : pods, compact ? cnow.data() : now, h->max_numa, w)) != NHD_OK)
+    if ((rc = upload_pod_set(h, n_run, compact ? cpods.data() : pods, compact ? cnow.data() : now, max_numa, w)) != NHD_OK)
         return rc;
 
     std::vector<int32_t> idx;
-    idx.reserve(pod_off.size() + ex_off.size() + ex.size());
-    idx.insert(idx.end(), pod_off.begin(), pod_off.end());
-    idx.insert(idx.end(), ex_off.begin(), ex_off.end());
-    idx.insert(idx.end(), ex.begin(), ex.end());
-    const size_t off_nodes = idx.size(), off_bad = off_nodes + (size_t)n_run;
+    idx.reserve(pod_off.size() + ex_off.size() + ex.size() + ed_off.size() + ed_node.size() + lift.size());
+    for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift}) idx.insert(idx.end(), v->begin(), v->end());
+    const size_t off_ex_off = pod_off.size(), off_ex = off_ex_off + ex_off.size(), off_ed_off = off_ex + ex.size();
+    const size_t off_ed_node = off_ed_off + ed_off.size(), off_lift = off_ed_node + ed_node.size();
+    const size_t n_slots = (size_t)n_run + n_ed, off_nodes = idx.size(), off_bad = off_nodes + n_slots;
+    /* d_swork: the working slots, then the edit records the kernel seeds them from */
     CK(grow_dev(h->d_sidx, h->sidx_cap, (off_bad + 1) * 4));
-    CK(grow_dev(h->d_swork, h->swork_cap, (size_t)n_run * sizeof(nhd_node_rec)));
+    CK(grow_dev(h->d_swork, h->swork_cap, (n_slots + n_ed) * sizeof(nhd_node_rec)));
     CK(cudaMemcpyAsync(h->d_sidx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(h->d_sidx + off_bad, 0, 4, h->stream));
+    uint4* d_edit_rec = h->d_swork + n_slots * REC_CHUNKS;
+    if (n_ed > 0)
+        CK(cudaMemcpyAsync(d_edit_rec, ed_rec.data(), (size_t)n_ed * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
 
     /* the candidate bitmaps of the call's pod types on the unchanged source records */
     if ((rc = launch_solve(h, w, false, true)) != NHD_OK) return rc;
@@ -1421,7 +1457,9 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
     ScenarioArgs sa;
     sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type; sa.now = w.now;
     sa.bitmaps = w.bitmaps; sa.pod_groups = w.pod_groups; sa.names_used = w.names_used;
-    sa.pod_start = h->d_sidx; sa.excl_start = h->d_sidx + pod_off.size(); sa.excl = sa.excl_start + ex_off.size();
+    sa.pod_start = h->d_sidx; sa.excl_start = h->d_sidx + off_ex_off; sa.excl = h->d_sidx + off_ex;
+    sa.lift = h->d_sidx + off_lift; sa.edit_start = h->d_sidx + off_ed_off; sa.edit_node = h->d_sidx + off_ed_node;
+    sa.edit_rec = d_edit_rec;
     sa.work = h->d_swork; sa.work_node = h->d_sidx + off_nodes; sa.out = w.out; sa.bad = (uint32_t*)(h->d_sidx + off_bad);
     sa.n_scenarios = n_acc; sa.n_types = w.n_types; sa.words = h->words;
     sa.min_busy = h->params.min_busy_secs;
@@ -1435,11 +1473,31 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
     std::vector<nhd_binding> run;
     if (compact) run.resize(n_run);
     if ((rc = fetch_scratch_bindings(h, n_run, compact ? run.data() : out)) != NHD_OK) return rc;
-    if (bad) return fail(h, NHD_ERR_STATE, "nhd_plan_scenarios: %u chosen nodes without a mapping", bad);
+    if (bad) return fail(h, NHD_ERR_STATE, "%s: %u chosen nodes without a mapping", what, bad);
     if (compact)
         for (int k = 0; k < n_acc; k++)
             memcpy(out + pod_start[acc[k]], run.data() + pod_off[k], (size_t)(pod_off[k + 1] - pod_off[k]) * sizeof(nhd_binding));
     return NHD_OK;
+}
+
+extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_scenarios, const int32_t* excl_start,
+                                      const int32_t* excluded, const int32_t* pod_start, const nhd_pod* pods,
+                                      const double* now, nhd_binding* out, int32_t* scenario_status,
+                                      int32_t* scenario_pod)
+{
+    return plan_scenarios(h, "nhd_plan_scenarios", source, n_scenarios, excl_start, excluded, nullptr, nullptr, nullptr,
+                          nullptr, pod_start, pods, now, out, scenario_status, scenario_pod);
+}
+
+extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                             const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                             const int32_t* edit_start, const int32_t* edit_node,
+                                             const nhd_node_rec* edit_rec, const int32_t* pod_start, const nhd_pod* pods,
+                                             const double* now, nhd_binding* out, int32_t* scenario_status,
+                                             int32_t* scenario_pod)
+{
+    return plan_scenarios(h, "nhd_plan_scenarios_edited", source, n_scenarios, excl_start, excluded, lift_at,
+                          edit_start, edit_node, edit_rec, pod_start, pods, now, out, scenario_status, scenario_pod);
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

@@ -2744,13 +2744,18 @@ __global__ void exclude_nodes_kernel(uint8_t* nodes, const int32_t* __restrict__
 /* ------------------------------------------------------------------ independent plans (nhd_plan_scenarios) */
 
 /*
- * Not part of a solve: many small plans at once, each on the source records with its own nodes in maintenance.  One
- * filter of the call's pod types on the unchanged source records serves every scenario, because a scenario's records
- * differ from them only at its excluded nodes (dropped by the maintenance stage, skipped here) and at the nodes its own
- * earlier pods reached (its touched set, evaluated on working records).  On an untouched node F[type] is FindNode's
- * candidate set apart from the busy window, as for a query.  So for pod i the first node of
- *     (untouched, not excluded, F[type], node-group gate, not busy for a GPU pod)  U  (touched, passes every stage)
- * is the reference's SelectNode at that pod.  One warp per scenario, its pods in order.
+ * Not part of a solve: many small plans at once, each on the source records with its own nodes in maintenance and its
+ * own replaced records (nhd_plan_scenarios_edited).  One filter of the call's pod types on the unchanged source records
+ * serves every scenario, because a scenario's records differ from them only at its excluded nodes (dropped by the
+ * maintenance stage, skipped here while the exclusion lasts), at its edited nodes and at the nodes its own earlier pods
+ * reached.  The last two form its touched set, which starts as the edited nodes and is evaluated on working records,
+ * never from the bitmaps.  On an untouched node F[type] is FindNode's candidate set apart from the busy window, as for a
+ * query; that holds for an excluded node once its exclusion is lifted too, since its source record is unchanged.  So
+ * for pod i the first node of
+ *     (untouched, not excluded, F[type], node-group gate, not busy for a GPU pod)  U  (touched, not excluded,
+ *     passes every stage)
+ * is the reference's SelectNode at that pod, "excluded" meaning in the scenario's list and i - p0 < lift[s].  One warp
+ * per scenario, its pods in order.
  */
 struct ScenarioArgs {
     const uint8_t* nodes;          /* the source records (mirror or snapshot, tiled layout), only read */
@@ -2763,8 +2768,13 @@ struct ScenarioArgs {
     const int32_t* pod_start;      /* [n_scenarios + 1]: scenario s owns pods pod_start[s] .. pod_start[s + 1] */
     const int32_t* excl_start;     /* [n_scenarios + 1] into excl */
     const int32_t* excl;           /* each scenario's excluded nodes, sorted, without duplicates */
-    uint4* work;                   /* [n_pods][8]: slot pod_start[s] + k = working record of scenario s's k-th touched node */
-    int32_t* work_node;            /* [n_pods]: the node of each slot */
+    const int32_t* lift;           /* [n_scenarios]: the exclusions hold for the scenario's pods k < lift[s] */
+    const int32_t* edit_start;     /* [n_scenarios + 1] into edit_node / edit_rec */
+    const int32_t* edit_node;      /* each scenario's edited nodes, each once */
+    const uint4* edit_rec;         /* [n_edits][8]: their records */
+    uint4* work;                   /* [n_pods + n_edits][8]: slot pod_start[s] + edit_start[s] + k = working record of
+                                      scenario s's k-th touched node; its edited nodes come first */
+    int32_t* work_node;            /* [n_pods + n_edits]: the node of each slot */
     nhd_binding* out;
     uint32_t* bad;                 /* chosen nodes on which no mapping was found: never expected, refused by the host */
     int n_scenarios, n_types, words;
@@ -2784,9 +2794,10 @@ __device__ __forceinline__ bool sorted_contains(const int32_t* v, int n, int x)
     return lo < n && v[lo] == x;
 }
 
-/* One warp per scenario (grid-stride).  For each pod: the first touched node that passes every stage on its working
- * record (explain_node, lanes over the touched set, warp minimum) and the first untouched candidate (query_select_kernel's
- * ballot scan, skipping excluded and touched nodes), GPU-less pass first for a pod without GPUs (Matcher.py:412-421);
+/* One warp per scenario (grid-stride).  The working set starts with the scenario's edited records.  For each pod: the
+ * first touched node, not excluded, that passes every stage on its working record (explain_node, lanes over the touched
+ * set, warp minimum) and the first untouched candidate (query_select_kernel's ballot scan, skipping excluded and touched
+ * nodes), GPU-less pass first for a pod without GPUs (Matcher.py:412-421);
  * then lane 0 runs the mapping and the assignment (query_assign_kernel's body) on that node's working record, keeps
  * the result as the node's working record and writes the binding. */
 __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const __grid_constant__ ScenarioArgs a)
@@ -2798,11 +2809,16 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
     for (int s = (int)((blockIdx.x * (unsigned)SCENARIO_THREADS + threadIdx.x) >> 5); s < a.n_scenarios; s += n_warps) {
         const int p0 = a.pod_start[s], p1 = a.pod_start[s + 1];
         const int32_t* ex = a.excl + a.excl_start[s];
-        const int n_ex = a.excl_start[s + 1] - a.excl_start[s];
-        uint4* work = a.work + (size_t)p0 * REC_CHUNKS;
-        int32_t* work_node = a.work_node + p0;
-        int n_touched = 0;
+        const int n_ex_held = a.excl_start[s + 1] - a.excl_start[s], lift = a.lift[s];
+        const int e0 = a.edit_start[s], n_edits = a.edit_start[s + 1] - e0;
+        uint4* work = a.work + (size_t)(p0 + e0) * REC_CHUNKS;
+        int32_t* work_node = a.work_node + p0 + e0;
+        for (int k = lane; k < n_edits * REC_CHUNKS; k += 32) work[k] = a.edit_rec[(size_t)e0 * REC_CHUNKS + k];
+        for (int k = lane; k < n_edits; k += 32) work_node[k] = a.edit_node[e0 + k];
+        __syncwarp();                                                  /* the edited nodes are the first touched ones */
+        int n_touched = n_edits;
         for (int i = p0; i < p1; i++) {
+            const int n_ex = i - p0 < lift ? n_ex_held : 0;           /* back in service from pod lift on */
             const int ti = a.pod_type[i];
             const PodType& t = a.types[ti];
             uint4* bout = reinterpret_cast<uint4*>(&a.out[i]);
@@ -2822,7 +2838,7 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
 #pragma unroll
                     for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)k * REC_CHUNKS + c];
                     const int node = work_node[k];
-                    if (node < best && (pass == 1 || u.r.n_gpus == 0) &&
+                    if (node < best && (pass == 1 || u.r.n_gpus == 0) && !sorted_contains(ex, n_ex, node) &&
                         explain_node(u.r, t, a.pod_groups ? gm : t.pod.group_mask, now, a.min_busy, a.cap) == NHD_WHY_COUNT) {
                         best = node;
                         best_k = k;

@@ -221,18 +221,26 @@ class Solver:
         return (out, counts) if explain else out
 
     def plan_scenarios(self, scenarios, source='mirror'):
-        """Many independent dry runs in one call (``nhd_plan_scenarios``).  ``scenarios``: a sequence of
-        ``(exclude, pods, now)``.  Returns one ``(code, pod, bindings)`` per scenario: ``code`` 0 and ``bindings`` what
-        ``plan_batch(pods, now, source, exclude)`` returns, or the refusal ``plan_batch`` would raise (``wire.ERR_*``),
-        the index of the pod it names and None.  Scenarios do not see each other.  Unlike ``plan_batch`` the tuple
-        limits are judged with the excluded nodes counted; ``plan_batch`` plans a scenario refused for that."""
+        """Many independent dry runs in one call (``nhd_plan_scenarios_edited``).  ``scenarios``: a sequence of
+        ``(exclude, pods, now[, lift[, edits]])``.  Returns one ``(code, pod, bindings)`` per scenario: ``code`` 0 and
+        ``bindings`` what ``plan_batch(pods, now, source, exclude)`` returns, or the refusal ``plan_batch`` would raise
+        (``wire.ERR_*``), the index of the pod it names and None.  Scenarios do not see each other.  Unlike
+        ``plan_batch`` the tuple limits are judged with the excluded nodes counted; ``plan_batch`` plans a scenario
+        refused for that.
+        ``lift`` (None: never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits``
+        (None: none): ``(nodes, records)``, node indices and a ``wire.NODE_DTYPE`` array, the records those nodes have
+        for the whole scenario.  With either, the bindings are those of ``solve_batch`` on a scratch copy of the records
+        with the edits applied, the excluded nodes in maintenance for the pods before ``lift`` and back after."""
         src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
         if src is None:
             raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
         # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
         # would cost more than the call itself)
-        exs, podb, nowl = [], [], []
-        for exclude, pods, now in scenarios:
+        exs, podb, nowl, lifts, ednodes, edrecs = [], [], [], [], [], []
+        for sc in scenarios:
+            exclude, pods, now = sc[:3]
+            lift = sc[3] if len(sc) > 3 else None
+            edits = sc[4] if len(sc) > 4 else None
             pods = np.asarray(pods)
             if pods.dtype != wire.POD_DTYPE:
                 pods = pods.astype(wire.POD_DTYPE)
@@ -240,23 +248,40 @@ class Solver:
             podb.append(np.ascontiguousarray(pods).tobytes())
             nowl.append(np.asarray(now, dtype='<f8').reshape(-1))
             assert pods.size == len(nowl[-1])
+            lifts.append(len(nowl[-1]) if lift is None else int(lift))
+            if edits is None:
+                ednodes.append(np.zeros(0, dtype='<i4'))
+            else:
+                nodes, recs = edits
+                ednodes.append(np.asarray(nodes, dtype='<i4').reshape(-1))
+                recs = np.asarray(recs, dtype=wire.NODE_DTYPE).reshape(-1)
+                assert len(recs) == len(ednodes[-1])
+                edrecs.append(recs.tobytes())
         n = len(podb)
         excl_start = np.zeros(n + 1, dtype='<i4')
         pod_start = np.zeros(n + 1, dtype='<i4')
+        edit_start = np.zeros(n + 1, dtype='<i4')
         excl_start[1:] = np.cumsum([len(e) for e in exs])
         pod_start[1:] = np.cumsum([len(p) for p in nowl])
+        edit_start[1:] = np.cumsum([len(e) for e in ednodes])
         ex = np.ascontiguousarray(np.concatenate(exs) if n else np.zeros(0), dtype='<i4')
         pods = np.frombuffer(b''.join(podb), dtype=wire.POD_DTYPE)
         now = np.ascontiguousarray(np.concatenate(nowl) if n else np.zeros(0), dtype='<f8')
+        lift = np.asarray(lifts, dtype='<i4')
+        ednode = np.ascontiguousarray(np.concatenate(ednodes) if n else np.zeros(0), dtype='<i4')
+        edrec = np.frombuffer(b''.join(edrecs), dtype=wire.NODE_DTYPE)
         out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
         status = np.zeros(n, dtype='<i4')
         which = np.zeros(n, dtype='<i4')
-        self._ck(self._L.nhd_plan_scenarios(self._h, src, n, excl_start.ctypes.data,
-                                            ex.ctypes.data if len(ex) else None, pod_start.ctypes.data,
-                                            pods.ctypes.data if len(pods) else None,
-                                            now.ctypes.data if len(pods) else None,
-                                            out.ctypes.data if len(pods) else None, status.ctypes.data,
-                                            which.ctypes.data))
+        self._ck(self._L.nhd_plan_scenarios_edited(self._h, src, n, excl_start.ctypes.data,
+                                                   ex.ctypes.data if len(ex) else None,
+                                                   lift.ctypes.data if n else None, edit_start.ctypes.data,
+                                                   ednode.ctypes.data if len(ednode) else None,
+                                                   edrec.ctypes.data if len(edrec) else None, pod_start.ctypes.data,
+                                                   pods.ctypes.data if len(pods) else None,
+                                                   now.ctypes.data if len(pods) else None,
+                                                   out.ctypes.data if len(pods) else None, status.ctypes.data,
+                                                   which.ctypes.data))
         return [(code, pod, out[a:b] if code == 0 else None)
                 for code, pod, a, b in zip(status.tolist(), which.tolist(), pod_start[:-1].tolist(), pod_start[1:].tolist())]
 
