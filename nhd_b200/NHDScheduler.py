@@ -188,6 +188,11 @@ class DeviceCluster:
                 packing.pack_pod(top, pod_groups[i], self._layout, out=pods[i])
         return pods
 
+    @staticmethod
+    def _clocks(n: int, now) -> np.ndarray:
+        """Per-pod clocks of ``n`` pods from one clock or one per pod."""
+        return np.full(n, now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
+
     def solve(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now: float, packed: Sequence = None):
         """Bindings of ``tops`` scheduled in order on the synced cluster (one GPU call).  ``packed``: records
         ``pack_pod`` already made of them; only the node-group mask is worked out again (``sync`` may have met new
@@ -214,8 +219,7 @@ class DeviceCluster:
         fn = getattr(self._solver, 'query_batch', None)
         if fn is None:
             return None
-        nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
-        return fn(self._pods(tops, pod_groups, packed), nows, source=source)
+        return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), source=source)
 
     def plan(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now, source: str = 'mirror',
              exclude: Iterable[str] = (), packed: Sequence = None, explain: bool = False):
@@ -231,8 +235,8 @@ class DeviceCluster:
         if missing:
             raise ValueError(f'cannot exclude unknown node(s) {missing}')
         idx = np.asarray([self._index[n] for n in exclude], dtype='<i4')
-        nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
-        return fn(self._pods(tops, pod_groups, packed), nows, source=source, exclude=idx, explain=explain)
+        return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), source=source, exclude=idx,
+                  explain=explain)
 
     def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror'):
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
@@ -256,10 +260,9 @@ class DeviceCluster:
             lift = sc[5] if len(sc) > 5 else None
             edits = sc[6] if len(sc) > 6 else None
             idx = np.asarray([self._index[n] for n in exclude], dtype='<i4')
-            nows = np.full(len(tops), now, dtype='<f8') if np.isscalar(now) else np.asarray(now, dtype='<f8')
             if edits:
                 edits = (np.asarray([self._index[n] for n in edits], dtype='<i4'), self._pack(list(edits.values())))
-            args.append((idx, self._pods(tops, pod_groups, packed), nows) +
+            args.append((idx, self._pods(tops, pod_groups, packed), self._clocks(len(tops), now)) +
                         ((lift, edits or None) if lift is not None or edits else ()))
         return fn(args, source=source)
 

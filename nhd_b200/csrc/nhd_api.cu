@@ -62,6 +62,75 @@ static NcclApi g_nccl;
 
 static_assert(offsetof(nhd_node_rec, flags) == 2 * 16 + REC_FLAGS_BYTE, "exclude_nodes_kernel's flags byte");
 
+/* ------------------------------------------------------------------ buffers */
+
+/* An owned device (or pinned host) allocation: grow(bytes) keeps it when it holds that many bytes and otherwise replaces
+ * it, contents lost, by one of max(bytes, 256) bytes.  Freed with its owner. */
+template <typename T, bool Pinned>
+struct Buf {
+    T* p = nullptr;
+    size_t cap = 0;
+    Buf() = default;
+    Buf(const Buf&) = delete;
+    Buf& operator=(const Buf&) = delete;
+    ~Buf() { release(); }
+    operator T*() const { return p; }
+    void release()
+    {
+        if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
+        p = nullptr;
+        cap = 0;
+    }
+    cudaError_t grow(size_t need)
+    {
+        if (need <= cap) return cudaSuccess;
+        release();
+        const size_t want = std::max(need, (size_t)256);
+        const cudaError_t e = Pinned ? cudaMallocHost((void**)&p, want) : cudaMalloc((void**)&p, want);
+        if (e == cudaSuccess) cap = want;
+        return e;
+    }
+};
+template <typename T> using DevBuf = Buf<T, false>;
+template <typename T> using PinnedBuf = Buf<T, true>;
+
+/*
+ * One solve's pod set and every buffer its kernels write (stage_pods fills and sizes it).  The handle holds two: batch,
+ * the staged batch that nhd_solve_staged commits and the explanations and nhd_read_filter read, and scratch, which every
+ * query and plan uses, so that those leave the staged batch, its bindings and its filter output alone.
+ */
+struct Workspace {
+    /* the pod set */
+    int n_pods = 0, n_types = 0, n_names = 0;
+    uint64_t names_used = 0;
+    double now0 = 0.0;                    /* clock of the first pod (the filter's BUSY row) */
+    bool const_clock = true;
+    DevBuf<PodType> types;
+    DevBuf<uint8_t> pod_arrays;           /* pod_type | now | group masks (when n_names > 0) */
+    PinnedBuf<uint8_t> staging;           /* types | pod_arrays */
+    std::vector<int32_t> pod_type_host;
+    /* the filter's output */
+    DevBuf<uint64_t> bitmaps;             /* [n_types + 2 + n_names][words] */
+    DevBuf<uint4> dyn;                    /* NodeDyn summaries */
+    DevBuf<uint8_t> ftab;                 /* direct-path tables, ftab_bytes(FAST_MAX_TYPES) */
+    /* the sweep's */
+    DevBuf<int32_t> cursors;              /* [max(n_types, 1)][3] */
+    DevBuf<int32_t> busy_list;            /* n_super * SUPER_NODES + 64 */
+    DevBuf<int32_t> pend;                 /* n_super * SUPER_NODES */
+    DevBuf<unsigned long long> prof;      /* debug counters (nhd_debug_counters reads the batch's) */
+    /* the bindings */
+    DevBuf<nhd_binding> out;              /* n_pods + 8 (spare records for check builds) */
+    PinnedBuf<nhd_binding> h_out;         /* bounce buffer of fetch_bindings */
+
+    size_t now_offset() const { return ((size_t)n_pods * 4 + 15) & ~(size_t)15; }
+    const int32_t* pod_type() const { return reinterpret_cast<const int32_t*>(pod_arrays.p); }
+    const double* now() const { return reinterpret_cast<const double*>(pod_arrays.p + now_offset()); }
+    const uint64_t* pod_groups() const      /* per-pod node-group masks when the pods mix lists, else null */
+    {
+        return n_names ? reinterpret_cast<const uint64_t*>(pod_arrays.p + now_offset() + (size_t)n_pods * 8) : nullptr;
+    }
+};
+
 /* ------------------------------------------------------------------ handle */
 
 struct nhd_handle {
@@ -79,46 +148,30 @@ struct nhd_handle {
        tuple limits are judged against the largest of these, and follow updates in both directions */
     std::vector<uint8_t> node_numa;
     int numa_hist[NHD_MAX_NUMA + 1] = {0, 0, 0, 0, 0};
-    uint8_t* d_nodes = nullptr;
-    uint8_t* d_snapshot = nullptr;
+    DevBuf<uint8_t> d_nodes, d_snapshot;
     size_t nodes_bytes = 0;
     bool loaded = false, have_snapshot = false;
+    DevBuf<uint16_t> d_class;             /* hardware class of every node of the mirror */
+    DevBuf<ClassSlot> d_class_slots;
+    DevBuf<ClsFast> d_cls_fast;           /* per hardware class */
+    DevBuf<uint32_t> d_sigs;              /* per-NUMA NIC signatures */
+    DevBuf<uint8_t> d_mapt;               /* GetNumaGroupIdx table of the direct path */
+    uint8_t* d_mapt2 = nullptr;           /* ... with the GPU stage (resolve_kernel); the device's shared copy, not owned */
+    DevBuf<uint64_t> d_memo;
+    DevBuf<int> d_vresult;
+    DevBuf<uint8_t> d_xchg;               /* node-sharded ranks: one slot per rank (summaries + bitmap columns) */
 
     /* staging for records (AoS) */
-    void* d_stage = nullptr;  size_t d_stage_cap = 0;
-    void* h_stage = nullptr;  size_t h_stage_cap = 0;
-    int32_t* d_idx = nullptr; size_t d_idx_cap = 0;
+    DevBuf<uint8_t> d_stage;
+    PinnedBuf<uint8_t> h_stage;
+    DevBuf<int32_t> d_idx;
 
-    /* batch */
-    int n_pods = 0, n_types = 0;
+    Workspace batch, scratch;
     bool staged = false, solved = false;
-    PodType* d_types = nullptr;     size_t types_cap = 0;
-    int32_t* d_pod_type = nullptr;  double* d_now = nullptr;  nhd_binding* d_out = nullptr;  size_t pods_cap = 0;
-    uint8_t* h_batch = nullptr;     size_t h_batch_cap = 0;     /* pinned: types | pod_type | now */
-    nhd_binding* h_out = nullptr;   size_t h_out_cap = 0;       /* pinned */
-    uint64_t* d_bitmaps = nullptr;  size_t bitmaps_cap = 0;
-    int32_t* d_cursors = nullptr;   size_t cursors_cap = 0;
-    int32_t* d_busy_list = nullptr;
-    int32_t* d_pend = nullptr;
-    uint4* d_dyn = nullptr;
-    uint16_t* d_class = nullptr;
-    ClassSlot* d_class_slots = nullptr;
-    unsigned long long* d_prof = nullptr;
-    int* d_vresult = nullptr;
-    uint64_t* d_memo = nullptr;
-    uint8_t* d_xchg = nullptr;  size_t xchg_cap = 0;     /* node-sharded ranks: one slot per rank (summaries + bitmap columns) */
-    uint8_t* d_ftab = nullptr;            /* direct-path tables of the staged batch's pod types */
-    uint8_t* d_mapt = nullptr;            /* GetNumaGroupIdx table of the direct path */
-    uint8_t* d_mapt2 = nullptr;           /* ... with the GPU stage (resolve_kernel); the device's shared copy, not owned */
-    uint32_t* d_sigs = nullptr;           /* per-NUMA NIC signatures */
-    ClsFast* d_cls_fast = nullptr;        /* per hardware class */
-    double now0 = 0.0;
-    bool const_clock = true;
+#ifdef NHD_CHECKS
+    unsigned long long* d_prof = nullptr;  /* the batch's sweep counters, mapped host: readable after a device fault */
+#endif
     long long shard_min_pairs = 1LL << 21;   /* nhd_shard_min_pairs() when the handle was created */
-    int n_names = 0;
-    uint64_t names_used = 0;
-    uint64_t* d_pod_groups = nullptr; size_t pod_groups_cap = 0;
-    std::vector<int32_t> pod_type_host;
 
     /* Generation of the device mirror: every call that changes it (or the staged batch) takes a new value.  The
      * explanations need the snapshot to be the batch's starting state and the mirror to hold exactly that batch's
@@ -126,37 +179,22 @@ struct nhd_handle {
     uint64_t gen = 1, snap_gen = 0, stage_gen = 0, explain_gen = 0;
     bool batch_on_snapshot = false;
     /* explanation scratch: per-node placement lists (CSR), the failed pods, per-pod counts, one pod's node reasons */
-    int32_t* d_xnode = nullptr;   size_t xnode_cap = 0;      /* node_cnt | node_start | cursor */
-    int32_t* d_xpod = nullptr;    size_t xpod_cap = 0;       /* node_pods | failed */
-    uint32_t* d_xcounts = nullptr; size_t xcounts_cap = 0;
-    uint8_t* d_xreasons = nullptr; size_t xreasons_cap = 0;
-    uint32_t* d_xsmall = nullptr;                             /* n_failed, survivors */
+    DevBuf<int32_t> d_xnode;              /* node_cnt | node_start | cursor */
+    DevBuf<int32_t> d_xpod;               /* node_pods | failed */
+    DevBuf<uint32_t> d_xcounts;
+    DevBuf<uint8_t> d_xreasons;
+    DevBuf<uint32_t> d_xsmall;            /* n_failed, survivors */
 
     /* Records generation: load and update change it, snapshot remembers it.  A query of the snapshot needs the two
      * equal, so that the nodes' hardware classes (d_class, d_cls_fast, d_sigs: the mirror's) describe the snapshot. */
     uint64_t rec_gen = 1, snap_rec_gen = 0;
-    /* query scratch (nhd_query_batch): its own pod types, per-pod arrays, bitmaps, summaries and tables, so that a
-     * query leaves the staged batch, its bindings and its filter output alone */
-    PodType* d_qtypes = nullptr;    size_t qtypes_cap = 0;
-    uint8_t* d_qpods = nullptr;     size_t qpods_cap = 0;        /* pod_type | now | group masks */
-    nhd_binding* d_qout = nullptr;  size_t qout_cap = 0;
-    uint8_t* h_q = nullptr;         size_t h_q_cap = 0;           /* pinned: types | pod_type | now | group masks */
-    nhd_binding* h_qout = nullptr;  size_t h_qout_cap = 0;        /* pinned */
-    uint64_t* d_qbitmaps = nullptr; size_t qbitmaps_cap = 0;
-    uint4* d_qdyn = nullptr;        size_t qdyn_cap = 0;
-    uint8_t* d_qftab = nullptr;
-    /* plan scratch (nhd_plan_batch), on top of the query's: the sweep's cursors, busy list and pend, its debug
-     * counters, and the copy of the records the excluded nodes are flagged in */
-    int32_t* d_pcursors = nullptr;  size_t pcursors_cap = 0;
-    int32_t* d_pbusy = nullptr;     size_t pbusy_cap = 0;
-    int32_t* d_ppend = nullptr;     size_t ppend_cap = 0;
-    unsigned long long* d_pprof = nullptr;
-    uint8_t* d_pnodes = nullptr;    size_t pnodes_cap = 0;
-    int32_t* d_pidx = nullptr;      size_t pidx_cap = 0;
-    /* scenario scratch (nhd_plan_scenarios), on top of the query's: pod offsets | exclusion offsets | exclusions |
-     * slot nodes | the failed-mapping word, and one working record per pod */
-    int32_t* d_sidx = nullptr;      size_t sidx_cap = 0;
-    uint4* d_swork = nullptr;       size_t swork_cap = 0;
+    /* a plan's copy of the records, with its excluded nodes flagged there, and their indices */
+    DevBuf<uint8_t> d_pnodes;
+    DevBuf<int32_t> d_pidx;
+    /* scenario plans: pod offsets | exclusion offsets | exclusions | edit offsets | edited nodes | lift indices | slot
+     * nodes | the failed-mapping word, and one working record per slot followed by the edit records */
+    DevBuf<int32_t> d_sidx;
+    DevBuf<uint4> d_swork;
 
     nhd_timing timing;
     std::string err;
@@ -181,30 +219,13 @@ static int32_t fail(nhd_handle* h, int32_t code, const char* fmt, ...)
                         __FILE__, __LINE__);                                                       \
     } while (0)
 
-template <typename T>
-static cudaError_t grow_dev(T*& p, size_t& cap, size_t need)
+/* the sweep's debug counters of w: a check build keeps the batch's in mapped host memory (nhd_create) */
+static unsigned long long* counters(nhd_handle* h, Workspace& w)
 {
-    if (need <= cap) return cudaSuccess;
-    if (p) cudaFree(p);
-    p = nullptr;
-    cap = 0;
-    size_t want = std::max(need, (size_t)256);
-    cudaError_t e = cudaMalloc((void**)&p, want);
-    if (e == cudaSuccess) cap = want;
-    return e;
-}
-
-template <typename T>
-static cudaError_t grow_pinned(T*& p, size_t& cap, size_t need)
-{
-    if (need <= cap) return cudaSuccess;
-    if (p) cudaFreeHost(p);
-    p = nullptr;
-    cap = 0;
-    size_t want = std::max(need, (size_t)256);
-    cudaError_t e = cudaMallocHost((void**)&p, want);
-    if (e == cudaSuccess) cap = want;
-    return e;
+#ifdef NHD_CHECKS
+    if (&w == &h->batch) return h->d_prof;
+#endif
+    return w.prof;
 }
 
 /* ------------------------------------------------------------------ validation */
@@ -333,27 +354,15 @@ extern "C" int32_t nhd_destroy(nhd_handle* h)
     if (h->comm && g_nccl.CommDestroy) g_nccl.CommDestroy(h->comm);
     cudaSetDevice(h->params.device);
     if (h->stream) cudaStreamSynchronize(h->stream);
-    cudaFree(h->d_nodes); cudaFree(h->d_snapshot); cudaFree(h->d_stage); cudaFree(h->d_idx);
-    cudaFree(h->d_types); cudaFree(h->d_pod_type); cudaFree(h->d_now); cudaFree(h->d_out);
-    cudaFree(h->d_bitmaps); cudaFree(h->d_cursors); cudaFree(h->d_busy_list); cudaFree(h->d_memo); cudaFree(h->d_dyn); cudaFree(h->d_class); cudaFree(h->d_class_slots); cudaFree(h->d_mapt); cudaFree(h->d_ftab); cudaFree(h->d_xchg); cudaFree(h->d_sigs); cudaFree(h->d_cls_fast); 
 #ifdef NHD_CHECKS
     cudaFreeHost(h->d_prof);
-#else
-    cudaFree(h->d_prof);
 #endif
-    cudaFree(h->d_pend); cudaFree(h->d_vresult); cudaFree(h->d_pod_groups);
-    cudaFree(h->d_xnode); cudaFree(h->d_xpod); cudaFree(h->d_xcounts); cudaFree(h->d_xreasons); cudaFree(h->d_xsmall);
-    cudaFree(h->d_qtypes); cudaFree(h->d_qpods); cudaFree(h->d_qout); cudaFree(h->d_qbitmaps); cudaFree(h->d_qdyn); cudaFree(h->d_qftab);
-    cudaFree(h->d_pcursors); cudaFree(h->d_pbusy); cudaFree(h->d_ppend); cudaFree(h->d_pprof); cudaFree(h->d_pnodes); cudaFree(h->d_pidx);
-    cudaFree(h->d_sidx); cudaFree(h->d_swork);
-    if (h->h_q) cudaFreeHost(h->h_q);
-    if (h->h_qout) cudaFreeHost(h->h_qout);
-    if (h->h_stage) cudaFreeHost(h->h_stage);
-    if (h->h_batch) cudaFreeHost(h->h_batch);
-    if (h->h_out) cudaFreeHost(h->h_out);
-    for (auto& e : h->ev) if (e) cudaEventDestroy(e);
-    if (h->stream) cudaStreamDestroy(h->stream);
-    delete h;
+    const cudaStream_t stream = h->stream;
+    cudaEvent_t ev[4];
+    std::copy(std::begin(h->ev), std::end(h->ev), ev);
+    delete h;                                            /* frees every buffer */
+    for (auto& e : ev) if (e) cudaEventDestroy(e);
+    if (stream) cudaStreamDestroy(stream);
     return NHD_OK;
 }
 
@@ -384,23 +393,22 @@ extern "C" int32_t nhd_create(const nhd_params* p, nhd_handle** out)
     h->smem_optin = (int)prop.sharedMemPerBlockOptin;
     CK(cudaStreamCreateWithFlags(&h->stream, cudaStreamNonBlocking));
     for (auto& ev : h->ev) CK(cudaEventCreate(&ev));
-    CK(cudaMalloc((void**)&h->d_memo, (size_t)MEMO_SLOTS * 16));
+    CK(h->d_memo.grow((size_t)MEMO_SLOTS * 16));
     CK(cudaMemsetAsync(h->d_memo, 0, (size_t)MEMO_SLOTS * 16, h->stream));
-    CK(cudaMalloc((void**)&h->d_vresult, 16));
+    CK(h->d_vresult.grow(16));
 #ifdef NHD_CHECKS
     CK(cudaHostAlloc((void**)&h->d_prof, 64 * 8, cudaHostAllocMapped));      /* readable after a device fault */
     memset(h->d_prof, 0, 64 * 8);
 #else
-    CK(cudaMalloc((void**)&h->d_prof, 64 * 8));
-    CK(cudaMemsetAsync(h->d_prof, 0, 64 * 8, h->stream));
+    CK(h->batch.prof.grow(64 * 8));
+    CK(cudaMemsetAsync(h->batch.prof, 0, 64 * 8, h->stream));
 #endif
-    CK(cudaMalloc((void**)&h->d_class_slots, (size_t)CLASS_SLOTS * sizeof(ClassSlot)));
+    CK(h->d_class_slots.grow((size_t)CLASS_SLOTS * sizeof(ClassSlot)));
     CK(cudaMemsetAsync(h->d_class_slots, 0, (size_t)CLASS_SLOTS * sizeof(ClassSlot), h->stream));
-    CK(cudaMalloc((void**)&h->d_mapt, (size_t)((MAPT_BYTES + 15) & ~15)));
-    CK(cudaMalloc((void**)&h->d_ftab, ftab_bytes(FAST_MAX_TYPES)));
-    CK(cudaMalloc((void**)&h->d_sigs, (size_t)FAST_NSIG * 4));
+    CK(h->d_mapt.grow((size_t)((MAPT_BYTES + 15) & ~15)));
+    CK(h->d_sigs.grow((size_t)FAST_NSIG * 4));
     CK(cudaMemsetAsync(h->d_sigs, 0, (size_t)FAST_NSIG * 4, h->stream));
-    CK(cudaMalloc((void**)&h->d_cls_fast, (size_t)CLASS_SLOTS * sizeof(ClsFast)));
+    CK(h->d_cls_fast.grow((size_t)CLASS_SLOTS * sizeof(ClsFast)));
     CK(cudaMemsetAsync(h->d_cls_fast, 0, (size_t)CLASS_SLOTS * sizeof(ClsFast), h->stream));
     mapt_kernel<<<(MAPT_BYTES + 127) / 128, 128, 0, h->stream>>>(h->d_mapt);
     CK(cudaGetLastError());
@@ -414,7 +422,7 @@ extern "C" int32_t nhd_create(const nhd_params* p, nhd_handle** out)
          * real batch instead of inside it (a first sweep used to take tens of milliseconds) */
         SweepArgs sa;
         memset(&sa, 0, sizeof(sa));
-        sa.prof = h->d_prof;                               /* (profile builds flush their counters) */
+        sa.prof = counters(h, h->batch);                   /* (profile builds flush their counters) */
         const size_t smem = (size_t)SMEMO_SLOTS * 16 + (size_t)DMEMO_SLOTS * 48 + (size_t)DCACHE_SLOTS * 36 + 16 +
                             (size_t)CLSNIC_SLOTS * 48 + (size_t)SPMEMO_SLOTS * 16 + ((MAPT_BYTES + 15) & ~15) + 4096;
         sweep_kernel<true><<<1, SWEEP_THREADS, smem, h->stream>>>(sa);
@@ -449,24 +457,24 @@ static int32_t upload_records(nhd_handle* h, int n, const nhd_node_rec* recs, co
                               bool track_while_copying = false)
 {
     const size_t bytes = (size_t)n * sizeof(nhd_node_rec);
-    CK(grow_dev(h->d_stage, h->d_stage_cap, bytes));
+    CK(h->d_stage.grow(bytes));
     const void* src = recs;
     if (!is_pinned_host(recs)) {
-        CK(grow_pinned(h->h_stage, h->h_stage_cap, bytes));
+        CK(h->h_stage.grow(bytes));
         memcpy(h->h_stage, recs, bytes);
         src = h->h_stage;
     }
     CK(cudaMemcpyAsync(h->d_stage, src, bytes, cudaMemcpyHostToDevice, h->stream));
     const int32_t* d_idx = nullptr;
     if (idx) {
-        CK(grow_dev(h->d_idx, h->d_idx_cap, (size_t)n * 4));
+        CK(h->d_idx.grow((size_t)n * 4));
         CK(cudaMemcpyAsync(h->d_idx, idx, (size_t)n * 4, cudaMemcpyHostToDevice, h->stream));
         d_idx = h->d_idx;
     }
     const int threads = 256;
     int vinit[4] = {0x7FFFFFFF, 0, 1, 0};
     CK(cudaMemcpyAsync(h->d_vresult, vinit, 16, cudaMemcpyHostToDevice, h->stream));
-    validate_kernel<<<(n + threads - 1) / threads, threads, 0, h->stream>>>((const nhd_node_rec*)h->d_stage, n, h->d_vresult);
+    validate_kernel<<<(n + threads - 1) / threads, threads, 0, h->stream>>>((const nhd_node_rec*)h->d_stage.p, n, h->d_vresult);
     CK(cudaGetLastError());
     int vres[4];
     CK(cudaMemcpyAsync(vres, h->d_vresult, 16, cudaMemcpyDeviceToHost, h->stream));
@@ -481,7 +489,7 @@ static int32_t upload_records(nhd_handle* h, int n, const nhd_node_rec* recs, co
     *max_numa = vres[2];
     const int total = n * REC_CHUNKS;
     ingest_kernel<<<(total + threads - 1) / threads, threads, 0, h->stream>>>(
-        (const uint4*)h->d_stage, d_idx, n, h->d_nodes);
+        (const uint4*)h->d_stage.p, d_idx, n, h->d_nodes);
     CK(cudaGetLastError());
     /* hardware classes of the (re)written nodes */
     classify_claim_kernel<<<(n + threads - 1) / threads, threads, 0, h->stream>>>(h->d_nodes, d_idx, n, h->d_class_slots, h->d_class);
@@ -502,15 +510,11 @@ extern "C" int32_t nhd_load_nodes(nhd_handle* h, int32_t n_nodes, const nhd_node
     const int n_super = std::max(1, (n_nodes + SUPER_NODES - 1) / SUPER_NODES);
     const size_t bytes = (size_t)n_super * SUPER_BYTES;
     if (bytes != h->nodes_bytes) {
-        cudaFree(h->d_nodes); cudaFree(h->d_snapshot); cudaFree(h->d_busy_list); cudaFree(h->d_dyn); cudaFree(h->d_class); cudaFree(h->d_pend);
-        h->d_nodes = h->d_snapshot = nullptr; h->d_busy_list = nullptr; h->d_dyn = nullptr; h->d_class = nullptr; h->d_pend = nullptr;
+        h->d_nodes.release(); h->d_snapshot.release(); h->d_class.release();
         h->nodes_bytes = 0;
-        CK(cudaMalloc((void**)&h->d_nodes, bytes));
-        CK(cudaMalloc((void**)&h->d_snapshot, bytes));
-        CK(cudaMalloc((void**)&h->d_busy_list, ((size_t)n_super * SUPER_NODES + 64) * 4));
-        CK(cudaMalloc((void**)&h->d_dyn, (size_t)n_super * SUPER_NODES * sizeof(NodeDyn)));
-        CK(cudaMalloc((void**)&h->d_class, (size_t)n_super * SUPER_NODES * sizeof(uint16_t)));
-        CK(cudaMalloc((void**)&h->d_pend, (size_t)n_super * SUPER_NODES * sizeof(int32_t)));
+        CK(h->d_nodes.grow(bytes));
+        CK(h->d_snapshot.grow(bytes));
+        CK(h->d_class.grow((size_t)n_super * SUPER_NODES * sizeof(uint16_t)));
         h->nodes_bytes = bytes;
     }
     h->n_nodes = n_nodes;
@@ -563,10 +567,10 @@ extern "C" int32_t nhd_read_nodes(nhd_handle* h, int32_t first, int32_t n, nhd_n
     if (n == 0) return NHD_OK;
     CK(cudaSetDevice(h->params.device));
     const size_t bytes = (size_t)n * sizeof(nhd_node_rec);
-    CK(grow_dev(h->d_stage, h->d_stage_cap, bytes));
-    CK(grow_pinned(h->h_stage, h->h_stage_cap, bytes));
+    CK(h->d_stage.grow(bytes));
+    CK(h->h_stage.grow(bytes));
     const int threads = 256, total = n * REC_CHUNKS;
-    export_kernel<<<(total + threads - 1) / threads, threads, 0, h->stream>>>(h->d_nodes, first, n, (uint4*)h->d_stage);
+    export_kernel<<<(total + threads - 1) / threads, threads, 0, h->stream>>>(h->d_nodes, first, n, (uint4*)h->d_stage.p);
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(h->h_stage, h->d_stage, bytes, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
@@ -705,65 +709,62 @@ static int32_t make_pod_types(nhd_handle* h, int n_pods, const nhd_pod* pods, co
     return NHD_OK;
 }
 
+/*
+ * Validate a pod set, de-duplicate it into pod types (tuple limits judged against max_numa) and copy it into w: the
+ * types, then pod_type | now | group masks, through w's pinned staging.  Every buffer of w is sized here, from the
+ * pod set and n_super, so that no allocation falls inside the solve that follows.
+ */
+static int32_t stage_pods(nhd_handle* h, Workspace& w, int n, const nhd_pod* pods, const double* now, int max_numa)
+{
+    uint64_t names_used = 0;
+    const bool multi_group = group_lists(n, pods, &names_used);
+    std::vector<PodType> types;
+    const int32_t rc = make_pod_types(h, n, pods, now, multi_group, max_numa, types, w.pod_type_host);
+    if (rc != NHD_OK) return rc;
+    CK(cudaSetDevice(h->params.device));
+    const int T = (int)types.size();
+    w.n_pods = n;
+    w.n_types = T;
+    w.n_names = multi_group ? __builtin_popcountll(names_used) : 0;
+    w.names_used = multi_group ? names_used : 0;
+    w.now0 = n ? now[0] : 0.0;
+    w.const_clock = true;
+    for (int i = 1; i < n; i++) if (now[i] != now[0]) { w.const_clock = false; break; }
+
+    const size_t types_bytes = (size_t)T * sizeof(PodType), off_now = w.now_offset(), off_gm = off_now + (size_t)n * 8;
+    const size_t pods_bytes = off_gm + (w.n_names ? (size_t)n * 8 : 0), n_slots = (size_t)h->n_super * SUPER_NODES;
+    CK(w.staging.grow(types_bytes + pods_bytes));
+    CK(w.types.grow(types_bytes));
+    CK(w.pod_arrays.grow(pods_bytes));
+    CK(w.bitmaps.grow((size_t)(T + 2 + w.n_names) * h->words * 8));
+    CK(w.dyn.grow(n_slots * sizeof(NodeDyn)));
+    CK(w.ftab.grow(ftab_bytes(FAST_MAX_TYPES)));
+    CK(w.cursors.grow((size_t)std::max(T, 1) * 3 * 4));
+    CK(w.busy_list.grow((n_slots + 64) * 4));
+    CK(w.pend.grow(n_slots * 4));
+    CK(w.prof.grow(64 * 8));
+    CK(w.out.grow(((size_t)n + 8) * sizeof(nhd_binding)));
+    if (n == 0) return NHD_OK;
+    uint8_t* hp = w.staging + types_bytes;
+    memcpy(w.staging, types.data(), types_bytes);
+    memcpy(hp, w.pod_type_host.data(), (size_t)n * 4);
+    memcpy(hp + off_now, now, (size_t)n * 8);
+    if (w.n_names)
+        for (int i = 0; i < n; i++) memcpy(hp + off_gm + (size_t)i * 8, &pods[i].group_mask, 8);
+    CK(cudaMemcpyAsync(w.types, w.staging, types_bytes, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(w.pod_arrays, hp, pods_bytes, cudaMemcpyHostToDevice, h->stream));
+    return NHD_OK;
+}
+
 extern "C" int32_t nhd_stage_batch(nhd_handle* h, int32_t n_pods, const nhd_pod* pods, const double* now)
 {
     if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now))) return NHD_ERR_INVALID;
     if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_stage_batch before nhd_load_nodes");
     const bool on_snapshot = h->gen == h->snap_gen;
     h->gen++;
-    CK(cudaSetDevice(h->params.device));
     h->staged = h->solved = false;
-
-    uint64_t names_used = 0;
-    const bool multi_group = group_lists(n_pods, pods, &names_used);
-    h->n_names = 0;
-    h->names_used = 0;
-    if (multi_group) {
-        h->names_used = names_used;
-        h->n_names = __builtin_popcountll(names_used);
-    }
-    std::vector<PodType> types;
-    const int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, h->max_numa, types, h->pod_type_host);
+    const int32_t rc = stage_pods(h, h->batch, n_pods, pods, now, h->max_numa);
     if (rc != NHD_OK) return rc;
-    const int T = (int)types.size();
-    const size_t types_bytes = (size_t)T * sizeof(PodType);
-    const size_t off_pt = (types_bytes + 15) & ~(size_t)15;
-    const size_t off_now = (off_pt + (size_t)n_pods * 4 + 15) & ~(size_t)15;
-    const size_t total = off_now + (size_t)n_pods * 8;
-    CK(grow_pinned(h->h_batch, h->h_batch_cap, total));
-    if (T) memcpy(h->h_batch, types.data(), types_bytes);
-    if (n_pods) {
-        memcpy(h->h_batch + off_pt, h->pod_type_host.data(), (size_t)n_pods * 4);
-        memcpy(h->h_batch + off_now, now, (size_t)n_pods * 8);
-    }
-    CK(grow_dev(h->d_types, h->types_cap, types_bytes));
-    if ((size_t)n_pods > h->pods_cap) {
-        cudaFree(h->d_pod_type); cudaFree(h->d_now); cudaFree(h->d_out);
-        h->d_pod_type = nullptr; h->d_now = nullptr; h->d_out = nullptr; h->pods_cap = 0;
-        CK(cudaMalloc((void**)&h->d_pod_type, (size_t)n_pods * 4));
-        CK(cudaMalloc((void**)&h->d_now, (size_t)n_pods * 8));
-        CK(cudaMalloc((void**)&h->d_out, ((size_t)n_pods + 8) * sizeof(nhd_binding)));      /* + spare records for check builds */
-        h->pods_cap = n_pods;
-    }
-    CK(grow_dev(h->d_bitmaps, h->bitmaps_cap, (size_t)(T + 2 + h->n_names) * h->words * 8));
-    if (multi_group) {
-        CK(grow_dev(h->d_pod_groups, h->pod_groups_cap, (size_t)n_pods * 8));
-        std::vector<uint64_t> gm(n_pods);
-        for (int i = 0; i < n_pods; i++) gm[i] = pods[i].group_mask;
-        CK(cudaMemcpyAsync(h->d_pod_groups, gm.data(), (size_t)n_pods * 8, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaStreamSynchronize(h->stream));
-    }
-    CK(grow_dev(h->d_cursors, h->cursors_cap, (size_t)std::max(T, 1) * 3 * 4));
-    if (T) CK(cudaMemcpyAsync(h->d_types, h->h_batch, types_bytes, cudaMemcpyHostToDevice, h->stream));
-    if (n_pods) {
-        CK(cudaMemcpyAsync(h->d_pod_type, h->h_batch + off_pt, (size_t)n_pods * 4, cudaMemcpyHostToDevice, h->stream));
-        CK(cudaMemcpyAsync(h->d_now, h->h_batch + off_now, (size_t)n_pods * 8, cudaMemcpyHostToDevice, h->stream));
-    }
-    h->n_pods = n_pods;
-    h->n_types = T;
-    h->now0 = n_pods ? now[0] : 0.0;
-    h->const_clock = true;
-    for (int i = 1; i < n_pods; i++) if (now[i] != now[0]) { h->const_clock = false; break; }
     h->staged = true;
     h->batch_on_snapshot = on_snapshot;
     h->stage_gen = h->gen;
@@ -779,52 +780,17 @@ extern "C" int32_t nhd_run_filter_only(nhd_handle* h)
     return nhd_sync(h);
 }
 
-/* One solve's inputs and outputs on the device: the records it starts from, the pod set, and every buffer its kernels
- * write.  A batch runs on the handle's own buffers (batch_work); a plan on the query scratch plus its own sweep buffers
- * (nhd_plan_batch), so that it leaves the staged batch, its bindings and its filter output alone. */
-struct SolveWork {
-    uint8_t* nodes;                   /* records at the start of the solve (tiled); only a batch's commit writes them */
-    const PodType* types;
-    const int32_t* pod_type;
-    const double* now;
-    const uint64_t* pod_groups;       /* per-pod node-group masks when n_names > 0, else null */
-    int n_pods, n_types, n_names;
-    uint64_t names_used;
-    double now0;                      /* clock of the first pod (the filter's BUSY row) */
-    bool const_clock;
-    uint64_t* bitmaps;                /* [n_types + 2 + n_names][words] */
-    uint4* dyn;                       /* NodeDyn summaries */
-    int32_t* cursors;                 /* [max(n_types, 1)][3] */
-    int32_t* busy_list;               /* n_super * SUPER_NODES + 64 */
-    int32_t* pend;                    /* n_super * SUPER_NODES */
-    uint8_t* ftab;                    /* ftab_bytes(FAST_MAX_TYPES) */
-    nhd_binding* out;                 /* n_pods + 8 (spare records for check builds) */
-    unsigned long long* prof;         /* the sweep's debug counters (nhd_debug_counters reads the batch's) */
-};
-
-static SolveWork batch_work(nhd_handle* h, uint8_t* records)
-{
-    SolveWork w;
-    w.nodes = records; w.types = h->d_types; w.pod_type = h->d_pod_type; w.now = h->d_now;
-    w.pod_groups = h->n_names ? h->d_pod_groups : nullptr;
-    w.n_pods = h->n_pods; w.n_types = h->n_types; w.n_names = h->n_names; w.names_used = h->names_used;
-    w.now0 = h->now0; w.const_clock = h->const_clock;
-    w.bitmaps = h->d_bitmaps; w.dyn = h->d_dyn; w.cursors = h->d_cursors; w.busy_list = h->d_busy_list; w.pend = h->d_pend;
-    w.ftab = h->d_ftab; w.out = h->d_out; w.prof = h->d_prof;
-    return w;
-}
-
 /*
- * The launches of a solve on one workspace: direct-path tables, filter, sweep, resolve, core ids.  batch = the handle's
- * staged batch: its timing events, the node-sharded filter + exchange when world_size > 1, and commit_kernel, which
- * folds the bindings into w.nodes.  Without it (a plan, or a query's filter) none of the three: every rank filters the
- * whole cluster and the records are only read.  filter_only stops after the filter.
+ * The launches of a solve of w's pod set on the records nodes: direct-path tables, filter, sweep, resolve, core ids.
+ * batch = the handle's staged batch on the mirror: its timing events, the node-sharded filter + exchange when
+ * world_size > 1, and commit_kernel, which folds the bindings into the mirror.  Without it (a plan, or a query's
+ * filter) none of the three: every rank filters the whole cluster and the records are only read.  filter_only stops
+ * after the filter.
  */
-static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool filter_only)
+static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, bool batch, bool filter_only)
 {
     const int T = w.n_types, W = h->words;
     int launches = 0;
-    if (batch) CK(cudaEventRecord(h->ev[0], h->stream));
 
     /* 1. snapshot predicate kernel over this rank's node shard.  With several ranks every rank filters the nodes
      * of S consecutive super-tiles into its slot of an exchange buffer (their NodeDyn summaries, then their
@@ -839,7 +805,8 @@ static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool 
     const int super_lo = sharded ? std::min(rk * S, h->n_super) : 0;
     const int super_hi = sharded ? std::min(super_lo + S, h->n_super) : h->n_super;
     const size_t slot_bytes = (size_t)S * 32 * (SUPER_NODES + rows);
-    if (sharded) CK(grow_dev(h->d_xchg, h->xchg_cap, slot_bytes * ws));
+    if (sharded) CK(h->d_xchg.grow(slot_bytes * ws));
+    if (batch) CK(cudaEventRecord(h->ev[0], h->stream));
     const bool have_ftab = T > 0 && T <= FAST_MAX_TYPES;
     if (w.n_pods > 0 && have_ftab) {
         /* 0. the direct-path tables of this batch's pod types (filter and sweep both read them) */
@@ -852,8 +819,8 @@ static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool 
     }
     if (w.n_pods > 0 && super_hi > super_lo) {
         FilterArgs fa;
-        fa.ftab = have_ftab ? w.ftab : nullptr; fa.mapt = h->d_mapt; fa.cls = h->d_cls_fast;
-        fa.nodes = w.nodes; fa.types = w.types; fa.n_types = T; fa.n_nodes = h->n_nodes;
+        fa.ftab = have_ftab ? w.ftab.p : nullptr; fa.mapt = h->d_mapt; fa.cls = h->d_cls_fast;
+        fa.nodes = nodes; fa.types = w.types; fa.n_types = T; fa.n_nodes = h->n_nodes;
         fa.super_lo = super_lo; fa.super_hi = super_hi;
         if (sharded) {
             uint8_t* slot = h->d_xchg + slot_bytes * rk;
@@ -882,8 +849,10 @@ static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool 
         ncclResult_t_ r = g_nccl.AllGather(h->d_xchg + slot_bytes * rk, h->d_xchg, slot_bytes, NCCL_INT8, h->comm, h->stream);
         if (r != 0) return fail(h, NHD_ERR_NCCL, "ncclAllGather: %s", g_nccl.GetErrorString ? g_nccl.GetErrorString(r) : "?");
         const size_t n16 = slot_bytes / 16 * ws;
-        unpack_slots_kernel<<<(unsigned)((n16 + 255) / 256), 256, 0, h->stream>>>(reinterpret_cast<const uint4*>(h->d_xchg), ws, S, h->n_super,
-                                                                              rows, W, w.dyn, w.bitmaps);
+        uint4* const dyn = w.dyn;
+        uint64_t* const bitmaps = w.bitmaps;
+        unpack_slots_kernel<<<(unsigned)((n16 + 255) / 256), 256, 0, h->stream>>>(reinterpret_cast<const uint4*>(h->d_xchg.p), ws, S, h->n_super,
+                                                                              rows, W, dyn, bitmaps);
         CK(cudaGetLastError());
         launches += 2;
     }
@@ -891,10 +860,12 @@ static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool 
 
     /* 3. sequential select + assign sweep (replicated on every rank) */
     if (w.n_pods > 0 && !filter_only) {
+        /* (the sweep's and the finishing kernels' record pointer is writable for commit_kernel, which only a batch runs) */
+        uint8_t* const records = const_cast<uint8_t*>(nodes);
         SweepArgs sa;
-        sa.nodes = w.nodes; sa.types = w.types; sa.pod_type = w.pod_type; sa.now = w.now; sa.out = w.out;
+        sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type(); sa.now = w.now(); sa.out = w.out;
         sa.n_pods = w.n_pods; sa.n_types = T; sa.n_nodes = h->n_nodes; sa.words = W;
-        sa.n_names = w.n_names; sa.names_used = w.names_used; sa.pod_groups = w.pod_groups;
+        sa.n_names = w.n_names; sa.names_used = w.names_used; sa.pod_groups = w.pod_groups();
         /* reserved_ (test knobs; every setting gives the same bindings): low byte 0 = default, 1 = the general one-warp
          * sweep only (no standing decisions), 2 = standing decisions but never the two pod classes side by side;
          * bits 8.. = debug switches of sweep_kernel */
@@ -903,9 +874,9 @@ static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool 
         sa.bitmaps = w.bitmaps; sa.dyn = w.dyn; sa.cursors = w.cursors; sa.busy_list = w.busy_list;
         /* the mapping memo is a pure cache of choose_mapping (its key holds every input: K, G and the three stage
          * masks), so every workspace shares the handle's */
-        sa.memo = h->d_memo; sa.prof = w.prof; sa.pend_pod = w.pend;
+        sa.memo = h->d_memo; sa.prof = counters(h, w); sa.pend_pod = w.pend;
         sa.mapt = h->d_mapt; sa.mapt2 = h->d_mapt2; sa.sigs = h->d_sigs; sa.cls_fast = h->d_cls_fast;
-        sa.ftab = (T > 0 && T <= FAST_MAX_TYPES) ? w.ftab : nullptr;
+        sa.ftab = (T > 0 && T <= FAST_MAX_TYPES) ? w.ftab.p : nullptr;
         sa.min_busy = h->params.min_busy_secs;
         memcpy(sa.cap, h->cap, sizeof(sa.cap));
         /* shared memory: memo front | pod types | cursors | (bitmaps when they fit) */
@@ -926,7 +897,7 @@ static int32_t launch_solve(nhd_handle* h, const SolveWork& w, bool batch, bool 
         }
         CK(cudaGetLastError());
         FinishArgs fin;
-        fin.nodes = w.nodes; fin.types = w.types; fin.pod_type = w.pod_type; fin.out = w.out;
+        fin.nodes = records; fin.types = w.types; fin.pod_type = w.pod_type(); fin.out = w.out;
         fin.dyn = w.dyn; fin.n_pods = w.n_pods;
         const int fthreads = 128, fgrid = (w.n_pods + fthreads - 1) / fthreads;
         resolve_kernel<<<(w.n_pods + 63) / 64, 64, 0, h->stream>>>(sa);
@@ -956,10 +927,31 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
     h->gen++;
     h->explain_gen = explainable ? h->gen : 0;
     CK(cudaSetDevice(h->params.device));
-    const int32_t rc = launch_solve(h, batch_work(h, h->d_nodes), true, filter_only);
+    const int32_t rc = launch_solve(h, h->batch, h->d_nodes, true, filter_only);
     if (rc != NHD_OK) return rc;
     h->solved = true;
     return NHD_OK;
+}
+
+/* device -> host: the first n bindings of w, through its bounce buffer unless out is pinned; waits for the device */
+static int32_t fetch_bindings(nhd_handle* h, Workspace& w, int n, nhd_binding* out)
+{
+    const size_t bytes = (size_t)n * sizeof(nhd_binding);
+    const bool direct = bytes == 0 || is_pinned_host(out);
+    if (!direct) CK(w.h_out.grow(bytes));
+    if (bytes) CK(cudaMemcpyAsync(direct ? (void*)out : (void*)w.h_out.p, w.out, bytes, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (!direct) memcpy(out, w.h_out, bytes);
+    return NHD_OK;
+}
+
+/* the batch's stage times, once its last event has completed */
+static void read_timing(nhd_handle* h)
+{
+    cudaEventElapsedTime(&h->timing.filter_ms, h->ev[0], h->ev[1]);
+    cudaEventElapsedTime(&h->timing.exchange_ms, h->ev[1], h->ev[2]);
+    cudaEventElapsedTime(&h->timing.sweep_ms, h->ev[2], h->ev[3]);
+    cudaEventElapsedTime(&h->timing.total_ms, h->ev[0], h->ev[3]);
 }
 
 extern "C" int32_t nhd_fetch_bindings(nhd_handle* h, nhd_binding* out)
@@ -967,20 +959,10 @@ extern "C" int32_t nhd_fetch_bindings(nhd_handle* h, nhd_binding* out)
     if (!h) return NHD_ERR_INVALID;
     if (!h->solved) return fail(h, NHD_ERR_STATE, "nhd_fetch_bindings without a solved batch");
     CK(cudaSetDevice(h->params.device));
-    const size_t bytes = (size_t)h->n_pods * sizeof(nhd_binding);
-    bool direct = false;
-    if (bytes) {
-        if (!out) return NHD_ERR_INVALID;
-        direct = is_pinned_host(out);
-        if (!direct) CK(grow_pinned(h->h_out, h->h_out_cap, bytes));
-        CK(cudaMemcpyAsync(direct ? (void*)out : (void*)h->h_out, h->d_out, bytes, cudaMemcpyDeviceToHost, h->stream));
-    }
-    CK(cudaStreamSynchronize(h->stream));
-    if (bytes && !direct) memcpy(out, h->h_out, bytes);
-    cudaEventElapsedTime(&h->timing.filter_ms, h->ev[0], h->ev[1]);
-    cudaEventElapsedTime(&h->timing.exchange_ms, h->ev[1], h->ev[2]);
-    cudaEventElapsedTime(&h->timing.sweep_ms, h->ev[2], h->ev[3]);
-    cudaEventElapsedTime(&h->timing.total_ms, h->ev[0], h->ev[3]);
+    if (h->batch.n_pods > 0 && !out) return NHD_ERR_INVALID;
+    const int32_t rc = fetch_bindings(h, h->batch, h->batch.n_pods, out);
+    if (rc != NHD_OK) return rc;
+    read_timing(h);
     return NHD_OK;
 }
 
@@ -989,12 +971,7 @@ extern "C" int32_t nhd_sync(nhd_handle* h)
     if (!h) return NHD_ERR_INVALID;
     CK(cudaSetDevice(h->params.device));
     CK(cudaStreamSynchronize(h->stream));
-    if (h->solved) {
-        cudaEventElapsedTime(&h->timing.filter_ms, h->ev[0], h->ev[1]);
-        cudaEventElapsedTime(&h->timing.exchange_ms, h->ev[1], h->ev[2]);
-        cudaEventElapsedTime(&h->timing.sweep_ms, h->ev[2], h->ev[3]);
-        cudaEventElapsedTime(&h->timing.total_ms, h->ev[0], h->ev[3]);
-    }
+    if (h->solved) read_timing(h);
     return NHD_OK;
 }
 
@@ -1019,17 +996,18 @@ extern "C" int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* wor
 {
     if (!h || !h->solved) return NHD_ERR_STATE;
     CK(cudaSetDevice(h->params.device));
-    if (n_types) *n_types = h->n_types;
+    const Workspace& w = h->batch;
+    if (n_types) *n_types = w.n_types;
     if (words_per_type) *words_per_type = h->words;
-    const int64_t need = (int64_t)(h->n_types + 2) * h->words;   /* group-name bitmaps are not exported */
+    const int64_t need = (int64_t)(w.n_types + 2) * h->words;    /* group-name bitmaps are not exported */
     if (words) {
         if (capacity_words < need) return NHD_ERR_INVALID;
-        CK(cudaMemcpyAsync(words, h->d_bitmaps, (size_t)need * 8, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaMemcpyAsync(words, w.bitmaps, (size_t)need * 8, cudaMemcpyDeviceToHost, h->stream));
         CK(cudaStreamSynchronize(h->stream));
     }
     if (pod_type) {
-        if (n_pods < h->n_pods) return NHD_ERR_INVALID;
-        memcpy(pod_type, h->pod_type_host.data(), (size_t)h->n_pods * 4);
+        if (n_pods < w.n_pods) return NHD_ERR_INVALID;
+        memcpy(pod_type, w.pod_type_host.data(), (size_t)w.n_pods * 4);
     }
     return NHD_OK;
 }
@@ -1044,14 +1022,15 @@ static int32_t explain_ready(nhd_handle* h)
     return NHD_OK;
 }
 
-/* The pods of a solve bound to each node, in pod order (CSR over w.out), and the list of NO_CANDIDATE pods.
+/* The pods of w's solve bound to each node, in pod order (CSR over w.out), and the list of NO_CANDIDATE pods.
  * Returns the number of NO_CANDIDATE pods in *n_failed. */
-static int32_t explain_prepare(nhd_handle* h, const SolveWork& w, int* n_failed)
+static int32_t explain_prepare(nhd_handle* h, const Workspace& w, int* n_failed)
 {
     const int N = h->n_nodes, P = w.n_pods;
-    CK(grow_dev(h->d_xnode, h->xnode_cap, ((size_t)3 * N + 2) * 4));
-    CK(grow_dev(h->d_xpod, h->xpod_cap, ((size_t)2 * P + 1) * 4));
-    if (!h->d_xsmall) CK(cudaMalloc((void**)&h->d_xsmall, 16));
+    const nhd_binding* out = w.out;
+    CK(h->d_xnode.grow(((size_t)3 * N + 2) * 4));
+    CK(h->d_xpod.grow(((size_t)2 * P + 1) * 4));
+    CK(h->d_xsmall.grow(16));
     int32_t* node_cnt = h->d_xnode;
     int32_t* node_start = h->d_xnode + N;            /* N + 1 entries */
     int32_t* cursor = h->d_xnode + 2 * N + 1;
@@ -1061,14 +1040,14 @@ static int32_t explain_prepare(nhd_handle* h, const SolveWork& w, int* n_failed)
     CK(cudaMemsetAsync(h->d_xsmall, 0, 16, h->stream));
     const int threads = 256;
     if (P > 0) {
-        explain_count_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(w.out, P, node_cnt, failed,
-                                                                                     (int32_t*)h->d_xsmall);
+        explain_count_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(out, P, node_cnt, failed,
+                                                                                     (int32_t*)h->d_xsmall.p);
         CK(cudaGetLastError());
     }
     explain_scan_kernel<<<1, EXPLAIN_SCAN_THREADS, 0, h->stream>>>(node_cnt, N, node_start, cursor);
     CK(cudaGetLastError());
     if (P > 0) {
-        explain_fill_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(w.out, P, cursor, node_pods);
+        explain_fill_kernel<<<(P + threads - 1) / threads, threads, 0, h->stream>>>(out, P, cursor, node_pods);
         CK(cudaGetLastError());
     }
     if (N > 0) {
@@ -1082,16 +1061,17 @@ static int32_t explain_prepare(nhd_handle* h, const SolveWork& w, int* n_failed)
     return NHD_OK;
 }
 
-/* one (failed pod x node) pass over a solve whose start records are w.nodes; counts and/or reasons may be null */
-static int32_t explain_launch(nhd_handle* h, const SolveWork& w, int n_failed, uint32_t* d_counts, uint8_t* d_reasons)
+/* one (failed pod x node) pass over w's solve, which started from the records nodes; counts and/or reasons may be null */
+static int32_t explain_launch(nhd_handle* h, const Workspace& w, const uint8_t* nodes, int n_failed, uint32_t* d_counts,
+                              uint8_t* d_reasons)
 {
     const int N = h->n_nodes, P = w.n_pods;
     if (n_failed == 0 || N == 0) return NHD_OK;
     ExplainArgs xa;
-    xa.snapshot = w.nodes; xa.types = w.types; xa.pod_type = w.pod_type; xa.now = w.now; xa.out = w.out;
-    xa.pod_groups = w.pod_groups;
+    xa.snapshot = nodes; xa.types = w.types; xa.pod_type = w.pod_type(); xa.now = w.now(); xa.out = w.out;
+    xa.pod_groups = w.pod_groups();
     xa.node_start = h->d_xnode + N; xa.node_pods = h->d_xpod; xa.failed = h->d_xpod + P;
-    xa.n_failed = (const int32_t*)h->d_xsmall;
+    xa.n_failed = (const int32_t*)h->d_xsmall.p;
     xa.n_nodes = N; xa.min_busy = h->params.min_busy_secs;
     memcpy(xa.cap, h->cap, sizeof(xa.cap));
     xa.counts = d_counts; xa.reasons = d_reasons; xa.survivors = h->d_xsmall + 1;
@@ -1112,28 +1092,29 @@ static int32_t explain_survivors(nhd_handle* h, const char* what)
     return NHD_OK;
 }
 
-/* per-reason node counts of every NO_CANDIDATE pod of the solve w into the host array counts (n_pods * NHD_WHY_COUNT) */
-static int32_t explain_counts(nhd_handle* h, const SolveWork& w, uint32_t* counts, const char* what)
+/* per-reason node counts of every NO_CANDIDATE pod of w's solve from the records nodes into the host array counts
+ * (n_pods * NHD_WHY_COUNT) */
+static int32_t explain_counts(nhd_handle* h, const Workspace& w, const uint8_t* nodes, uint32_t* counts, const char* what)
 {
     const size_t bytes = (size_t)w.n_pods * NHD_WHY_COUNT * 4;
     if (bytes == 0) return NHD_OK;
     int nf = 0;
     int32_t rc;
     if ((rc = explain_prepare(h, w, &nf)) != NHD_OK) return rc;
-    CK(grow_dev(h->d_xcounts, h->xcounts_cap, bytes));
+    CK(h->d_xcounts.grow(bytes));
     CK(cudaMemsetAsync(h->d_xcounts, 0, bytes, h->stream));
-    if ((rc = explain_launch(h, w, nf, h->d_xcounts, nullptr)) != NHD_OK) return rc;
+    if ((rc = explain_launch(h, w, nodes, nf, h->d_xcounts, nullptr)) != NHD_OK) return rc;
     CK(cudaMemcpyAsync(counts, h->d_xcounts, bytes, cudaMemcpyDeviceToHost, h->stream));
     return explain_survivors(h, what);
 }
 
 extern "C" int32_t nhd_explain_batch(nhd_handle* h, uint32_t* counts)
 {
-    if (!h || (h->n_pods > 0 && !counts)) return NHD_ERR_INVALID;
+    if (!h || (h->batch.n_pods > 0 && !counts)) return NHD_ERR_INVALID;
     int32_t rc = explain_ready(h);
     if (rc != NHD_OK) return rc;
     CK(cudaSetDevice(h->params.device));
-    return explain_counts(h, batch_work(h, h->d_snapshot), counts, "nhd_explain_batch");
+    return explain_counts(h, h->batch, h->d_snapshot, counts, "nhd_explain_batch");
 }
 
 extern "C" int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_reason)
@@ -1141,24 +1122,24 @@ extern "C" int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_rea
     if (!h || (h->n_nodes > 0 && !node_reason)) return NHD_ERR_INVALID;
     int32_t rc = explain_ready(h);
     if (rc != NHD_OK) return rc;
-    if (pod < 0 || pod >= h->n_pods) return fail(h, NHD_ERR_INVALID, "pod %d outside the batch of %d", pod, h->n_pods);
+    const Workspace& w = h->batch;
+    if (pod < 0 || pod >= w.n_pods) return fail(h, NHD_ERR_INVALID, "pod %d outside the batch of %d", pod, w.n_pods);
     CK(cudaSetDevice(h->params.device));
     int32_t status = 0;
-    CK(cudaMemcpyAsync(&status, &h->d_out[pod].status, 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(&status, &w.out[pod].status, 4, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     if (status != NHD_NO_CANDIDATE) {
         memset(node_reason, NHD_WHY_NONE, (size_t)h->n_nodes);
         return NHD_OK;
     }
-    const SolveWork w = batch_work(h, h->d_snapshot);
     int nf = 0;
     if ((rc = explain_prepare(h, w, &nf)) != NHD_OK) return rc;
     const int32_t one[1] = {pod};                    /* explain just this pod: failed[0] = pod, n_failed = 1 */
     const int32_t n1 = 1;
-    CK(cudaMemcpyAsync(h->d_xpod + h->n_pods, one, 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_xpod + w.n_pods, one, 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemcpyAsync(h->d_xsmall, &n1, 4, cudaMemcpyHostToDevice, h->stream));
-    CK(grow_dev(h->d_xreasons, h->xreasons_cap, (size_t)h->n_nodes));
-    if ((rc = explain_launch(h, w, 1, nullptr, h->d_xreasons)) != NHD_OK) return rc;
+    CK(h->d_xreasons.grow((size_t)h->n_nodes));
+    if ((rc = explain_launch(h, w, h->d_snapshot, 1, nullptr, h->d_xreasons)) != NHD_OK) return rc;
     CK(cudaMemcpyAsync(node_reason, h->d_xreasons, (size_t)h->n_nodes, cudaMemcpyDeviceToHost, h->stream));
     return explain_survivors(h, "nhd_explain_pod");
 }
@@ -1167,7 +1148,7 @@ extern "C" int32_t nhd_explain_pod(nhd_handle* h, int32_t pod, uint8_t* node_rea
 
 /* the records a query or a plan reads: NHD_QUERY_MIRROR or NHD_QUERY_SNAPSHOT, the latter only while the hardware
  * classes (d_class, d_cls_fast, d_sigs: the mirror's) describe it, i.e. no load or update since the snapshot */
-static int32_t source_records(nhd_handle* h, int32_t source, const char* what, uint8_t** records)
+static int32_t source_records(nhd_handle* h, int32_t source, const char* what, const uint8_t** records)
 {
     if (source != NHD_QUERY_MIRROR && source != NHD_QUERY_SNAPSHOT)
         return fail(h, NHD_ERR_INVALID, "%s source %d is neither NHD_QUERY_MIRROR nor NHD_QUERY_SNAPSHOT", what, source);
@@ -1175,69 +1156,6 @@ static int32_t source_records(nhd_handle* h, int32_t source, const char* what, u
     if (source == NHD_QUERY_SNAPSHOT && (!h->have_snapshot || h->snap_rec_gen != h->rec_gen))
         return fail(h, NHD_ERR_STATE, "a snapshot %s needs nhd_snapshot with no nhd_load_nodes / nhd_update_nodes since", what);
     *records = source == NHD_QUERY_SNAPSHOT ? h->d_snapshot : h->d_nodes;
-    return NHD_OK;
-}
-
-/*
- * A query's or a plan's pods: validated and de-duplicated into pod types as by nhd_stage_batch (tuple limits judged
- * against max_numa), then copied into the query scratch with room for their filter output and bindings.  Fills the
- * pod-set and filter fields of w (n_pods > 0); the sweep's own buffers are the plan's business.
- */
-static int32_t upload_pod_set(nhd_handle* h, int n_pods, const nhd_pod* pods, const double* now, int max_numa,
-                              SolveWork& w)
-{
-    uint64_t names_used = 0;
-    const bool multi_group = group_lists(n_pods, pods, &names_used);
-    std::vector<PodType> types;
-    std::vector<int32_t> pod_type;
-    const int32_t rc = make_pod_types(h, n_pods, pods, now, multi_group, max_numa, types, pod_type);
-    if (rc != NHD_OK) return rc;
-    CK(cudaSetDevice(h->params.device));
-    const int T = (int)types.size(), W = h->words;
-    const int n_names = multi_group ? __builtin_popcountll(names_used) : 0;
-
-    /* host -> device: types | pod_type | now | group masks, one pinned buffer */
-    const size_t types_bytes = (size_t)T * sizeof(PodType);
-    const size_t off_pt = 0, off_now = ((size_t)n_pods * 4 + 15) & ~(size_t)15;
-    const size_t off_gm = off_now + (size_t)n_pods * 8, pods_bytes = off_gm + (multi_group ? (size_t)n_pods * 8 : 0);
-    CK(grow_pinned(h->h_q, h->h_q_cap, types_bytes + pods_bytes));
-    memcpy(h->h_q, types.data(), types_bytes);
-    uint8_t* hp = h->h_q + types_bytes;
-    memcpy(hp + off_pt, pod_type.data(), (size_t)n_pods * 4);
-    memcpy(hp + off_now, now, (size_t)n_pods * 8);
-    if (multi_group)
-        for (int i = 0; i < n_pods; i++) memcpy(hp + off_gm + (size_t)i * 8, &pods[i].group_mask, 8);
-    CK(grow_dev(h->d_qtypes, h->qtypes_cap, types_bytes));
-    CK(grow_dev(h->d_qpods, h->qpods_cap, pods_bytes));
-    CK(grow_dev(h->d_qout, h->qout_cap, ((size_t)n_pods + 8) * sizeof(nhd_binding)));
-    CK(grow_dev(h->d_qbitmaps, h->qbitmaps_cap, (size_t)(T + 2 + n_names) * W * 8));
-    CK(grow_dev(h->d_qdyn, h->qdyn_cap, (size_t)W * 64 * sizeof(NodeDyn)));
-    if (!h->d_qftab) CK(cudaMalloc((void**)&h->d_qftab, ftab_bytes(FAST_MAX_TYPES)));
-    CK(cudaMemcpyAsync(h->d_qtypes, h->h_q, types_bytes, cudaMemcpyHostToDevice, h->stream));
-    CK(cudaMemcpyAsync(h->d_qpods, hp, pods_bytes, cudaMemcpyHostToDevice, h->stream));
-
-    w.types = h->d_qtypes;
-    w.pod_type = reinterpret_cast<const int32_t*>(h->d_qpods + off_pt);
-    w.now = reinterpret_cast<const double*>(h->d_qpods + off_now);
-    w.pod_groups = multi_group ? reinterpret_cast<const uint64_t*>(h->d_qpods + off_gm) : nullptr;
-    w.n_pods = n_pods; w.n_types = T; w.n_names = n_names; w.names_used = multi_group ? names_used : 0;
-    w.now0 = now[0];
-    w.const_clock = true;
-    for (int i = 1; i < n_pods; i++) if (now[i] != now[0]) { w.const_clock = false; break; }
-    w.bitmaps = h->d_qbitmaps; w.dyn = h->d_qdyn; w.ftab = h->d_qftab; w.out = h->d_qout;
-    w.cursors = nullptr; w.busy_list = nullptr; w.pend = nullptr; w.prof = nullptr;
-    return NHD_OK;
-}
-
-/* device -> host: the first n_pods bindings of the scratch, waiting for the device */
-static int32_t fetch_scratch_bindings(nhd_handle* h, int n_pods, nhd_binding* out)
-{
-    const size_t out_bytes = (size_t)n_pods * sizeof(nhd_binding);
-    const bool direct = is_pinned_host(out);
-    if (!direct) CK(grow_pinned(h->h_qout, h->h_qout_cap, out_bytes));
-    CK(cudaMemcpyAsync(direct ? (void*)out : (void*)h->h_qout, h->d_qout, out_bytes, cudaMemcpyDeviceToHost, h->stream));
-    CK(cudaStreamSynchronize(h->stream));
-    if (!direct) memcpy(out, h->h_qout, out_bytes);
     return NHD_OK;
 }
 
@@ -1251,21 +1169,20 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
                                    nhd_binding* out)
 {
     if (!h || n_pods < 0 || (n_pods > 0 && (!pods || !now || !out))) return NHD_ERR_INVALID;
-    uint8_t* nodes = nullptr;
+    const uint8_t* nodes = nullptr;
     int32_t rc = source_records(h, source, "query", &nodes);
     if (rc != NHD_OK) return rc;
     if (n_pods == 0) return NHD_OK;
-    SolveWork w;
-    w.nodes = nodes;
-    if ((rc = upload_pod_set(h, n_pods, pods, now, h->max_numa, w)) != NHD_OK) return rc;
+    Workspace& w = h->scratch;
+    if ((rc = stage_pods(h, w, n_pods, pods, now, h->max_numa)) != NHD_OK) return rc;
 
     /* the candidate bitmaps of the query's pod types on the chosen records */
-    if ((rc = launch_solve(h, w, false, true)) != NHD_OK) return rc;
+    if ((rc = launch_solve(h, w, nodes, false, true)) != NHD_OK) return rc;
 
     /* each pod on its own: the node, then the mapping and the assignment on a copy of its record */
     QueryArgs qa;
-    qa.nodes = nodes; qa.types = w.types; qa.pod_type = w.pod_type; qa.now = w.now;
-    qa.bitmaps = w.bitmaps; qa.pod_groups = w.pod_groups; qa.names_used = w.names_used;
+    qa.nodes = nodes; qa.types = w.types; qa.pod_type = w.pod_type(); qa.now = w.now();
+    qa.bitmaps = w.bitmaps; qa.pod_groups = w.pod_groups(); qa.names_used = w.names_used;
     qa.out = w.out; qa.n_pods = n_pods; qa.n_types = w.n_types; qa.words = h->words;
     qa.min_busy = h->params.min_busy_secs;
     memcpy(qa.cap, h->cap, sizeof(qa.cap));
@@ -1274,14 +1191,13 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
     CK(cudaGetLastError());
     query_assign_kernel<<<(n_pods + 63) / 64, 64, 0, h->stream>>>(qa);
     CK(cudaGetLastError());
-    return fetch_scratch_bindings(h, n_pods, out);
+    return fetch_bindings(h, w, n_pods, out);
 }
 
 /*
  * The bindings nhd_solve_batch would return on the chosen records with the excluded nodes in maintenance, and
- * optionally nhd_explain_batch's counts after it, with nothing written but the plan's own scratch: the solve's own
- * launches (launch_solve) on a workspace of the query scratch plus the plan's cursors, busy list and pend, without the
- * commit and without sharding.  With exclusions the records are first copied into a plan-owned array and the excluded
+ * optionally nhd_explain_batch's counts after it, with nothing written but the scratch: the solve's own launches
+ * (launch_solve) on the scratch workspace, without the commit and without sharding.  With exclusions the records are first copied into a plan-owned array and the excluded
  * nodes flagged there (exclude_nodes_kernel); without, the source records are read in place.
  */
 extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
@@ -1290,7 +1206,7 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
 {
     if (!h || n_pods < 0 || n_excluded < 0 || (n_excluded > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)))
         return NHD_ERR_INVALID;
-    uint8_t* records = nullptr;
+    const uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
     if (rc != NHD_OK) return rc;
 
@@ -1315,28 +1231,21 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
     int max_numa = 1;
     for (int k = 2; k <= NHD_MAX_NUMA; k++) if (hist[k] > 0) max_numa = k;
     if (n_pods == 0) return NHD_OK;
-    SolveWork w;
-    if ((rc = upload_pod_set(h, n_pods, pods, now, max_numa, w)) != NHD_OK) return rc;
-
-    const size_t n_slots = (size_t)h->n_super * SUPER_NODES;
-    CK(grow_dev(h->d_pcursors, h->pcursors_cap, (size_t)std::max(w.n_types, 1) * 3 * 4));
-    CK(grow_dev(h->d_pbusy, h->pbusy_cap, (n_slots + 64) * 4));
-    CK(grow_dev(h->d_ppend, h->ppend_cap, n_slots * 4));
-    if (!h->d_pprof) CK(cudaMalloc((void**)&h->d_pprof, 64 * 8));
-    w.cursors = h->d_pcursors; w.busy_list = h->d_pbusy; w.pend = h->d_ppend; w.prof = h->d_pprof;
-    w.nodes = records;
+    Workspace& w = h->scratch;
+    if ((rc = stage_pods(h, w, n_pods, pods, now, max_numa)) != NHD_OK) return rc;
+    const uint8_t* nodes = records;
     if (!ex.empty()) {
-        CK(grow_dev(h->d_pnodes, h->pnodes_cap, h->nodes_bytes));
-        CK(grow_dev(h->d_pidx, h->pidx_cap, ex.size() * 4));
+        CK(h->d_pnodes.grow(h->nodes_bytes));
+        CK(h->d_pidx.grow(ex.size() * 4));
         CK(cudaMemcpyAsync(h->d_pnodes, records, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
         CK(cudaMemcpyAsync(h->d_pidx, ex.data(), ex.size() * 4, cudaMemcpyHostToDevice, h->stream));
         exclude_nodes_kernel<<<(unsigned)((ex.size() + 255) / 256), 256, 0, h->stream>>>(h->d_pnodes, h->d_pidx, (int)ex.size());
         CK(cudaGetLastError());
-        w.nodes = h->d_pnodes;
+        nodes = h->d_pnodes;
     }
-    if ((rc = launch_solve(h, w, false, false)) != NHD_OK) return rc;
-    if (why_counts && (rc = explain_counts(h, w, why_counts, "nhd_plan_batch")) != NHD_OK) return rc;
-    return fetch_scratch_bindings(h, n_pods, out);
+    if ((rc = launch_solve(h, w, nodes, false, false)) != NHD_OK) return rc;
+    if (why_counts && (rc = explain_counts(h, w, nodes, why_counts, "nhd_plan_batch")) != NHD_OK) return rc;
+    return fetch_bindings(h, w, n_pods, out);
 }
 
 /*
@@ -1366,7 +1275,7 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     const int n_edit = edit_start ? edit_start[n_scenarios] : 0;
     if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)) || (n_edit > 0 && (!edit_node || !edit_rec)))
         return NHD_ERR_INVALID;
-    uint8_t* records = nullptr;
+    const uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
     if (rc != NHD_OK) return rc;
     for (int e = 0; e < n_excl; e++)
@@ -1431,9 +1340,8 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
             cnow.insert(cnow.end(), now + pod_start[s], now + pod_start[s + 1]);
         }
     }
-    SolveWork w;
-    w.nodes = records;
-    if ((rc = upload_pod_set(h, n_run, compact ? cpods.data() : pods, compact ? cnow.data() : now, max_numa, w)) != NHD_OK)
+    Workspace& w = h->scratch;
+    if ((rc = stage_pods(h, w, n_run, compact ? cpods.data() : pods, compact ? cnow.data() : now, max_numa)) != NHD_OK)
         return rc;
 
     std::vector<int32_t> idx;
@@ -1443,8 +1351,8 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     const size_t off_ed_node = off_ed_off + ed_off.size(), off_lift = off_ed_node + ed_node.size();
     const size_t n_slots = (size_t)n_run + n_ed, off_nodes = idx.size(), off_bad = off_nodes + n_slots;
     /* d_swork: the working slots, then the edit records the kernel seeds them from */
-    CK(grow_dev(h->d_sidx, h->sidx_cap, (off_bad + 1) * 4));
-    CK(grow_dev(h->d_swork, h->swork_cap, (n_slots + n_ed) * sizeof(nhd_node_rec)));
+    CK(h->d_sidx.grow((off_bad + 1) * 4));
+    CK(h->d_swork.grow((n_slots + n_ed) * sizeof(nhd_node_rec)));
     CK(cudaMemcpyAsync(h->d_sidx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(h->d_sidx + off_bad, 0, 4, h->stream));
     uint4* d_edit_rec = h->d_swork + n_slots * REC_CHUNKS;
@@ -1452,11 +1360,11 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         CK(cudaMemcpyAsync(d_edit_rec, ed_rec.data(), (size_t)n_ed * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
 
     /* the candidate bitmaps of the call's pod types on the unchanged source records */
-    if ((rc = launch_solve(h, w, false, true)) != NHD_OK) return rc;
+    if ((rc = launch_solve(h, w, records, false, true)) != NHD_OK) return rc;
 
     ScenarioArgs sa;
-    sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type; sa.now = w.now;
-    sa.bitmaps = w.bitmaps; sa.pod_groups = w.pod_groups; sa.names_used = w.names_used;
+    sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type(); sa.now = w.now();
+    sa.bitmaps = w.bitmaps; sa.pod_groups = w.pod_groups(); sa.names_used = w.names_used;
     sa.pod_start = h->d_sidx; sa.excl_start = h->d_sidx + off_ex_off; sa.excl = h->d_sidx + off_ex;
     sa.lift = h->d_sidx + off_lift; sa.edit_start = h->d_sidx + off_ed_off; sa.edit_node = h->d_sidx + off_ed_node;
     sa.edit_rec = d_edit_rec;
@@ -1472,7 +1380,7 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     CK(cudaMemcpyAsync(&bad, h->d_sidx + off_bad, 4, cudaMemcpyDeviceToHost, h->stream));
     std::vector<nhd_binding> run;
     if (compact) run.resize(n_run);
-    if ((rc = fetch_scratch_bindings(h, n_run, compact ? run.data() : out)) != NHD_OK) return rc;
+    if ((rc = fetch_bindings(h, w, n_run, compact ? run.data() : out)) != NHD_OK) return rc;
     if (bad) return fail(h, NHD_ERR_STATE, "%s: %u chosen nodes without a mapping", what, bad);
     if (compact)
         for (int k = 0; k < n_acc; k++)
@@ -1512,8 +1420,8 @@ extern "C" int32_t nhd_debug_counters(nhd_handle* h, uint64_t* out32)
 #endif
     CK(cudaSetDevice(h->params.device));
     CK(cudaStreamSynchronize(h->stream));
-    CK(cudaMemcpy(out32, h->d_prof, 64 * 8, cudaMemcpyDeviceToHost));
-    CK(cudaMemset(h->d_prof, 0, 64 * 8));
+    CK(cudaMemcpy(out32, h->batch.prof, 64 * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemset(h->batch.prof, 0, 64 * 8));
     return NHD_OK;
 }
 

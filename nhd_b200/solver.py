@@ -53,6 +53,14 @@ def pinned_array(n, dtype):
 _PINNED = {}
 
 
+def _source(source):
+    """The ``nhd_query_batch`` / ``nhd_plan_*`` source code of ``'mirror'`` or ``'snapshot'``."""
+    src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
+    if src is None:
+        raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
+    return src
+
+
 class Solver:
     def __init__(self, speed_table, nic_bw_avail_percent=0.9, min_busy_secs=30.0, device=0,
                  rank=0, world_size=1, nccl_id: bytes = None, single_warp: bool = False, cpu_warps: int = 0,
@@ -188,9 +196,7 @@ class Solver:
         """Where each pod would go on its own (``nhd_query_batch``): per pod the binding ``solve_batch`` would return
         for that pod alone, on the current records (``source='mirror'``) or on those of the last ``snapshot()``
         (``'snapshot'``).  Nothing is placed: records, snapshot, the last batch and its explanations stay as they are."""
-        src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
-        if src is None:
-            raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
+        src = _source(source)
         pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
         now = np.ascontiguousarray(now, dtype='<f8')
         assert len(pods) == len(now)
@@ -205,9 +211,7 @@ class Solver:
         (``'snapshot'``), with the node indices ``exclude`` taken as in maintenance.  With ``explain=True`` returns
         ``(bindings, counts)``, counts being what ``explain_batch`` would return after that solve.  Nothing is placed:
         records, snapshot, the last batch and its explanations stay as they are."""
-        src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
-        if src is None:
-            raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
+        src = _source(source)
         pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
         now = np.ascontiguousarray(now, dtype='<f8')
         assert len(pods) == len(now)
@@ -231,9 +235,7 @@ class Solver:
         (None: none): ``(nodes, records)``, node indices and a ``wire.NODE_DTYPE`` array, the records those nodes have
         for the whole scenario.  With either, the bindings are those of ``solve_batch`` on a scratch copy of the records
         with the edits applied, the excluded nodes in maintenance for the pods before ``lift`` and back after."""
-        src = {'mirror': wire.QUERY_MIRROR, 'snapshot': wire.QUERY_SNAPSHOT}.get(source)
-        if src is None:
-            raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
+        src = _source(source)
         # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
         # would cost more than the call itself)
         exs, podb, nowl, lifts, ednodes, edrecs = [], [], [], [], [], []
