@@ -2627,7 +2627,9 @@ __global__ void __launch_bounds__(EXPLAIN_THREADS) explain_kernel(const __grid_c
  * Not part of a solve: where each pod of a query would go on its own.  The query's pod types were filtered on the
  * chosen record array into the query's own bitmaps (filter_kernel), so F[type] is exactly FindNode's candidate set on
  * those records apart from the busy window.  Every pod is independent: one warp picks its node, then one thread works
- * out the mapping and the assignment on a private copy of that node's record.
+ * out the mapping and the assignment on a private copy of that node's record.  scenario_plan_kernel repeats both steps
+ * for its untouched nodes; a change to the busy-window or node-group rules goes into both (DESIGN.md section 8.7 says
+ * why queries do not run on it).
  */
 struct QueryArgs {
     const uint8_t* nodes;          /* the records queried (mirror or snapshot, tiled layout) */
