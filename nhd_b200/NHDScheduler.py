@@ -188,6 +188,14 @@ class DeviceCluster:
                 packing.pack_pod(top, pod_groups[i], self._layout, out=pods[i])
         return pods
 
+    def _indices(self, names: Iterable[str], what: str) -> np.ndarray:
+        """Indices of the nodes ``names``; a ValueError lists the unknown ones (``what``: what the caller does to them)."""
+        names = list(names)
+        missing = [n for n in names if n not in self._index]
+        if missing:
+            raise ValueError(f'cannot {what} unknown node(s) {missing}')
+        return np.asarray([self._index[n] for n in names], dtype='<i4')
+
     @staticmethod
     def _clocks(n: int, now) -> np.ndarray:
         """Per-pod clocks of ``n`` pods from one clock or one per pod."""
@@ -231,10 +239,7 @@ class DeviceCluster:
         fn = getattr(self._solver, 'plan_batch', None)
         if fn is None:
             return None
-        missing = [n for n in exclude if n not in self._index]
-        if missing:
-            raise ValueError(f'cannot exclude unknown node(s) {missing}')
-        idx = np.asarray([self._index[n] for n in exclude], dtype='<i4')
+        idx = self._indices(exclude, 'exclude')
         return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), source=source, exclude=idx,
                   explain=explain)
 
@@ -249,19 +254,18 @@ class DeviceCluster:
         fn = getattr(self._solver, 'plan_scenarios', None)
         if fn is None:
             return None
-        missing = sorted({n for sc in scenarios for n in list(sc[0]) + list(sc[6] if len(sc) > 6 and sc[6] else ())
-                          if n not in self._index})
-        if missing:
-            raise ValueError(f'cannot exclude or edit unknown node(s) {missing}')
+        # every scenario's names are checked before any is packed
+        self._indices(sorted({n for sc in scenarios for n in list(sc[0]) + list(sc[6] if len(sc) > 6 and sc[6] else ())}),
+                      'exclude or edit')
         args = []
         for sc in scenarios:
             exclude, tops, pod_groups, now = sc[:4]
             packed = sc[4] if len(sc) > 4 else None
             lift = sc[5] if len(sc) > 5 else None
             edits = sc[6] if len(sc) > 6 else None
-            idx = np.asarray([self._index[n] for n in exclude], dtype='<i4')
+            idx = self._indices(exclude, 'exclude')
             if edits:
-                edits = (np.asarray([self._index[n] for n in edits], dtype='<i4'), self._pack(list(edits.values())))
+                edits = (self._indices(edits, 'edit'), self._pack(list(edits.values())))
             args.append((idx, self._pods(tops, pod_groups, packed), self._clocks(len(tops), now)) +
                         ((lift, edits or None) if lift is not None or edits else ()))
         return fn(args, source=source)
@@ -302,6 +306,11 @@ class _Pending:
         self.pos, self.key = pos, key
         self.pobj = self.tcfg = self.top = self.groups = self.unsupported = self.rec = None
         self.ready = False
+
+    @property
+    def solvable(self) -> bool:
+        """Read, parsed and within the packed layout: the pod goes to the solver."""
+        return self.top is not None and self.unsupported is None
 
 
 class NHDScheduler:
@@ -346,6 +355,11 @@ class NHDScheduler:
     def _touch(self, name):
         """The host changed node ``name`` outside the solver: re-send it before the next batch."""
         self._dirty.add(name)
+
+    def _sync(self):
+        """Make the device copy equal to the nodes, re-sending the ones the host changed."""
+        self.cluster.sync(self.nodes, self._dirty)
+        self._dirty.clear()
 
     def close(self):
         self.cluster.close()
@@ -582,32 +596,25 @@ class NHDScheduler:
                 if not e.ready:
                     self._prepare(e)
             now = float(self._clock())
-            solvable = [e for e in run if e.top is not None and e.unsupported is None]
+            solvable = [e for e in run if e.solvable]
             bindings, why, contended = {}, None, None
             if solvable and self.nodes:
-                self.cluster.sync(self.nodes, self._dirty)
-                self._dirty.clear()
-                out = []
-                while solvable:
-                    try:
-                        out = self.cluster.solve([e.top for e in solvable], [e.groups for e in solvable], now,
-                                                 packed=[e.rec for e in solvable])
-                        break
-                    except Exception as err:
-                        # a limit that depends on the cluster as well (numa^(groups+1) tuples, include/nhd_b200.h):
-                        # the library refuses the whole batch and names the pod; that pod fails loudly, the rest goes on
-                        m = re.search(r'pod (\d+)', str(err)) if getattr(err, 'code', None) == wire.ERR_UNSUPPORTED else None
-                        if m is None or int(m.group(1)) >= len(solvable):
-                            raise
-                        solvable.pop(int(m.group(1))).unsupported = str(err)
+                self._sync()
+                out, solvable, dropped = self._without_refused(
+                    lambda es: self.cluster.solve([e.top for e in es], [e.groups for e in es], now,
+                                                  packed=[e.rec for e in es]), solvable)
+                for e, err in dropped:                  # the pod fails loudly (_finish), the rest goes on
+                    e.unsupported = str(err)
                 self.pods_solved += len(solvable)
-                bindings = {e.pos: out[i] for i, e in enumerate(solvable)}
-                # why the NO_CANDIDATE pods found no node: read before a rewind replaces the solved batch
-                why = self.cluster.explain() if any(int(b['status']) == wire.NO_CANDIDATE for b in out) else None
-                if why is not None:
-                    why = {e.pos: why[i] for i, e in enumerate(solvable)}
-                if self.diagnose_contention and any(int(b['status']) == wire.NO_CANDIDATE for b in out):
-                    contended = self._contention(solvable, out, now)
+                if solvable:
+                    bindings = {e.pos: b for e, b in zip(solvable, out)}
+                    if any(int(b['status']) == wire.NO_CANDIDATE for b in out):
+                        # why the NO_CANDIDATE pods found no node: read before a rewind replaces the solved batch
+                        why = self.cluster.explain()
+                        if why is not None:
+                            why = {e.pos: w for e, w in zip(solvable, why)}
+                        if self.diagnose_contention:
+                            contended = self._contention(solvable, out, now)
             cut = None
             for e in run:
                 b = bindings.get(e.pos)
@@ -649,13 +656,13 @@ class NHDScheduler:
         """{pos: node name or None} for the NO_CANDIDATE pods of the batch just solved: the node each would have been
         placed on alone, at the state the batch started from (a query of the snapshot ``solve`` took).  None when the
         solver in use cannot answer queries."""
-        failed = [i for i, b in enumerate(out) if int(b['status']) == wire.NO_CANDIDATE]
-        q = self.cluster.query([solvable[i].top for i in failed], [solvable[i].groups for i in failed], now,
-                               source='snapshot', packed=[solvable[i].rec for i in failed])
+        failed = [e for e, b in zip(solvable, out) if int(b['status']) == wire.NO_CANDIDATE]
+        q = self.cluster.query([e.top for e in failed], [e.groups for e in failed], now, source='snapshot',
+                               packed=[e.rec for e in failed])
         if q is None:
             return None
-        return {solvable[i].pos: self.cluster.name_of(int(b['node'])) if int(b['status']) == wire.PLACED else None
-                for i, b in zip(failed, q)}
+        placed = self._placements(failed, q)          # a pod listed twice is read and queried the same both times
+        return {e.pos: placed[(e.key[0], e.key[1])] for e in failed}
 
     def _contended(self, e: _Pending, nodename):
         """Remember and log that pod ``e`` found no node although it would have fit alone on ``nodename`` at the start
@@ -696,33 +703,19 @@ class NHDScheduler:
         pods do not see each other.  Only the Kubernetes reads of a scheduling attempt happen: no event, no write;
         ``pod_state`` and the ``Node`` objects stay as they are.  Nodes the host changed are synced first, as for a
         batch."""
-        entries = [_Pending(i, k) for i, k in enumerate(keys)]
-        for e in entries:
-            self._prepare(e, events=False)
+        entries = self._read(keys)
         result = {(e.key[0], e.key[1]): None for e in entries}
-        ok = [e for e in entries if e.top is not None and e.unsupported is None]
+        ok = [e for e in entries if e.solvable]
         if not ok or not self.nodes:
             return result
-        self.cluster.sync(self.nodes, self._dirty)
-        self._dirty.clear()
+        self._sync()
         now = float(self._clock())
-        while ok:
-            try:
-                out = self.cluster.query([e.top for e in ok], [e.groups for e in ok], now,
-                                         packed=[e.rec for e in ok])
-                break
-            except Exception as err:                  # a pod beyond the tuple limits: it gets None, the rest goes on
-                m = re.search(r'pod (\d+)', str(err)) if getattr(err, 'code', None) == wire.ERR_UNSUPPORTED else None
-                if m is None or int(m.group(1)) >= len(ok):
-                    raise
-                ok.pop(int(m.group(1)))
-        else:
-            return result
-        if out is None:
-            raise RuntimeError('the solver in use cannot answer placement queries (no query_batch)')
-        for e, b in zip(ok, out):
-            if int(b['status']) == wire.PLACED:
-                result[(e.key[0], e.key[1])] = self.cluster.name_of(int(b['node']))
+        out, ok, _ = self._without_refused(
+            lambda es: self._supported(self.cluster.query([e.top for e in es], [e.groups for e in es], now,
+                                                          packed=[e.rec for e in es]),
+                                       'answer placement queries (no query_batch)'), ok)
+        if ok:
+            result.update(self._placements(ok, out))
         return result
 
     def PlanPods(self, keys: Sequence):
@@ -743,8 +736,7 @@ class NHDScheduler:
         missing = [n for n in names if n not in self.nodes]
         if missing:
             raise ValueError(f'unknown node(s) {missing}')
-        keys = [(ns, pod) for n in names for (pod, ns) in self.nodes[n].pod_info]
-        return self._plan(keys, names)
+        return self._plan(self._pods_on(names), names)
 
     def PlanDrains(self, node_groups: Sequence[Sequence[str]] = None) -> Dict:
         """Which nodes (or groups of nodes) could be taken down, each group on its own?  ``{tuple(group): placement}``
@@ -753,49 +745,30 @@ class NHDScheduler:
         do not see each other.  Each pod is read from Kubernetes once, as a scheduling attempt reads it: no event, no
         write; ``pod_state``, the ``Node`` objects and the counters stay as they are.  Reasons are not returned:
         ``PlanDrain(group)`` gives them for the groups that do not drain."""
-        if node_groups is None:
-            node_groups = [[n] for n, v in self.nodes.items() if v.pod_info]
-        groups = [tuple(g) for g in node_groups]
-        missing = sorted({n for g in groups for n in g if n not in self.nodes})
-        if missing:
-            raise ValueError(f'unknown node(s) {missing}')
-        prepared = {}
-        group_entries = []
-        for g in groups:
-            entries = []
-            for n in g:
-                for (pod, ns) in self.nodes[n].pod_info:
-                    if (ns, pod) not in prepared:
-                        e = _Pending(len(prepared), (ns, pod))
-                        self._prepare(e, events=False)
-                        prepared[(ns, pod)] = e
-                    entries.append(prepared[(ns, pod)])
-            group_entries.append(entries)
+        groups = self._node_groups(node_groups)
+        seen = {}
+        group_entries = [self._read(self._pods_on(g), seen) for g in groups]
         result = {}
         todo = []
         for g, entries in zip(groups, group_entries):
             result[g] = {(e.key[0], e.key[1]): None for e in entries}
-            ok = [e for e in entries if e.top is not None and e.unsupported is None]
+            ok = [e for e in entries if e.solvable]
             if ok and self.nodes:
                 todo.append((g, entries, ok))
         if not todo:
             return result
-        self.cluster.sync(self.nodes, self._dirty)
-        self._dirty.clear()
+        self._sync()
         now = float(self._clock())
-        res = self.cluster.plan_scenarios([(g, [e.top for e in ok], [e.groups for e in ok], now, [e.rec for e in ok])
-                                           for g, _, ok in todo])
-        if res is None:
-            raise RuntimeError('the solver in use cannot plan scenarios (no plan_scenarios)')
+        res = self._supported(
+            self.cluster.plan_scenarios([(g, [e.top for e in ok], [e.groups for e in ok], now, [e.rec for e in ok])
+                                         for g, _, ok in todo]), 'plan scenarios (no plan_scenarios)')
         for (g, entries, ok), (code, _, out) in zip(todo, res):
             if out is None:
                 # refused (the tuple limits are judged with the group's own nodes counted): the single plan judges
                 # them without, and drops a pod beyond them, or raises, as PlanDrain does
                 result[g] = self._plan_prepared(entries, list(g), now)[0]
-                continue
-            for e, b in zip(ok, out):
-                if int(b['status']) == wire.PLACED:
-                    result[g][(e.key[0], e.key[1])] = self.cluster.name_of(int(b['node']))
+            else:
+                result[g].update(self._placements(ok, out))
         return result
 
     def PlanDefrag(self, keys: Sequence = None, node_groups: Sequence[Sequence[str]] = None,
@@ -819,39 +792,22 @@ class NHDScheduler:
         Only reads happen, as ``PlanDrains``: each pod is read from Kubernetes once (a scheduling attempt's reads and
         a release's); the releases run on copies of the ``Node`` objects; ``pod_state``, the ``Node`` objects and the
         counters stay as they are."""
-        if node_groups is None:
-            node_groups = [[n] for n, v in self.nodes.items() if v.pod_info]
-        groups = [tuple(g) for g in node_groups]
-        missing = sorted({n for g in groups for n in g if n not in self.nodes})
-        if missing:
-            raise ValueError(f'unknown node(s) {missing}')
+        groups = self._node_groups(node_groups)
         if keys is None:
             phase = self._service_pods()
             keys = [k for k in phase if self._wanted(phase)(k)]
         delay = float(self._node_cls.MIN_BUSY_SECS if delay is None else delay)
-        prepared, targets = {}, {}
-
-        def prepare(key):
-            if key not in prepared:
-                e = _Pending(len(prepared), key)
-                self._prepare(e, events=False)
-                prepared[key] = e
-            return prepared[key]
-        tail = [prepare((k[0], k[1])) for k in keys]
-        tail_ok = [e for e in tail if e.top is not None and e.unsupported is None]
-        group_pods = []
-        for g in groups:
-            pods = [(ns, pod) for n in g for (pod, ns) in self.nodes[n].pod_info]
-            for key in pods:
-                if key not in targets:
-                    targets[key] = self._release_target(key[1], key[0])
-            group_pods.append(pods)
-        entries = [[prepare(key) for key in pods] for pods in group_pods]
+        seen, targets = {}, {}
+        tail = [e for e in self._read([(k[0], k[1]) for k in keys], seen) if e.solvable]
+        group_pods = [self._pods_on(g) for g in groups]
+        for key in (key for pods in group_pods for key in pods):
+            if key not in targets:
+                targets[key] = self._release_target(key[1], key[0])
+        entries = [self._read(pods, seen) for pods in group_pods]
         result = {g: ({key: None for key in pods}, None) for g, pods in zip(groups, group_pods)}
         if not self.nodes:
             return result
-        self.cluster.sync(self.nodes, self._dirty)
-        self._dirty.clear()
+        self._sync()
         now = float(self._clock())
         todo = []
         for g, pods, moved in zip(groups, group_pods, entries):
@@ -868,13 +824,11 @@ class NHDScheduler:
                 if node not in edits:
                     edits[node] = _copy_node(self.nodes[node])
                 self._give_back(edits[node], key[1], key[0], top, now)
-            ok = [e for e in moved if e.top is not None and e.unsupported is None]
-            todo.append((g, ok, tail_ok, edits))
+            todo.append((g, [e for e in moved if e.solvable], tail, edits))
         while todo:
-            res = self.cluster.plan_scenarios([self._defrag_scenario(g, ok, tail, edits, now, delay)
-                                               for g, ok, tail, edits in todo])
-            if res is None:
-                raise RuntimeError('the solver in use cannot plan scenarios (no plan_scenarios)')
+            res = self._supported(self.cluster.plan_scenarios([self._defrag_scenario(g, ok, tail, edits, now, delay)
+                                                               for g, ok, tail, edits in todo]),
+                                  'plan scenarios (no plan_scenarios)')
             retry = []
             for (g, ok, tail, edits), (code, pod, out) in zip(todo, res):
                 if out is None:
@@ -889,14 +843,10 @@ class NHDScheduler:
                     retry.append((g, ok, tail, edits))
                     continue
                 moved, _ = result[g]
-                for e, b in zip(ok, out[:len(ok)]):
-                    if int(b['status']) == wire.PLACED:
-                        moved[e.key] = self.cluster.name_of(int(b['node']))
+                moved.update(self._placements(ok, out[:len(ok)]))
                 if all(v is not None for v in moved.values()):
                     pending = {(k[0], k[1]): None for k in keys}
-                    for e, b in zip(tail, out[len(ok):]):
-                        if int(b['status']) == wire.PLACED:
-                            pending[e.key] = self.cluster.name_of(int(b['node']))
+                    pending.update(self._placements(tail, out[len(ok):]))
                     result[g] = (moved, pending)
             todo = retry
         return result
@@ -909,43 +859,89 @@ class NHDScheduler:
         return (g, [e.top for e in pods], [e.groups for e in pods], clock, [e.rec for e in pods], len(moved), edits)
 
     def _plan(self, keys: Sequence, exclude: Sequence[str]):
-        entries = [_Pending(i, k) for i, k in enumerate(keys)]
-        for e in entries:
-            self._prepare(e, events=False)
-        ok = [e for e in entries if e.top is not None and e.unsupported is None]
-        if not ok or not self.nodes:
+        entries = self._read(keys)
+        if not self.nodes or not any(e.solvable for e in entries):
             return {(e.key[0], e.key[1]): None for e in entries}, {}
-        self.cluster.sync(self.nodes, self._dirty)
-        self._dirty.clear()
+        self._sync()
         return self._plan_prepared(entries, exclude, float(self._clock()))
 
     def _plan_prepared(self, entries: Sequence, exclude: Sequence[str], now: float):
         """``_plan`` from pods already read from Kubernetes, on the synced cluster at clock ``now``."""
         placement = {(e.key[0], e.key[1]): None for e in entries}
-        reasons = {}
-        ok = [e for e in entries if e.top is not None and e.unsupported is None]
-        while ok:
-            try:
-                res = self.cluster.plan([e.top for e in ok], [e.groups for e in ok], now, exclude=exclude,
-                                        packed=[e.rec for e in ok], explain=True)
-                break
-            except Exception as err:                  # a pod beyond the tuple limits: it gets None, the rest goes on
-                m = re.search(r'pod (\d+)', str(err)) if getattr(err, 'code', None) == wire.ERR_UNSUPPORTED else None
-                if m is None or int(m.group(1)) >= len(ok):
-                    raise
-                ok.pop(int(m.group(1)))
-        else:
-            return placement, reasons
-        if res is None:
-            raise RuntimeError('the solver in use cannot plan batches (no plan_batch)')
+        res, ok, _ = self._without_refused(
+            lambda es: self._supported(self.cluster.plan([e.top for e in es], [e.groups for e in es], now,
+                                                         exclude=exclude, packed=[e.rec for e in es], explain=True),
+                                       'plan batches (no plan_batch)'), [e for e in entries if e.solvable])
+        if not ok:
+            return placement, {}
         out, counts = res
-        for e, b, c in zip(ok, out, counts):
-            key = (e.key[0], e.key[1])
-            if int(b['status']) == wire.PLACED:
-                placement[key] = self.cluster.name_of(int(b['node']))
-            elif int(b['status']) == wire.NO_CANDIDATE:
-                reasons[key] = {name: int(n) for name, n in zip(wire.WHY_NAMES, c) if int(n)}
+        placement.update(self._placements(ok, out))
+        reasons = {(e.key[0], e.key[1]): {name: int(n) for name, n in zip(wire.WHY_NAMES, c) if int(n)}
+                   for e, b, c in zip(ok, out, counts) if int(b['status']) == wire.NO_CANDIDATE}
         return placement, reasons
+
+    # ---- shared by the batch, the previews and the plans ------------------------------------------------------
+    def _read(self, keys: Sequence, seen: Dict = None) -> List[_Pending]:
+        """The pods ``keys`` read from Kubernetes as a scheduling attempt reads them, without its events
+        (``_prepare(events=False)``).  ``seen``: a dict, shared by calls that read each pod once, from key to entry."""
+        entries = []
+        for i, k in enumerate(keys):
+            e = None if seen is None else seen.get(k)
+            if e is None:
+                e = _Pending(i, k)
+                self._prepare(e, events=False)
+                if seen is not None:
+                    seen[k] = e
+            entries.append(e)
+        return entries
+
+    def _pods_on(self, names: Sequence[str]) -> List[tuple]:
+        """``(ns, name)`` of the pods on the nodes ``names``: nodes in the given order, pods in ``Node.pod_info``
+        order."""
+        return [(ns, pod) for n in names for (pod, ns) in self.nodes[n].pod_info]
+
+    def _node_groups(self, node_groups) -> List[tuple]:
+        """``node_groups`` as tuples, by default every node that holds pods on its own, in node order."""
+        if node_groups is None:
+            node_groups = [[n] for n, v in self.nodes.items() if v.pod_info]
+        groups = [tuple(g) for g in node_groups]
+        missing = sorted({n for g in groups for n in g if n not in self.nodes})
+        if missing:
+            raise ValueError(f'unknown node(s) {missing}')
+        return groups
+
+    @staticmethod
+    def _without_refused(call: Callable, entries: Sequence):
+        """``call(entries)`` without the pods the library refuses.  A request beyond the limit that depends on the
+        cluster as well (numa^(groups+1) tuples, include/nhd_b200.h) makes the library refuse the whole call and name
+        the pod; that entry is dropped and ``call`` made again with the rest.  Returns ``(result, kept entries,
+        [(dropped entry, error)])``, ``result`` None when every entry was dropped.  Any other error propagates."""
+        kept, dropped = list(entries), []
+        while kept:
+            try:
+                return call(kept), kept, dropped
+            except Exception as err:
+                m = re.search(r'pod (\d+)', str(err)) if getattr(err, 'code', None) == wire.ERR_UNSUPPORTED else None
+                if m is None or int(m.group(1)) >= len(kept):
+                    raise
+                dropped.append((kept.pop(int(m.group(1))), err))
+        return None, kept, dropped
+
+    def _placements(self, entries: Sequence, out) -> Dict:
+        """``{(ns, name): node name}`` of ``entries`` from their bindings ``out``, None for a pod not placed (a pod
+        listed twice keeps the node either entry got)."""
+        placement = {(e.key[0], e.key[1]): None for e in entries}
+        for e, b in zip(entries, out):
+            if int(b['status']) == wire.PLACED:
+                placement[(e.key[0], e.key[1])] = self.cluster.name_of(int(b['node']))
+        return placement
+
+    @staticmethod
+    def _supported(res, what: str):
+        """``res``, the answer of a ``DeviceCluster`` call that is None when the solver in use lacks the method."""
+        if res is None:
+            raise RuntimeError(f'the solver in use cannot {what}')
+        return res
 
     def CheckPendingPods(self):
         """``NHDScheduler.py:425-441`` with the pending set solved as one batch."""
@@ -1067,8 +1063,7 @@ class NHDScheduler:
         (``nhd_read_nodes`` + ``nhd_node_stats_from_records``) instead of walking the Python objects;
         ``totalhuge_gb``, ``totalpods`` and ``nicstats`` are not placement state and come from the host."""
         from nhd_b200 import ingest
-        self.cluster.sync(self.nodes, self._dirty)
-        self._dirty.clear()
+        self._sync()
         st = ingest.node_stats(self.cluster.read_records())
         rows = []
         by_name = {r['name']: r for r in self.GetBasicNodeStats()} if self.cluster.stubs else {}
