@@ -234,7 +234,8 @@ int32_t nhd_update_nodes(nhd_handle* h, int32_t n, const int32_t* idx, const nhd
 int32_t nhd_read_nodes(nhd_handle* h, int32_t first, int32_t n, nhd_node_rec* out);
 
 /* Snapshot / restore of the device mirror (device-to-device; used by benchmarks
- * to replay a batch from the same cluster state). */
+ * to replay a batch from the same cluster state).  A restore brings back the snapshot's
+ * records with their hardware classes and tuple limits, updates since the snapshot included. */
 int32_t nhd_snapshot(nhd_handle* h);
 int32_t nhd_restore(nhd_handle* h);
 

@@ -148,6 +148,10 @@ struct nhd_handle {
        tuple limits are judged against the largest of these, and follow updates in both directions */
     std::vector<uint8_t> node_numa;
     int numa_hist[NHD_MAX_NUMA + 1] = {0, 0, 0, 0, 0};
+    /* ... as they were at the last nhd_snapshot: nhd_restore puts them back with the records */
+    std::vector<uint8_t> snap_node_numa;
+    int snap_numa_hist[NHD_MAX_NUMA + 1] = {0, 0, 0, 0, 0};
+    int snap_max_numa = 1;
     DevBuf<uint8_t> d_nodes, d_snapshot;
     size_t nodes_bytes = 0;
     bool loaded = false, have_snapshot = false;
@@ -451,6 +455,19 @@ static bool is_pinned_host(const void* p)
     return at.type == cudaMemoryTypeHost;
 }
 
+/* hardware classes of the mirror's nodes idx[0..n) (all of [0, n) when idx is null), then the per-class tables */
+static int32_t classify(nhd_handle* h, const int32_t* d_idx, int n)
+{
+    const int threads = 256;
+    classify_claim_kernel<<<(n + threads - 1) / threads, threads, 0, h->stream>>>(h->d_nodes, d_idx, n, h->d_class_slots, h->d_class);
+    CK(cudaGetLastError());
+    classify_verify_kernel<<<(n + threads - 1) / threads, threads, 0, h->stream>>>(h->d_nodes, d_idx, n, h->d_class_slots, h->d_class);
+    cls_fast_kernel<<<(CLASS_SLOTS + 255) / 256, 256, 0, h->stream>>>(h->d_class_slots, h->d_cls_fast, h->d_sigs);
+    CK(cudaGetLastError());
+    CK(cudaStreamSynchronize(h->stream));
+    return NHD_OK;
+}
+
 /* host -> device, ingest into the tiled layout, validate on the device, classify.  Records that
  * already sit in pinned memory (nhd_alloc_pinned) are copied straight from the caller's buffer. */
 static int32_t upload_records(nhd_handle* h, int n, const nhd_node_rec* recs, const int32_t* idx, int* max_numa,
@@ -491,14 +508,7 @@ static int32_t upload_records(nhd_handle* h, int n, const nhd_node_rec* recs, co
     ingest_kernel<<<(total + threads - 1) / threads, threads, 0, h->stream>>>(
         (const uint4*)h->d_stage.p, d_idx, n, h->d_nodes);
     CK(cudaGetLastError());
-    /* hardware classes of the (re)written nodes */
-    classify_claim_kernel<<<(n + threads - 1) / threads, threads, 0, h->stream>>>(h->d_nodes, d_idx, n, h->d_class_slots, h->d_class);
-    CK(cudaGetLastError());
-    classify_verify_kernel<<<(n + threads - 1) / threads, threads, 0, h->stream>>>(h->d_nodes, d_idx, n, h->d_class_slots, h->d_class);
-    cls_fast_kernel<<<(CLASS_SLOTS + 255) / 256, 256, 0, h->stream>>>(h->d_class_slots, h->d_cls_fast, h->d_sigs);
-    CK(cudaGetLastError());
-    CK(cudaStreamSynchronize(h->stream));
-    return NHD_OK;
+    return classify(h, d_idx, n);
 }
 
 extern "C" int32_t nhd_load_nodes(nhd_handle* h, int32_t n_nodes, const nhd_node_rec* recs)
@@ -580,7 +590,8 @@ extern "C" int32_t nhd_read_nodes(nhd_handle* h, int32_t first, int32_t n, nhd_n
 
 extern "C" int32_t nhd_snapshot(nhd_handle* h)
 {
-    if (!h || !h->loaded) return NHD_ERR_STATE;
+    if (!h) return NHD_ERR_STATE;
+    if (!h->loaded) return fail(h, NHD_ERR_STATE, "nhd_snapshot before nhd_load_nodes");
     CK(cudaSetDevice(h->params.device));
     h->gen++;
     CK(cudaMemcpyAsync(h->d_snapshot, h->d_nodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
@@ -588,15 +599,26 @@ extern "C" int32_t nhd_snapshot(nhd_handle* h)
     h->have_snapshot = true;
     h->snap_gen = h->gen;
     h->snap_rec_gen = h->rec_gen;
+    h->snap_node_numa = h->node_numa;
+    memcpy(h->snap_numa_hist, h->numa_hist, sizeof(h->numa_hist));
+    h->snap_max_numa = h->max_numa;
     return NHD_OK;
 }
 
+/* The snapshot's records back into the mirror, with the tuple-limit bookkeeping they had.  After an nhd_update_nodes
+ * the mirror's hardware classes describe the updated records, so every node is classified again. */
 extern "C" int32_t nhd_restore(nhd_handle* h)
 {
-    if (!h || !h->loaded || !h->have_snapshot) return NHD_ERR_STATE;
+    if (!h) return NHD_ERR_STATE;
+    if (!h->loaded || !h->have_snapshot)
+        return fail(h, NHD_ERR_STATE, "nhd_restore needs an nhd_snapshot since the last nhd_load_nodes");
     h->gen++;
     CK(cudaSetDevice(h->params.device));
     CK(cudaMemcpyAsync(h->d_nodes, h->d_snapshot, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
+    h->node_numa = h->snap_node_numa;
+    memcpy(h->numa_hist, h->snap_numa_hist, sizeof(h->numa_hist));
+    h->max_numa = h->snap_max_numa;
+    if (h->rec_gen != h->snap_rec_gen && h->n_nodes > 0) return classify(h, nullptr, h->n_nodes);
     return NHD_OK;
 }
 
