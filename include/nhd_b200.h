@@ -341,7 +341,7 @@ int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_excluded, const 
  * Malformed arguments make the whole call NHD_ERR_INVALID: a null pointer, offsets that do not start at 0 or go down,
  * an excluded index outside [0, n_nodes); a duplicate exclusion counts once.  Nothing is written that a caller can
  * observe (the same list as nhd_plan_batch), no collective is entered (any rank may call alone), and the call waits
- * for the device before returning.  Explanations are not part of it: nhd_plan_batch gives a scenario's why_counts.
+ * for the device before returning.  Explanations are not part of it: nhd_plan_scenarios_explained gives them.
  * Meant for many small scenarios (the pods of one node or one rack): one warp runs each, and a pod's cost grows with
  * the number of nodes its scenario's earlier pods reached.  A large single batch belongs to nhd_plan_batch.
  */
@@ -373,6 +373,27 @@ int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int32_t n_scena
                                   const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
                                   const int32_t* pod_start, const nhd_pod* pods, const double* now,
                                   nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod);
+
+/*
+ * nhd_plan_scenarios_edited with reasons: "why does this planned pod find no node?".  Arguments, validation, refusals,
+ * tuple limits, bindings, side effects (none observable), collectives and waiting are exactly those of
+ * nhd_plan_scenarios_edited; with why_counts == NULL the call is nhd_plan_scenarios_edited.
+ *   why_counts     pod_start[n_scenarios] * NHD_WHY_COUNT entries.  For an accepted scenario s and its pod k with status
+ *                  NHD_NO_CANDIDATE, row pod_start[s] + k counts per reason the nodes whose first dropping stage is that
+ *                  reason, on the scenario's records as that pod saw them: the source records with s's edits, with its
+ *                  earlier pods' effects (placements, and the busy stamp of a failed assignment) and with its excluded
+ *                  nodes in maintenance while k < lift_at[s], at clock now[pod_start[s] + k].  That is the row
+ *                  nhd_explain_batch would give the pod after the five steps of nhd_plan_scenarios_edited, taken on the
+ *                  records at the start of the pod's own phase.  Rows of the other pods of accepted scenarios are zero;
+ *                  rows of refused scenarios are not written.
+ * A NO_CANDIDATE row that would not sum to n_nodes, or a node passing every stage for such a pod, is NHD_ERR_STATE.
+ */
+int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                     const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                     const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                                     const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                     nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                     uint32_t* why_counts);
 
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */

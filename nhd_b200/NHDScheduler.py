@@ -243,14 +243,15 @@ class DeviceCluster:
         return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), source=source, exclude=idx,
                   explain=explain)
 
-    def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror'):
+    def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror', explain: bool = False):
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
         of ``(exclude, tops, pod_groups, now[, packed[, lift[, edits]]])`` with ``exclude`` node names.  ``lift`` (None:
         never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits`` (None: none):
         ``{node name: Node-like object}``, packed as ``sync`` packs nodes, the records those nodes have for the whole
         scenario.  Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
-        when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods.  None when the solver
-        in use cannot plan scenarios (a stand-in without ``plan_scenarios``)."""
+        when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods; ``explain=True``: one
+        ``(code, pod, bindings, counts)``, ``counts`` the per-reason node counts of the NO_CANDIDATE pods.  None when
+        the solver in use cannot plan scenarios (a stand-in without ``plan_scenarios``)."""
         fn = getattr(self._solver, 'plan_scenarios', None)
         if fn is None:
             return None
@@ -268,7 +269,7 @@ class DeviceCluster:
                 edits = (self._indices(edits, 'edit'), self._pack(list(edits.values())))
             args.append((idx, self._pods(tops, pod_groups, packed), self._clocks(len(tops), now)) +
                         ((lift, edits or None) if lift is not None or edits else ()))
-        return fn(args, source=source)
+        return fn(args, source=source, explain=True) if explain else fn(args, source=source)
 
     def rewind(self, k: int):
         """Put the device back to the state right after pod ``k`` of the last batch (restore the
@@ -738,41 +739,45 @@ class NHDScheduler:
             raise ValueError(f'unknown node(s) {missing}')
         return self._plan(self._pods_on(names), names)
 
-    def PlanDrains(self, node_groups: Sequence[Sequence[str]] = None) -> Dict:
+    def PlanDrains(self, node_groups: Sequence[Sequence[str]] = None, reasons: bool = False) -> Dict:
         """Which nodes (or groups of nodes) could be taken down, each group on its own?  ``{tuple(group): placement}``
         with ``placement`` what ``PlanDrain(list(group))[0]`` returns from the same state; by default every node that
-        holds pods is its own group, in node order.  All groups are planned side by side in one GPU call; the groups
-        do not see each other.  Each pod is read from Kubernetes once, as a scheduling attempt reads it: no event, no
-        write; ``pod_state``, the ``Node`` objects and the counters stay as they are.  Reasons are not returned:
-        ``PlanDrain(group)`` gives them for the groups that do not drain."""
+        holds pods is its own group, in node order.  ``reasons=True``: ``{tuple(group): (placement, reasons)}``, the
+        whole of what ``PlanDrain(list(group))`` returns, ``reasons[(ns, name)]`` being ``{reason name: nodes}`` for each
+        pod that would find no node.  All groups are planned side by side in one GPU call; the groups do not see each
+        other.  Each pod is read from Kubernetes once, as a scheduling attempt reads it: no event, no write;
+        ``pod_state``, the ``Node`` objects and the counters stay as they are."""
         groups = self._node_groups(node_groups)
         seen = {}
         group_entries = [self._read(self._pods_on(g), seen) for g in groups]
         result = {}
         todo = []
         for g, entries in zip(groups, group_entries):
-            result[g] = {(e.key[0], e.key[1]): None for e in entries}
+            result[g] = ({(e.key[0], e.key[1]): None for e in entries}, {})
             ok = [e for e in entries if e.solvable]
             if ok and self.nodes:
                 todo.append((g, entries, ok))
-        if not todo:
-            return result
-        self._sync()
-        now = float(self._clock())
-        res = self._supported(
-            self.cluster.plan_scenarios([(g, [e.top for e in ok], [e.groups for e in ok], now, [e.rec for e in ok])
-                                         for g, _, ok in todo]), 'plan scenarios (no plan_scenarios)')
-        for (g, entries, ok), (code, _, out) in zip(todo, res):
-            if out is None:
-                # refused (the tuple limits are judged with the group's own nodes counted): the single plan judges
-                # them without, and drops a pod beyond them, or raises, as PlanDrain does
-                result[g] = self._plan_prepared(entries, list(g), now)[0]
-            else:
-                result[g].update(self._placements(ok, out))
-        return result
+        if todo:
+            self._sync()
+            now = float(self._clock())
+            res = self._supported(
+                self.cluster.plan_scenarios([(g, [e.top for e in ok], [e.groups for e in ok], now, [e.rec for e in ok])
+                                             for g, _, ok in todo], explain=reasons),
+                'plan scenarios (no plan_scenarios)')
+            for (g, entries, ok), r in zip(todo, res):
+                out = r[2]
+                if out is None:
+                    # refused (the tuple limits are judged with the group's own nodes counted): the single plan judges
+                    # them without, and drops a pod beyond them, or raises, as PlanDrain does
+                    result[g] = self._plan_prepared(entries, list(g), now)
+                else:
+                    result[g][0].update(self._placements(ok, out))
+                    if reasons:
+                        result[g][1].update(self._reasons(ok, out, r[3]))
+        return result if reasons else {g: v[0] for g, v in result.items()}
 
     def PlanDefrag(self, keys: Sequence = None, node_groups: Sequence[Sequence[str]] = None,
-                   delay: float = None) -> Dict:
+                   delay: float = None, reasons: bool = False) -> Dict:
         """Which nodes (or groups of nodes), drained and put back in service, would let the pending pods place?  For
         every group, the maintenance workflow planned from the same state, all groups side by side in one GPU call:
           1. ``NODE_MAINT_START`` on the group's nodes;
@@ -791,7 +796,10 @@ class NHDScheduler:
         (its delete would re-scan every node): its pods map to None and ``pending`` is None.
         Only reads happen, as ``PlanDrains``: each pod is read from Kubernetes once (a scheduling attempt's reads and
         a release's); the releases run on copies of the ``Node`` objects; ``pod_state``, the ``Node`` objects and the
-        counters stay as they are."""
+        counters stay as they are.
+        ``reasons=True``: ``{tuple(group): (moved, pending, reasons)}``, ``reasons[(ns, name)]`` being ``{reason name:
+        nodes}`` (as ``PlanDrain`` gives them) for each moved pod that finds no node and, when ``pending`` is not None,
+        each pod of ``keys`` that finds no node, at the state that pod sees in the workflow."""
         groups = self._node_groups(node_groups)
         if keys is None:
             phase = self._service_pods()
@@ -804,9 +812,9 @@ class NHDScheduler:
             if key not in targets:
                 targets[key] = self._release_target(key[1], key[0])
         entries = [self._read(pods, seen) for pods in group_pods]
-        result = {g: ({key: None for key in pods}, None) for g, pods in zip(groups, group_pods)}
+        result = {g: ({key: None for key in pods}, None, {}) for g, pods in zip(groups, group_pods)}
         if not self.nodes:
-            return result
+            return result if reasons else {g: v[:2] for g, v in result.items()}
         self._sync()
         now = float(self._clock())
         todo = []
@@ -827,10 +835,11 @@ class NHDScheduler:
             todo.append((g, [e for e in moved if e.solvable], tail, edits))
         while todo:
             res = self._supported(self.cluster.plan_scenarios([self._defrag_scenario(g, ok, tail, edits, now, delay)
-                                                               for g, ok, tail, edits in todo]),
+                                                               for g, ok, tail, edits in todo], explain=reasons),
                                   'plan scenarios (no plan_scenarios)')
             retry = []
-            for (g, ok, tail, edits), (code, pod, out) in zip(todo, res):
+            for (g, ok, tail, edits), r in zip(todo, res):
+                code, pod, out = r[:3]
                 if out is None:
                     # a pod beyond the tuple limits (judged with the group's nodes and the edited records counted):
                     # it gets None, as in PlanDrain, and the group is planned again without it
@@ -842,14 +851,18 @@ class NHDScheduler:
                         tail = tail[:pod - len(ok)] + tail[pod - len(ok) + 1:]
                     retry.append((g, ok, tail, edits))
                     continue
-                moved, _ = result[g]
+                moved, _, why = result[g]
                 moved.update(self._placements(ok, out[:len(ok)]))
+                if reasons:
+                    why.update(self._reasons(ok, out[:len(ok)], r[3][:len(ok)]))
                 if all(v is not None for v in moved.values()):
                     pending = {(k[0], k[1]): None for k in keys}
                     pending.update(self._placements(tail, out[len(ok):]))
-                    result[g] = (moved, pending)
+                    if reasons:
+                        why.update(self._reasons(tail, out[len(ok):], r[3][len(ok):]))
+                    result[g] = (moved, pending, why)
             todo = retry
-        return result
+        return result if reasons else {g: v[:2] for g, v in result.items()}
 
     @staticmethod
     def _defrag_scenario(g, moved, tail, edits, now, delay):
@@ -876,9 +889,14 @@ class NHDScheduler:
             return placement, {}
         out, counts = res
         placement.update(self._placements(ok, out))
-        reasons = {(e.key[0], e.key[1]): {name: int(n) for name, n in zip(wire.WHY_NAMES, c) if int(n)}
-                   for e, b, c in zip(ok, out, counts) if int(b['status']) == wire.NO_CANDIDATE}
-        return placement, reasons
+        return placement, self._reasons(ok, out, counts)
+
+    @staticmethod
+    def _reasons(entries: Sequence, out, counts) -> Dict:
+        """``{(ns, name): {reason name: nodes}}`` of the NO_CANDIDATE pods among ``entries`` from their bindings ``out``
+        and per-reason node counts ``counts``."""
+        return {(e.key[0], e.key[1]): {name: int(n) for name, n in zip(wire.WHY_NAMES, c) if int(n)}
+                for e, b, c in zip(entries, out, counts) if int(b['status']) == wire.NO_CANDIDATE}
 
     # ---- shared by the batch, the previews and the plans ------------------------------------------------------
     def _read(self, keys: Sequence, seen: Dict = None) -> List[_Pending]:

@@ -18,8 +18,10 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <map>
 #include <mutex>
 #include <string>
+#include <tuple>
 #include <unordered_map>
 #include <vector>
 
@@ -1279,11 +1281,61 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
  * limits are judged against the whole cluster's NUMA counts and those of the edit records: the shared filter
  * enumerates the tuples of every node, the excluded ones included, and an edited node is evaluated on its own record.
  */
+/*
+ * why_counts of the scenario call just run on w (its bindings b, its pods and clocks run_pods / run_now, its correction
+ * rows in d_xpod + 2 * n_run): the NO_CANDIDATE pods' keys (pod type, clock, node-group mask) de-duplicated, one
+ * explain_kernel pass per key over the source records with no bindings (empty per-node lists), then
+ * scenario_why_combine_kernel adds each pod's correction to its key's row.  rows: n_run * NHD_WHY_COUNT host entries.
+ * Buffers were sized before the scenario kernel; one host wait.
+ */
+static int32_t scenario_reasons(nhd_handle* h, const Workspace& w, const uint8_t* records, int n_run,
+                                const nhd_pod* run_pods, const double* run_now, const nhd_binding* b, uint32_t* rows,
+                                const char* what)
+{
+    const int N = h->n_nodes;
+    std::vector<int32_t> idx(2 * (size_t)n_run, -1);              /* base_row | key representatives */
+    std::map<std::tuple<int32_t, uint64_t, uint64_t>, int32_t> keys;
+    int n_keys = 0;
+    for (int i = 0; i < n_run; i++) {
+        if (b[i].status != NHD_NO_CANDIDATE) continue;
+        uint64_t clock;
+        memcpy(&clock, &run_now[i], 8);
+        const auto it = keys.emplace(std::make_tuple(w.pod_type_host[i], clock, w.n_names ? run_pods[i].group_mask : 0), i).first;
+        if (it->second == i) idx[(size_t)n_run + n_keys++] = i;
+        idx[i] = it->second;
+    }
+    if (n_keys == 0) {
+        memset(rows, 0, (size_t)n_run * NHD_WHY_COUNT * 4);
+        return NHD_OK;
+    }
+    uint32_t* base = h->d_xcounts;
+    uint32_t* d_rows = h->d_xcounts + (size_t)n_run * NHD_WHY_COUNT;
+    const int32_t small[4] = {n_keys, 0, 0, 0};                  /* n_failed (keys), survivors, bad */
+    CK(cudaMemcpyAsync(h->d_xpod, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemcpyAsync(h->d_xsmall, small, 16, cudaMemcpyHostToDevice, h->stream));
+    CK(cudaMemsetAsync(h->d_xnode + N, 0, ((size_t)N + 1) * 4, h->stream));
+    CK(cudaMemsetAsync(base, 0, (size_t)n_run * NHD_WHY_COUNT * 4, h->stream));
+    /* the key's row on the source records: the representative pod with nothing bound before it; nodes that pass
+     * every stage land in survivors, which is not read (pass bucket = n_nodes - row sum) */
+    int32_t rc = explain_launch(h, w, records, n_keys, base, nullptr);
+    if (rc != NHD_OK) return rc;
+    scenario_why_combine_kernel<<<(unsigned)((n_run + 255) / 256), 256, 0, h->stream>>>(
+        base, h->d_xpod, h->d_xpod + 2 * (size_t)n_run, n_run, N, d_rows, h->d_xsmall + 2);
+    CK(cudaGetLastError());
+    uint32_t bad = 0;
+    CK(cudaMemcpyAsync(rows, d_rows, (size_t)n_run * NHD_WHY_COUNT * 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaMemcpyAsync(&bad, h->d_xsmall + 2, 4, cudaMemcpyDeviceToHost, h->stream));
+    CK(cudaStreamSynchronize(h->stream));
+    if (bad) return fail(h, NHD_ERR_STATE, "%s: %u NO_CANDIDATE rows with a negative bucket or a node passing every stage",
+                         what, bad);
+    return NHD_OK;
+}
+
 static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, int32_t n_scenarios,
                               const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
                               const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
                               const int32_t* pod_start, const nhd_pod* pods, const double* now, nhd_binding* out,
-                              int32_t* scenario_status, int32_t* scenario_pod)
+                              int32_t* scenario_status, int32_t* scenario_pod, uint32_t* why_counts)
 {
     if (!h || n_scenarios < 0 || !excl_start || !pod_start || (n_scenarios > 0 && (!scenario_status || !scenario_pod)))
         return NHD_ERR_INVALID;
@@ -1380,6 +1432,12 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     uint4* d_edit_rec = h->d_swork + n_slots * REC_CHUNKS;
     if (n_ed > 0)
         CK(cudaMemcpyAsync(d_edit_rec, ed_rec.data(), (size_t)n_ed * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
+    if (why_counts) {       /* scenario_reasons' buffers: base rows | rows, base_row | keys | corrections, node lists */
+        CK(h->d_xcounts.grow((size_t)2 * n_run * NHD_WHY_COUNT * 4));
+        CK(h->d_xpod.grow((size_t)n_run * (NHD_WHY_COUNT + 3) * 4));
+        CK(h->d_xnode.grow(((size_t)2 * h->n_nodes + 1) * 4));
+        CK(h->d_xsmall.grow(16));
+    }
 
     /* the candidate bitmaps of the call's pod types on the unchanged source records */
     if ((rc = launch_solve(h, w, records, false, true)) != NHD_OK) return rc;
@@ -1394,9 +1452,13 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     sa.n_scenarios = n_acc; sa.n_types = w.n_types; sa.words = h->words;
     sa.min_busy = h->params.min_busy_secs;
     memcpy(sa.cap, h->cap, sizeof(sa.cap));
+    sa.why_delta = why_counts ? h->d_xpod + 2 * (size_t)n_run : nullptr;
     const int warps_per_cta = SCENARIO_THREADS / 32;
     const int grid = std::min((n_acc + warps_per_cta - 1) / warps_per_cta, h->sm_count * 16);
-    scenario_plan_kernel<<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
+    if (why_counts)
+        scenario_plan_kernel<true><<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
+    else
+        scenario_plan_kernel<false><<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
     CK(cudaGetLastError());
     uint32_t bad = 0;
     CK(cudaMemcpyAsync(&bad, h->d_sidx + off_bad, 4, cudaMemcpyDeviceToHost, h->stream));
@@ -1404,9 +1466,21 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     if (compact) run.resize(n_run);
     if ((rc = fetch_bindings(h, w, n_run, compact ? run.data() : out)) != NHD_OK) return rc;
     if (bad) return fail(h, NHD_ERR_STATE, "%s: %u chosen nodes without a mapping", what, bad);
+    std::vector<uint32_t> run_rows;
+    if (why_counts) {
+        if (compact) run_rows.resize((size_t)n_run * NHD_WHY_COUNT);
+        if ((rc = scenario_reasons(h, w, records, n_run, compact ? cpods.data() : pods, compact ? cnow.data() : now,
+                                   compact ? run.data() : out, compact ? run_rows.data() : why_counts, what)) != NHD_OK)
+            return rc;
+    }
     if (compact)
-        for (int k = 0; k < n_acc; k++)
-            memcpy(out + pod_start[acc[k]], run.data() + pod_off[k], (size_t)(pod_off[k + 1] - pod_off[k]) * sizeof(nhd_binding));
+        for (int k = 0; k < n_acc; k++) {
+            const size_t n_k = (size_t)(pod_off[k + 1] - pod_off[k]);
+            memcpy(out + pod_start[acc[k]], run.data() + pod_off[k], n_k * sizeof(nhd_binding));
+            if (why_counts)
+                memcpy(why_counts + (size_t)pod_start[acc[k]] * NHD_WHY_COUNT,
+                       run_rows.data() + (size_t)pod_off[k] * NHD_WHY_COUNT, n_k * NHD_WHY_COUNT * 4);
+        }
     return NHD_OK;
 }
 
@@ -1416,7 +1490,7 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
                                       int32_t* scenario_pod)
 {
     return plan_scenarios(h, "nhd_plan_scenarios", source, n_scenarios, excl_start, excluded, nullptr, nullptr, nullptr,
-                          nullptr, pod_start, pods, now, out, scenario_status, scenario_pod);
+                          nullptr, pod_start, pods, now, out, scenario_status, scenario_pod, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1427,7 +1501,21 @@ extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int3
                                              int32_t* scenario_pod)
 {
     return plan_scenarios(h, "nhd_plan_scenarios_edited", source, n_scenarios, excl_start, excluded, lift_at,
-                          edit_start, edit_node, edit_rec, pod_start, pods, now, out, scenario_status, scenario_pod);
+                          edit_start, edit_node, edit_rec, pod_start, pods, now, out, scenario_status, scenario_pod,
+                          nullptr);
+}
+
+extern "C" int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                                const int32_t* excl_start, const int32_t* excluded,
+                                                const int32_t* lift_at, const int32_t* edit_start,
+                                                const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                                                const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                                nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                                uint32_t* why_counts)
+{
+    return plan_scenarios(h, "nhd_plan_scenarios_explained", source, n_scenarios, excl_start, excluded, lift_at,
+                          edit_start, edit_node, edit_rec, pod_start, pods, now, out, scenario_status, scenario_pod,
+                          why_counts);
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

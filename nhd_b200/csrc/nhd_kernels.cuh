@@ -2782,6 +2782,9 @@ struct ScenarioArgs {
     int n_scenarios, n_types, words;
     double min_busy;
     double cap[NHD_MAX_SPEED_CLASSES];
+    int32_t* why_delta;            /* scenario_plan_kernel<true>: [n_pods][NHD_WHY_COUNT + 1], written for NO_CANDIDATE
+                                      pods only: per reason (pass last), the nodes of C(i) counted on the scenario's
+                                      records minus those counted on the source records */
 };
 
 constexpr int SCENARIO_THREADS = 128;
@@ -2796,12 +2799,59 @@ __device__ __forceinline__ bool sorted_contains(const int32_t* v, int n, int x)
     return lo < n && v[lo] == x;
 }
 
+/* scenario_plan_kernel<true> at a NO_CANDIDATE pod, the whole warp: the nodes whose record differs from the source
+ * record, C(i) = the touched nodes (working records) and the held exclusions that are not touched (source records),
+ * NHD_NODE_MAINTENANCE set on the local copy while held, each evaluated on that record and on its source record
+ * (explain_node).  Lane 0 writes per reason, pass bucket last, the nodes counted on the scenario's records minus those
+ * counted on the source records: the pod's row is the source records' count plus this row (DESIGN.md section 8.11). */
+__device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const PodType& t, uint64_t groups, double now,
+                                                const int32_t* ex, int n_ex, const uint4* work,
+                                                const int32_t* work_node, int n_touched, int32_t* row)
+{
+    const int lane = threadIdx.x & 31, total = n_touched + n_ex;
+    int acc[NHD_WHY_COUNT + 1];
+#pragma unroll
+    for (int r = 0; r <= NHD_WHY_COUNT; r++) acc[r] = 0;
+    for (int base = 0; base < total; base += 32) {
+        const int k = base + lane;
+        int was = -1, is = -1;
+        if (k < total) {
+            const int node = k < n_touched ? work_node[k] : ex[k - n_touched];
+            bool counted = true;                                       /* a touched exclusion counts as touched */
+            for (int j = 0; j < n_touched && k >= n_touched && counted; j++) counted = work_node[j] != node;
+            if (counted) {
+                RecU src, u;
+                load_rec(a.nodes, node, src);
+                if (k < n_touched) {
+#pragma unroll
+                    for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)k * REC_CHUNKS + c];
+                } else {
+                    u = src;
+                }
+                if (sorted_contains(ex, n_ex, node)) u.r.flags |= (uint8_t)NHD_NODE_MAINTENANCE;
+                was = explain_node(src.r, t, groups, now, a.min_busy, a.cap);
+                is = explain_node(u.r, t, groups, now, a.min_busy, a.cap);
+                if (was == is) was = is = -1;
+            }
+        }
+#pragma unroll
+        for (int r = 0; r <= NHD_WHY_COUNT; r++)
+            acc[r] += __popc(__ballot_sync(0xFFFFFFFFu, is == r)) - __popc(__ballot_sync(0xFFFFFFFFu, was == r));
+    }
+    if (lane == 0) {
+#pragma unroll
+        for (int r = 0; r <= NHD_WHY_COUNT; r++) row[r] = acc[r];
+    }
+}
+
 /* One warp per scenario (grid-stride).  The working set starts with the scenario's edited records.  For each pod: the
  * first touched node, not excluded, that passes every stage on its working record (explain_node, lanes over the touched
  * set, warp minimum) and the first untouched candidate (query_select_kernel's ballot scan, skipping excluded and touched
  * nodes), GPU-less pass first for a pod without GPUs (Matcher.py:412-421);
  * then lane 0 runs the mapping and the assignment (query_assign_kernel's body) on that node's working record, keeps
- * the result as the node's working record and writes the binding. */
+ * the result as the node's working record and writes the binding.  WHY: at a NO_CANDIDATE pod, before any later pod
+ * overwrites the working set, the pod's correction row (scenario_why_delta). */
+template <bool WHY>
 __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const __grid_constant__ ScenarioArgs a)
 {
     const int lane = threadIdx.x & 31, W = a.words;
@@ -2910,10 +2960,44 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
                 }
                 for (int c = 0; c < 8; c++) bout[c] = bu.q[c];
             }
+            if constexpr (WHY) {
+                if (chosen < 0)                                        /* warp-uniform */
+                    scenario_why_delta(a, t, a.pod_groups ? gm : t.pod.group_mask, now, ex, n_ex, work, work_node,
+                                       n_touched, a.why_delta + (size_t)i * (NHD_WHY_COUNT + 1));
+            }
             if (chosen >= 0 && slot == n_touched) n_touched++;
             __syncwarp();                                              /* the slot is read by every lane from here on */
         }
     }
+}
+
+/* nhd_plan_scenarios_explained, one thread per pod: a NO_CANDIDATE pod's row is the source records' row of its key
+ * (explain_kernel's counts row base_row[i]; its pass bucket is n_nodes minus the row's sum) plus the pod's correction
+ * row; every other pod (base_row[i] < 0) gets a zero row.  A negative bucket or a node left passing every stage means
+ * the state was not rebuilt as the pod saw it: counted in *bad, which the host refuses. */
+__global__ void scenario_why_combine_kernel(const uint32_t* __restrict__ base, const int32_t* __restrict__ base_row,
+                                            const int32_t* __restrict__ delta, int n_pods, int n_nodes,
+                                            uint32_t* __restrict__ out, uint32_t* bad)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_pods) return;
+    uint32_t* o = out + (size_t)i * NHD_WHY_COUNT;
+    const int b = base_row[i];
+    if (b < 0) {
+        for (int r = 0; r < NHD_WHY_COUNT; r++) o[r] = 0;
+        return;
+    }
+    const uint32_t* br = base + (size_t)b * NHD_WHY_COUNT;
+    const int32_t* d = delta + (size_t)i * (NHD_WHY_COUNT + 1);
+    long long pass = n_nodes + (long long)d[NHD_WHY_COUNT];
+    bool ok = true;
+    for (int r = 0; r < NHD_WHY_COUNT; r++) {
+        const long long v = (long long)br[r] + d[r];
+        pass -= br[r];
+        ok = ok && v >= 0;
+        o[r] = v < 0 ? 0u : (uint32_t)v;
+    }
+    if (!ok || pass != 0) atomicAdd(bad, 1u);
 }
 
 } // namespace nhd

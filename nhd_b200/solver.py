@@ -224,11 +224,14 @@ class Solver:
                                         counts.ctypes.data if explain else None))
         return (out, counts) if explain else out
 
-    def plan_scenarios(self, scenarios, source='mirror'):
+    def plan_scenarios(self, scenarios, source='mirror', explain=False):
         """Many independent dry runs in one call (``nhd_plan_scenarios_edited``).  ``scenarios``: a sequence of
         ``(exclude, pods, now[, lift[, edits]])``.  Returns one ``(code, pod, bindings)`` per scenario: ``code`` 0 and
         ``bindings`` what ``plan_batch(pods, now, source, exclude)`` returns, or the refusal ``plan_batch`` would raise
-        (``wire.ERR_*``), the index of the pod it names and None.  Scenarios do not see each other.  Unlike
+        (``wire.ERR_*``), the index of the pod it names and None.  ``explain=True`` (``nhd_plan_scenarios_explained``):
+        one ``(code, pod, bindings, counts)`` per scenario, ``counts`` a ``(n_s, wire.WHY_COUNT)`` uint32 array of
+        per-reason node counts for the NO_CANDIDATE pods at the state each saw (zero rows for the others), as
+        ``plan_batch(..., explain=True)`` gives them, or None when refused.  Scenarios do not see each other.  Unlike
         ``plan_batch`` the tuple limits are judged with the excluded nodes counted; ``plan_batch`` plans a scenario
         refused for that.
         ``lift`` (None: never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits``
@@ -275,16 +278,19 @@ class Solver:
         out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
         status = np.zeros(n, dtype='<i4')
         which = np.zeros(n, dtype='<i4')
-        self._ck(self._L.nhd_plan_scenarios_edited(self._h, src, n, excl_start.ctypes.data,
-                                                   ex.ctypes.data if len(ex) else None,
-                                                   lift.ctypes.data if n else None, edit_start.ctypes.data,
-                                                   ednode.ctypes.data if len(ednode) else None,
-                                                   edrec.ctypes.data if len(edrec) else None, pod_start.ctypes.data,
-                                                   pods.ctypes.data if len(pods) else None,
-                                                   now.ctypes.data if len(pods) else None,
-                                                   out.ctypes.data if len(pods) else None, status.ctypes.data,
-                                                   which.ctypes.data))
-        return [(code, pod, out[a:b] if code == 0 else None)
+        args = (self._h, src, n, excl_start.ctypes.data, ex.ctypes.data if len(ex) else None,
+                lift.ctypes.data if n else None, edit_start.ctypes.data, ednode.ctypes.data if len(ednode) else None,
+                edrec.ctypes.data if len(edrec) else None, pod_start.ctypes.data,
+                pods.ctypes.data if len(pods) else None, now.ctypes.data if len(pods) else None,
+                out.ctypes.data if len(pods) else None, status.ctypes.data, which.ctypes.data)
+        if not explain:
+            self._ck(self._L.nhd_plan_scenarios_edited(*args))
+            return [(code, pod, out[a:b] if code == 0 else None)
+                    for code, pod, a, b in zip(status.tolist(), which.tolist(), pod_start[:-1].tolist(),
+                                               pod_start[1:].tolist())]
+        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4')
+        self._ck(self._L.nhd_plan_scenarios_explained(*args, counts.ctypes.data if len(pods) else None))
+        return [(code, pod, out[a:b], counts[a:b]) if code == 0 else (code, pod, None, None)
                 for code, pod, a, b in zip(status.tolist(), which.tolist(), pod_start[:-1].tolist(), pod_start[1:].tolist())]
 
     def filter_bitmaps(self):

@@ -9,7 +9,8 @@ the exclusion lifted.  Three cases:
   * n-1: one call, one scenario per node holding pods;
   * racks: one call, 64 racks of 32 consecutive nodes (rack r = nodes 1024 r .. 1024 r + 31);
   * the same two sets as ``nhd_plan_scenarios`` of the drains alone (no edits, no lift, no pending tail): what the
-    return-to-service phase adds.
+    return-to-service phase adds;
+  * each defrag set again with reasons (``nhd_plan_scenarios_explained``).
 Prints, per case, the device time of one call (kernels and device-side copies, summed per kernel from torch.profiler's
 CUDA activity) and the host time per call (median).  The card's name and power limit are read in the same run.
 
@@ -29,6 +30,7 @@ sys.path.insert(0, os.path.join(ROOT, 'tools'))
 
 import workload                                     # noqa: E402
 from drains_bench import timed                      # noqa: E402
+from nhd_b200 import wire                           # noqa: E402
 from nhd_b200.solver import Solver                  # noqa: E402
 
 CAP = 64
@@ -70,10 +72,13 @@ def main(argv=None):
             defrag = [f for _, f in pairs]
             dev, host, kern = timed(lambda: s.plan_scenarios(defrag), args.reps)
             ddev, dhost, dkern = timed(lambda: s.plan_scenarios(drains), args.reps)
+            xdev, xhost, xkern = timed(lambda: s.plan_scenarios(defrag, explain=True), args.reps)
             rows.append({'set': name, 'scenarios': len(defrag), 'pods': int(sum(len(sc[1]) for sc in defrag)),
                          'call_device_ms': round(dev, 4), 'call_host_ms': round(host, 4), 'per_kernel_ms': kern,
                          'drains_only_device_ms': round(ddev, 4), 'drains_only_host_ms': round(dhost, 4),
-                         'drains_only_per_kernel_ms': dkern})
+                         'drains_only_per_kernel_ms': dkern, 'reasons_device_ms': round(xdev, 4),
+                         'reasons_host_ms': round(xhost, 4), 'reasons_per_kernel_ms': xkern,
+                         'no_candidate': sum(int((g[2]['status'] == wire.NO_CANDIDATE).sum()) for g in s.plan_scenarios(defrag))})
     finally:
         s.close()
     info = {'gpu': torch.cuda.get_device_name(0), 'nodes': len(recs), 'pending': n_tail, 'reps': args.reps}
@@ -92,6 +97,9 @@ def main(argv=None):
                   f"{r['drains_only_host_ms']:.4f} ms host")
             print('    call:   ' + ', '.join(f'{k} {v}' for k, v in r['per_kernel_ms'].items()))
             print('    drains: ' + ', '.join(f'{k} {v}' for k, v in r['drains_only_per_kernel_ms'].items()))
+            print(f"    with reasons ({r['no_candidate']} NO_CANDIDATE pods): {r['reasons_device_ms']:.4f} ms device / "
+                  f"{r['reasons_host_ms']:.4f} ms host")
+            print('    reasons: ' + ', '.join(f'{k} {v}' for k, v in r['reasons_per_kernel_ms'].items()))
 
 
 if __name__ == '__main__':

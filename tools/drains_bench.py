@@ -6,7 +6,8 @@ After the 4 096-pod solve of config 4 (so that the nodes hold pods), two scenari
   * racks: 64 racks of 32 consecutive nodes (rack r = nodes 1024 r .. 1024 r + 31), each excluded with its pods.
 Prints, per set, the device time of one call (kernels and device-side copies, summed per kernel from torch.profiler's
 CUDA activity), the host time per call (median), and the same two figures for the loop of ``nhd_plan_batch`` calls
-answering the same scenarios one by one.  The card's name and power limit are read in the same run.
+answering the same scenarios one by one; then the same with reasons: ``nhd_plan_scenarios_explained`` and the loop of
+``nhd_plan_batch(..., why_counts)``.  The card's name and power limit are read in the same run.
 
     python tools/drains_bench.py [--reps 5] [--json]
 """
@@ -23,6 +24,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 import workload                                     # noqa: E402
+from nhd_b200 import wire                           # noqa: E402
 from nhd_b200.solver import Solver                  # noqa: E402
 
 
@@ -77,9 +79,20 @@ def main(argv=None):
                 for ex, p, c in scens:
                     s.plan_batch(p, c, exclude=ex)
             ldev, lhost, lkern = timed(loop, args.loop_reps)
+            xdev, xhost, xkern = timed(lambda: s.plan_scenarios(scens, explain=True), args.reps)
+
+            def xloop():
+                for ex, p, c in scens:
+                    s.plan_batch(p, c, exclude=ex, explain=True)
+            xldev, xlhost, xlkern = timed(xloop, args.loop_reps)
+            failed = sum(int((g[2]['status'] == wire.NO_CANDIDATE).sum()) for g in s.plan_scenarios(scens))
             rows.append({'set': name, 'scenarios': len(scens), 'pods': int(sum(len(p) for _, p, _ in scens)),
+                         'no_candidate': failed,
                          'call_device_ms': round(dev, 4), 'call_host_ms': round(host, 4), 'per_kernel_ms': kern,
-                         'loop_device_ms': round(ldev, 3), 'loop_host_ms': round(lhost, 3), 'loop_per_kernel_ms': lkern})
+                         'loop_device_ms': round(ldev, 3), 'loop_host_ms': round(lhost, 3), 'loop_per_kernel_ms': lkern,
+                         'reasons_call_device_ms': round(xdev, 4), 'reasons_call_host_ms': round(xhost, 4),
+                         'reasons_per_kernel_ms': xkern, 'reasons_loop_device_ms': round(xldev, 3),
+                         'reasons_loop_host_ms': round(xlhost, 3), 'reasons_loop_per_kernel_ms': xlkern})
     finally:
         s.close()
     info = {'gpu': torch.cuda.get_device_name(0), 'nodes': len(recs), 'reps': args.reps, 'loop_reps': args.loop_reps}
@@ -99,6 +112,11 @@ def main(argv=None):
                   f"{r['loop_host_ms']:.3f} ms host")
             print('    call: ' + ', '.join(f'{k} {v}' for k, v in r['per_kernel_ms'].items()))
             print('    loop: ' + ', '.join(f'{k} {v}' for k, v in r['loop_per_kernel_ms'].items()))
+            print(f"    with reasons ({r['no_candidate']} NO_CANDIDATE pods): one call {r['reasons_call_device_ms']:.4f} ms "
+                  f"device / {r['reasons_call_host_ms']:.4f} ms host; loop {r['reasons_loop_device_ms']:.3f} ms device / "
+                  f"{r['reasons_loop_host_ms']:.3f} ms host")
+            print('    call: ' + ', '.join(f'{k} {v}' for k, v in r['reasons_per_kernel_ms'].items()))
+            print('    loop: ' + ', '.join(f'{k} {v}' for k, v in r['reasons_loop_per_kernel_ms'].items()))
 
 
 if __name__ == '__main__':
