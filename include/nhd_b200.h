@@ -395,6 +395,35 @@ int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, int32_t n_sc
                                      nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
                                      uint32_t* why_counts);
 
+/*
+ * nhd_plan_scenarios_explained on a grown cluster: "would these added nodes let the pending pods place?".  Scenario s
+ * also adds the records add_rec[a], a in [add_start[s], add_start[s+1]):
+ *   - added node a joins the node order right before source node add_at[a] (add_at[a] == n_nodes: after the last
+ *     node); added nodes with the same add_at keep their array order; add_at never goes down inside a scenario;
+ *   - an added node is in service for the whole scenario: exclusions, edits and lift_at refer to source nodes only.
+ *   out[pod_start[s] .. pod_start[s+1])  when scenario_status[s] == NHD_OK: byte for byte what nhd_solve_batch would
+ *                  return after the five steps of nhd_plan_scenarios_edited taken on a scratch copy of the source
+ *                  records with the edits applied and the added records inserted at their positions, every node index
+ *                  mapped back: a source node to its index, added node a to n_nodes + a (a the call-wide index into
+ *                  add_rec, also when refused scenarios are left out).
+ *   why_counts     (may be NULL) as for nhd_plan_scenarios_explained, counted over the scenario's grown node list: a
+ *                  NO_CANDIDATE row sums to n_nodes + add_start[s+1] - add_start[s].
+ * The tuple limits are judged against the largest of the cluster's largest schedulable NUMA count, the n_numa of every
+ * edit record and the n_numa of every added record of the call.  Besides nhd_plan_scenarios_explained's malformed
+ * arguments, the whole call is NHD_ERR_INVALID for add offsets that do not start at 0 or go down, an add_at outside
+ * [0, n_nodes] or going down inside a scenario, an added record nhd_validate_node rejects, and an added record with a
+ * NIC of a speed class at or above the handle's n_speed_classes (the handle holds no capacity for it).  add_start ==
+ * NULL means no additions (add_at and add_rec are not read): the call is nhd_plan_scenarios_explained.  Side effects
+ * (none observable), collectives and waiting as for nhd_plan_scenarios.
+ */
+int32_t nhd_plan_scenarios_grown(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                 const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                 const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                                 const int32_t* add_start, const int32_t* add_at, const nhd_node_rec* add_rec,
+                                 const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                 nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                 uint32_t* why_counts);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

@@ -178,6 +178,21 @@ class DeviceCluster:
             self._solver.update_nodes(idx, recs)
             self.delta_nodes += len(idx)
 
+    def pack_candidates(self, nodes: Sequence) -> np.ndarray:
+        """Records of nodes the cluster does not hold (planned additions), packed with the cluster layout as ``sync``
+        packs nodes; this may register new group names and NIC speeds (a new speed: the next ``sync`` reloads, so
+        sync after packing candidates).  A node whose labels were refused (inactive) is the inactive stub ``sync``
+        would make of it; an active node outside the packed limits is a ValueError naming it, never a stub."""
+        recs = np.zeros(len(nodes), dtype=wire.NODE_DTYPE)
+        for i, node in enumerate(nodes):
+            try:
+                packing.pack_node(node, self._layout, out=recs[i])
+            except packing.UnsupportedError as err:
+                if node.active:
+                    raise ValueError(f'candidate node {node.name} is outside the packed limits: {err}') from err
+                packing.stub_record(recs[i])
+        return recs
+
     def _pods(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], packed: Sequence = None) -> np.ndarray:
         pods = np.zeros(len(tops), dtype=wire.POD_DTYPE)
         for i, top in enumerate(tops):
@@ -248,18 +263,25 @@ class DeviceCluster:
         of ``(exclude, tops, pod_groups, now[, packed[, lift[, edits]]])`` with ``exclude`` node names.  ``lift`` (None:
         never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits`` (None: none):
         ``{node name: Node-like object}``, packed as ``sync`` packs nodes, the records those nodes have for the whole
-        scenario.  Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
+        scenario.  ``adds`` (eighth element, None: none): ``[(before, node)]``, Node-like objects in service for the
+        whole scenario, each joining the node order right before the node named ``before`` (None: after the last
+        node), packed by ``pack_candidates`` before any pod (a pod may request a group name only a candidate carries).
+        Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
         when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods; ``explain=True``: one
-        ``(code, pod, bindings, counts)``, ``counts`` the per-reason node counts of the NO_CANDIDATE pods.  None when
-        the solver in use cannot plan scenarios (a stand-in without ``plan_scenarios``)."""
+        ``(code, pod, bindings, counts)``, ``counts`` the per-reason node counts of the NO_CANDIDATE pods.  A pod
+        placed on an added node gets node ``n_nodes + a``, ``a`` counting the additions of the call in the order given,
+        scenario by scenario (``name_of`` does not know them).  None when the solver in use cannot plan scenarios (a
+        stand-in without ``plan_scenarios``)."""
         fn = getattr(self._solver, 'plan_scenarios', None)
         if fn is None:
             return None
-        # every scenario's names are checked before any is packed
-        self._indices(sorted({n for sc in scenarios for n in list(sc[0]) + list(sc[6] if len(sc) > 6 and sc[6] else ())}),
-                      'exclude or edit')
-        args = []
-        for sc in scenarios:
+        # every scenario's names are checked, and every candidate packed, before any pod is packed
+        self._indices(sorted({n for sc in scenarios for n in list(sc[0]) + list(sc[6] if len(sc) > 6 and sc[6] else ())} |
+                             {b for sc in scenarios if len(sc) > 7 and sc[7] for b, _ in sc[7] if b is not None}),
+                      'exclude, edit or add before')
+        added = [self.pack_candidates([node for _, node in sc[7]]) if len(sc) > 7 and sc[7] else None for sc in scenarios]
+        args, perm = [], []                           # perm: the call's additions in position order -> as given
+        for sc, recs in zip(scenarios, added):
             exclude, tops, pod_groups, now = sc[:4]
             packed = sc[4] if len(sc) > 4 else None
             lift = sc[5] if len(sc) > 5 else None
@@ -267,9 +289,22 @@ class DeviceCluster:
             idx = self._indices(exclude, 'exclude')
             if edits:
                 edits = (self._indices(edits, 'edit'), self._pack(list(edits.values())))
+            adds = None
+            if recs is not None:
+                at = np.asarray([len(self._names) if b is None else self._index[b] for b, _ in sc[7]], dtype='<i4')
+                order = np.argsort(at, kind='stable')
+                adds = (at[order], recs[order])
+                perm.extend((len(perm) + order).tolist())
             args.append((idx, self._pods(tops, pod_groups, packed), self._clocks(len(tops), now)) +
-                        ((lift, edits or None) if lift is not None or edits else ()))
-        return fn(args, source=source, explain=True) if explain else fn(args, source=source)
+                        ((lift, edits or None, adds) if lift is not None or edits or adds else ()))
+        res = fn(args, source=source, explain=True) if explain else fn(args, source=source)
+        if perm and sorted(perm) != perm:
+            n, back = len(self._names), np.asarray(perm, dtype=np.int64)
+            for r in res:
+                if r[2] is not None:
+                    on = r[2]['node'] >= n
+                    r[2]['node'][on] = n + back[r[2]['node'][on] - n]
+        return res
 
     def rewind(self, k: int):
         """Put the device back to the state right after pod ``k`` of the last batch (restore the
@@ -863,6 +898,71 @@ class NHDScheduler:
                     result[g] = (moved, pending, why)
             todo = retry
         return result if reasons else {g: v[:2] for g, v in result.items()}
+
+    def PlanExpansion(self, additions: Sequence[Sequence], keys: Sequence = None, reasons: bool = False) -> List:
+        """Which added nodes would let the pending pods place?  ``additions``: a sequence of scenarios, each a sequence
+        of ``(node, before)``: ``node`` a Node-like object built as ``BuildInitialNodeList`` builds one (``Node(name,
+        True)``, ``ParseLabels``, ``SetHugepages``), joining ``nodes`` right before the node named ``before`` (None:
+        after the last node).  For every scenario, the pods of ``keys`` scheduled in order, as the next
+        ``CheckPendingPods`` would, on the cluster with that scenario's nodes added; all scenarios side by side in one
+        GPU call, none seeing another.  "How many copies of this shape?" is scenarios of 1..K copies.
+        Returns one ``{(ns, name): node name or None}`` per scenario, an added node named by its own name; a pod
+        beyond the solver's tuple limits (judged with the scenario's added nodes counted) maps to None.
+        ``reasons=True``: one ``(placement, reasons)`` per scenario, ``reasons[(ns, name)]`` being ``{reason name:
+        nodes}`` for each pod that finds no node, the nodes counted over the grown cluster (as ``PlanDrain`` gives them).
+        ``keys`` (``(ns, name[, uid])``) defaults to the pods the next ``CheckPendingPods`` would attempt, in its order.
+        A candidate named like an existing node or like another candidate of its scenario, an unknown ``before`` and
+        an active candidate outside the packed limits are ValueErrors.  Only reads happen, as ``PlanDrains``: each pod
+        is read from Kubernetes once; ``pod_state``, the ``Node`` objects and the counters stay as they are."""
+        scens = [[(node, before) for node, before in sc] for sc in additions]
+        for sc in scens:
+            names = [node.name for node, _ in sc]
+            clash = sorted({n for n in names if n in self.nodes or names.count(n) > 1})
+            if clash:
+                raise ValueError(f'candidate node name(s) {clash} already in use')
+            missing = sorted({b for _, b in sc if b is not None and b not in self.nodes})
+            if missing:
+                raise ValueError(f'unknown node(s) {missing}')
+        if keys is None:
+            phase = self._service_pods()
+            keys = [k for k in phase if self._wanted(phase)(k)]
+        entries = [e for e in self._read([(k[0], k[1]) for k in keys], {}) if e.solvable]
+        result = [({(k[0], k[1]): None for k in keys}, {}) for _ in scens]
+        if self.nodes and entries:
+            for sc in scens:                        # a candidate's new NIC speed: the sync below reloads the solver
+                self.cluster.pack_candidates([node for node, _ in sc])
+            self._sync()
+            now = float(self._clock())
+            todo = [(j, entries) for j in range(len(scens))]
+            while todo:
+                res = self._supported(
+                    self.cluster.plan_scenarios([((), [e.top for e in ok], [e.groups for e in ok], now,
+                                                  [e.rec for e in ok], None, None,
+                                                  [(before, node) for node, before in scens[j]]) for j, ok in todo],
+                                                explain=reasons),
+                    'plan scenarios (no plan_scenarios)')
+                added = [node.name for j, _ in todo for node, _ in scens[j]]
+                n_nodes, retry = len(self.nodes), []
+                for (j, ok), r in zip(todo, res):
+                    code, pod, out = r[:3]
+                    if out is None:
+                        # a pod beyond the tuple limits: it gets None, as in PlanDefrag, and the scenario is planned
+                        # again without it
+                        if code != wire.ERR_UNSUPPORTED:
+                            raise RuntimeError(f'nhd_plan_scenarios_grown refused scenario {j}: code {code}, pod {pod}')
+                        ok = ok[:pod] + ok[pod + 1:]
+                        if ok:
+                            retry.append((j, ok))
+                        continue
+                    placement, why = result[j]
+                    for e, b in zip(ok, out):
+                        if int(b['status']) == wire.PLACED:
+                            n = int(b['node'])
+                            placement[(e.key[0], e.key[1])] = self.cluster.name_of(n) if n < n_nodes else added[n - n_nodes]
+                    if reasons:
+                        why.update(self._reasons(ok, out, r[3]))
+                todo = retry
+        return result if reasons else [p for p, _ in result]
 
     @staticmethod
     def _defrag_scenario(g, moved, tail, edits, now, delay):

@@ -1278,8 +1278,10 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
  * the accepted scenarios are de-duplicated into one pod set and filtered once on the unchanged source records
  * (launch_solve's tables + filter, as a query), then one warp per scenario walks its pods in order
  * (scenario_plan_kernel), starting from its edited records and lifting its exclusions at its lift index.  The tuple
- * limits are judged against the whole cluster's NUMA counts and those of the edit records: the shared filter
- * enumerates the tuples of every node, the excluded ones included, and an edited node is evaluated on its own record.
+ * limits are judged against the whole cluster's NUMA counts and those of the edit and added records: the shared filter
+ * enumerates the tuples of every node, the excluded ones included, and an edited or added node is evaluated on its own
+ * record.  Added nodes (nhd_plan_scenarios_grown) live only in the working slots, after the edited ones; a binding on
+ * one names it n_nodes + its call-wide index.
  */
 /*
  * why_counts of the scenario call just run on w (its bindings b, its pods and clocks run_pods / run_now, its correction
@@ -1334,20 +1336,22 @@ static int32_t scenario_reasons(nhd_handle* h, const Workspace& w, const uint8_t
 static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, int32_t n_scenarios,
                               const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
                               const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                              const int32_t* add_start, const int32_t* add_at, const nhd_node_rec* add_rec,
                               const int32_t* pod_start, const nhd_pod* pods, const double* now, nhd_binding* out,
                               int32_t* scenario_status, int32_t* scenario_pod, uint32_t* why_counts)
 {
     if (!h || n_scenarios < 0 || !excl_start || !pod_start || (n_scenarios > 0 && (!scenario_status || !scenario_pod)))
         return NHD_ERR_INVALID;
-    if (excl_start[0] != 0 || pod_start[0] != 0 || (edit_start && edit_start[0] != 0))
+    if (excl_start[0] != 0 || pod_start[0] != 0 || (edit_start && edit_start[0] != 0) || (add_start && add_start[0] != 0))
         return fail(h, NHD_ERR_INVALID, "scenario offsets must start at 0");
     for (int s = 0; s < n_scenarios; s++)
         if (excl_start[s + 1] < excl_start[s] || pod_start[s + 1] < pod_start[s] ||
-            (edit_start && edit_start[s + 1] < edit_start[s]))
+            (edit_start && edit_start[s + 1] < edit_start[s]) || (add_start && add_start[s + 1] < add_start[s]))
             return fail(h, NHD_ERR_INVALID, "scenario %d: offsets go down", s);
     const int n_excl = excl_start[n_scenarios], n_pods = pod_start[n_scenarios];
-    const int n_edit = edit_start ? edit_start[n_scenarios] : 0;
-    if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)) || (n_edit > 0 && (!edit_node || !edit_rec)))
+    const int n_edit = edit_start ? edit_start[n_scenarios] : 0, n_add = add_start ? add_start[n_scenarios] : 0;
+    if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)) || (n_edit > 0 && (!edit_node || !edit_rec)) ||
+        (n_add > 0 && (!add_at || !add_rec)))
         return NHD_ERR_INVALID;
     const uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
@@ -1373,12 +1377,27 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         if (lift_at[s] < 0 || lift_at[s] > pod_start[s + 1] - pod_start[s])
             return fail(h, NHD_ERR_INVALID, "scenario %d: lift index %d outside [0, %d]", s, lift_at[s],
                         pod_start[s + 1] - pod_start[s]);
+    for (int s = 0; s < n_scenarios && n_add > 0; s++)
+        for (int e = add_start[s]; e < add_start[s + 1]; e++) {
+            if (add_at[e] < 0 || add_at[e] > h->n_nodes)
+                return fail(h, NHD_ERR_INVALID, "added node %d: position %d outside [0, %d]", e, add_at[e], h->n_nodes);
+            if (e > add_start[s] && add_at[e] < add_at[e - 1])
+                return fail(h, NHD_ERR_INVALID, "scenario %d: added node positions go down at %d", s, e);
+            if (nhd_validate_node(&add_rec[e]) != NHD_OK)
+                return fail(h, NHD_ERR_INVALID, "added record %d rejected by nhd_validate_node", e);
+            /* the handle holds capacities for its own speed classes only */
+            for (int k = 0; k < add_rec[e].n_nics; k++)
+                if (nic_speed_class(add_rec[e], k) >= h->params.n_speed_classes)
+                    return fail(h, NHD_ERR_INVALID, "added record %d: NIC %d has speed class %d, the handle has %d", e,
+                                k, nic_speed_class(add_rec[e], k), h->params.n_speed_classes);
+            max_numa = std::max(max_numa, (int)add_rec[e].n_numa);
+        }
 
     /* per scenario: its refusal, or its place among the accepted ones (pods, exclusions and edits compacted, the
      * exclusions sorted and each once).  idx = pod offsets | exclusion offsets | exclusions | edit offsets | edited
-     * nodes | lift indices of the accepted scenarios. */
-    std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex, ed_off{0}, ed_node, lift;
-    std::vector<nhd_node_rec> ed_rec;
+     * nodes | lift indices | add offsets | add positions of the accepted scenarios. */
+    std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex, ed_off{0}, ed_node, lift, ad_off{0}, ad_at;
+    std::vector<nhd_node_rec> ed_rec, ad_rec;
     for (int s = 0; s < n_scenarios; s++) {
         scenario_status[s] = NHD_OK;
         scenario_pod[s] = -1;
@@ -1400,8 +1419,13 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         }
         ed_off.push_back((int32_t)ed_node.size());
         lift.push_back(lift_at ? lift_at[s] : pod_start[s + 1] - pod_start[s]);
+        if (n_add > 0) {
+            ad_at.insert(ad_at.end(), add_at + add_start[s], add_at + add_start[s + 1]);
+            ad_rec.insert(ad_rec.end(), add_rec + add_start[s], add_rec + add_start[s + 1]);
+        }
+        ad_off.push_back((int32_t)ad_at.size());
     }
-    const int n_acc = (int)acc.size(), n_run = pod_off.back(), n_ed = ed_off.back();
+    const int n_acc = (int)acc.size(), n_run = pod_off.back(), n_ed = ed_off.back(), n_ad = ad_off.back();
     if (n_run == 0) return NHD_OK;
     const bool compact = n_run != n_pods;
     std::vector<nhd_pod> cpods;
@@ -1419,19 +1443,25 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         return rc;
 
     std::vector<int32_t> idx;
-    idx.reserve(pod_off.size() + ex_off.size() + ex.size() + ed_off.size() + ed_node.size() + lift.size());
-    for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift}) idx.insert(idx.end(), v->begin(), v->end());
+    idx.reserve(pod_off.size() + ex_off.size() + ex.size() + ed_off.size() + ed_node.size() + lift.size() +
+                ad_off.size() + ad_at.size());
+    for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift, &ad_off, &ad_at})
+        idx.insert(idx.end(), v->begin(), v->end());
     const size_t off_ex_off = pod_off.size(), off_ex = off_ex_off + ex_off.size(), off_ed_off = off_ex + ex.size();
     const size_t off_ed_node = off_ed_off + ed_off.size(), off_lift = off_ed_node + ed_node.size();
-    const size_t n_slots = (size_t)n_run + n_ed, off_nodes = idx.size(), off_bad = off_nodes + n_slots;
-    /* d_swork: the working slots, then the edit records the kernel seeds them from */
+    const size_t off_ad_off = off_lift + lift.size(), off_ad_at = off_ad_off + ad_off.size();
+    const size_t n_slots = (size_t)n_run + n_ed + n_ad, off_nodes = idx.size(), off_bad = off_nodes + n_slots;
+    /* d_swork: the working slots, then the edit records and the added records the kernel seeds them from */
     CK(h->d_sidx.grow((off_bad + 1) * 4));
-    CK(h->d_swork.grow((n_slots + n_ed) * sizeof(nhd_node_rec)));
+    CK(h->d_swork.grow((n_slots + n_ed + n_ad) * sizeof(nhd_node_rec)));
     CK(cudaMemcpyAsync(h->d_sidx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(h->d_sidx + off_bad, 0, 4, h->stream));
     uint4* d_edit_rec = h->d_swork + n_slots * REC_CHUNKS;
+    uint4* d_add_rec = d_edit_rec + (size_t)n_ed * REC_CHUNKS;
     if (n_ed > 0)
         CK(cudaMemcpyAsync(d_edit_rec, ed_rec.data(), (size_t)n_ed * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
+    if (n_ad > 0)
+        CK(cudaMemcpyAsync(d_add_rec, ad_rec.data(), (size_t)n_ad * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
     if (why_counts) {       /* scenario_reasons' buffers: base rows | rows, base_row | keys | corrections, node lists */
         CK(h->d_xcounts.grow((size_t)2 * n_run * NHD_WHY_COUNT * 4));
         CK(h->d_xpod.grow((size_t)n_run * (NHD_WHY_COUNT + 3) * 4));
@@ -1448,8 +1478,9 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     sa.pod_start = h->d_sidx; sa.excl_start = h->d_sidx + off_ex_off; sa.excl = h->d_sidx + off_ex;
     sa.lift = h->d_sidx + off_lift; sa.edit_start = h->d_sidx + off_ed_off; sa.edit_node = h->d_sidx + off_ed_node;
     sa.edit_rec = d_edit_rec;
+    sa.add_start = h->d_sidx + off_ad_off; sa.add_at = h->d_sidx + off_ad_at; sa.add_rec = d_add_rec;
     sa.work = h->d_swork; sa.work_node = h->d_sidx + off_nodes; sa.out = w.out; sa.bad = (uint32_t*)(h->d_sidx + off_bad);
-    sa.n_scenarios = n_acc; sa.n_types = w.n_types; sa.words = h->words;
+    sa.n_scenarios = n_acc; sa.n_types = w.n_types; sa.words = h->words; sa.n_nodes = h->n_nodes;
     sa.min_busy = h->params.min_busy_secs;
     memcpy(sa.cap, h->cap, sizeof(sa.cap));
     sa.why_delta = why_counts ? h->d_xpod + 2 * (size_t)n_run : nullptr;
@@ -1476,7 +1507,11 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     if (compact)
         for (int k = 0; k < n_acc; k++) {
             const size_t n_k = (size_t)(pod_off[k + 1] - pod_off[k]);
-            memcpy(out + pod_start[acc[k]], run.data() + pod_off[k], n_k * sizeof(nhd_binding));
+            nhd_binding* o = out + pod_start[acc[k]];
+            memcpy(o, run.data() + pod_off[k], n_k * sizeof(nhd_binding));
+            if (n_ad > 0)                          /* added nodes by their call-wide index, as the caller numbered them */
+                for (size_t i = 0; i < n_k; i++)
+                    if (o[i].node >= h->n_nodes) o[i].node += add_start[acc[k]] - ad_off[k];
             if (why_counts)
                 memcpy(why_counts + (size_t)pod_start[acc[k]] * NHD_WHY_COUNT,
                        run_rows.data() + (size_t)pod_off[k] * NHD_WHY_COUNT, n_k * NHD_WHY_COUNT * 4);
@@ -1490,7 +1525,8 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
                                       int32_t* scenario_pod)
 {
     return plan_scenarios(h, "nhd_plan_scenarios", source, n_scenarios, excl_start, excluded, nullptr, nullptr, nullptr,
-                          nullptr, pod_start, pods, now, out, scenario_status, scenario_pod, nullptr);
+                          nullptr, nullptr, nullptr, nullptr, pod_start, pods, now, out, scenario_status, scenario_pod,
+                          nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1501,8 +1537,8 @@ extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int3
                                              int32_t* scenario_pod)
 {
     return plan_scenarios(h, "nhd_plan_scenarios_edited", source, n_scenarios, excl_start, excluded, lift_at,
-                          edit_start, edit_node, edit_rec, pod_start, pods, now, out, scenario_status, scenario_pod,
-                          nullptr);
+                          edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, out,
+                          scenario_status, scenario_pod, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1514,8 +1550,22 @@ extern "C" int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, i
                                                 uint32_t* why_counts)
 {
     return plan_scenarios(h, "nhd_plan_scenarios_explained", source, n_scenarios, excl_start, excluded, lift_at,
-                          edit_start, edit_node, edit_rec, pod_start, pods, now, out, scenario_status, scenario_pod,
-                          why_counts);
+                          edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, out,
+                          scenario_status, scenario_pod, why_counts);
+}
+
+extern "C" int32_t nhd_plan_scenarios_grown(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                            const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                            const int32_t* edit_start, const int32_t* edit_node,
+                                            const nhd_node_rec* edit_rec, const int32_t* add_start,
+                                            const int32_t* add_at, const nhd_node_rec* add_rec,
+                                            const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                            nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                            uint32_t* why_counts)
+{
+    return plan_scenarios(h, "nhd_plan_scenarios_grown", source, n_scenarios, excl_start, excluded, lift_at,
+                          edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now, out,
+                          scenario_status, scenario_pod, why_counts);
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

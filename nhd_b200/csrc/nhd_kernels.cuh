@@ -2758,6 +2758,10 @@ __global__ void exclude_nodes_kernel(uint8_t* nodes, const int32_t* __restrict__
  *     passes every stage)
  * is the reference's SelectNode at that pod, "excluded" meaning in the scenario's list and i - p0 < lift[s].  One warp
  * per scenario, its pods in order.
+ * A scenario's added nodes (nhd_plan_scenarios_grown) have no source record and no bit in any bitmap: they are touched
+ * from the start, and "first" means first in the grown node order.  Source node n has the order key (n, 2^32 - 1),
+ * added node a the key (add_at[a], a), so an added node comes right before the source node it joins in front of, and
+ * added nodes at one position keep their array order.
  */
 struct ScenarioArgs {
     const uint8_t* nodes;          /* the source records (mirror or snapshot, tiled layout), only read */
@@ -2774,12 +2778,17 @@ struct ScenarioArgs {
     const int32_t* edit_start;     /* [n_scenarios + 1] into edit_node / edit_rec */
     const int32_t* edit_node;      /* each scenario's edited nodes, each once */
     const uint4* edit_rec;         /* [n_edits][8]: their records */
-    uint4* work;                   /* [n_pods + n_edits][8]: slot pod_start[s] + edit_start[s] + k = working record of
-                                      scenario s's k-th touched node; its edited nodes come first */
-    int32_t* work_node;            /* [n_pods + n_edits]: the node of each slot */
+    const int32_t* add_start;      /* [n_scenarios + 1] into add_at / add_rec */
+    const int32_t* add_at;         /* each scenario's added nodes: the source node each joins in front of (n_nodes: at
+                                      the end), never going down inside a scenario */
+    const uint4* add_rec;          /* [n_adds][8]: their records */
+    uint4* work;                   /* [n_pods + n_edits + n_adds][8]: slot pod_start[s] + edit_start[s] + add_start[s]
+                                      + k = working record of scenario s's k-th touched node; its edited nodes come
+                                      first, then its added ones */
+    int32_t* work_node;            /* [n_pods + n_edits + n_adds]: the node of each slot, n_nodes + a for added node a */
     nhd_binding* out;
     uint32_t* bad;                 /* chosen nodes on which no mapping was found: never expected, refused by the host */
-    int n_scenarios, n_types, words;
+    int n_scenarios, n_types, words, n_nodes;
     double min_busy;
     double cap[NHD_MAX_SPEED_CLASSES];
     int32_t* why_delta;            /* scenario_plan_kernel<true>: [n_pods][NHD_WHY_COUNT + 1], written for NO_CANDIDATE
@@ -2803,7 +2812,8 @@ __device__ __forceinline__ bool sorted_contains(const int32_t* v, int n, int x)
  * record, C(i) = the touched nodes (working records) and the held exclusions that are not touched (source records),
  * NHD_NODE_MAINTENANCE set on the local copy while held, each evaluated on that record and on its source record
  * (explain_node).  Lane 0 writes per reason, pass bucket last, the nodes counted on the scenario's records minus those
- * counted on the source records: the pod's row is the source records' count plus this row (DESIGN.md section 8.11). */
+ * counted on the source records: the pod's row is the source records' count plus this row (DESIGN.md section 8.11).
+ * An added node has no source record: it counts on its working record only. */
 __device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const PodType& t, uint64_t groups, double now,
                                                 const int32_t* ex, int n_ex, const uint4* work,
                                                 const int32_t* work_node, int n_touched, int32_t* row)
@@ -2820,8 +2830,9 @@ __device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const Pod
             bool counted = true;                                       /* a touched exclusion counts as touched */
             for (int j = 0; j < n_touched && k >= n_touched && counted; j++) counted = work_node[j] != node;
             if (counted) {
+                const bool added = node >= a.n_nodes;
                 RecU src, u;
-                load_rec(a.nodes, node, src);
+                if (!added) load_rec(a.nodes, node, src);
                 if (k < n_touched) {
 #pragma unroll
                     for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)k * REC_CHUNKS + c];
@@ -2829,7 +2840,7 @@ __device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const Pod
                     u = src;
                 }
                 if (sorted_contains(ex, n_ex, node)) u.r.flags |= (uint8_t)NHD_NODE_MAINTENANCE;
-                was = explain_node(src.r, t, groups, now, a.min_busy, a.cap);
+                was = added ? -1 : explain_node(src.r, t, groups, now, a.min_busy, a.cap);
                 is = explain_node(u.r, t, groups, now, a.min_busy, a.cap);
                 if (was == is) was = is = -1;
             }
@@ -2844,9 +2855,9 @@ __device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const Pod
     }
 }
 
-/* One warp per scenario (grid-stride).  The working set starts with the scenario's edited records.  For each pod: the
- * first touched node, not excluded, that passes every stage on its working record (explain_node, lanes over the touched
- * set, warp minimum) and the first untouched candidate (query_select_kernel's ballot scan, skipping excluded and touched
+/* One warp per scenario (grid-stride).  The working set starts with the scenario's edited records, then its added
+ * ones.  For each pod: the first touched node, not excluded, that passes every stage on its working record
+ * (explain_node, lanes over the touched set, warp minimum of the order key) and the first untouched candidate (query_select_kernel's ballot scan, skipping excluded and touched
  * nodes), GPU-less pass first for a pod without GPUs (Matcher.py:412-421);
  * then lane 0 runs the mapping and the assignment (query_assign_kernel's body) on that node's working record, keeps
  * the result as the node's working record and writes the binding.  WHY: at a NO_CANDIDATE pod, before any later pod
@@ -2863,12 +2874,16 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
         const int32_t* ex = a.excl + a.excl_start[s];
         const int n_ex_held = a.excl_start[s + 1] - a.excl_start[s], lift = a.lift[s];
         const int e0 = a.edit_start[s], n_edits = a.edit_start[s + 1] - e0;
-        uint4* work = a.work + (size_t)(p0 + e0) * REC_CHUNKS;
-        int32_t* work_node = a.work_node + p0 + e0;
+        const int a0 = a.add_start[s], n_adds = a.add_start[s + 1] - a0;
+        uint4* work = a.work + (size_t)(p0 + e0 + a0) * REC_CHUNKS;
+        int32_t* work_node = a.work_node + p0 + e0 + a0;
         for (int k = lane; k < n_edits * REC_CHUNKS; k += 32) work[k] = a.edit_rec[(size_t)e0 * REC_CHUNKS + k];
         for (int k = lane; k < n_edits; k += 32) work_node[k] = a.edit_node[e0 + k];
-        __syncwarp();                                                  /* the edited nodes are the first touched ones */
-        int n_touched = n_edits;
+        for (int k = lane; k < n_adds * REC_CHUNKS; k += 32)
+            work[(size_t)n_edits * REC_CHUNKS + k] = a.add_rec[(size_t)a0 * REC_CHUNKS + k];
+        for (int k = lane; k < n_adds; k += 32) work_node[n_edits + k] = a.n_nodes + a0 + k;
+        __syncwarp();                                    /* the edited nodes are the first touched ones, then the added */
+        int n_touched = n_edits + n_adds;
         for (int i = p0; i < p1; i++) {
             const int n_ex = i - p0 < lift ? n_ex_held : 0;           /* back in service from pod lift on */
             const int ti = a.pod_type[i];
@@ -2883,26 +2898,32 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
             const double now = a.now[i];
             int chosen = -1, slot = -1;
             for (int pass = t.needs_gpu ? 1 : 0; pass < 2 && chosen < 0; pass++) {
-                /* the first touched node that passes FindNode's stages on its working record */
-                int best = 0x7FFFFFFF, best_k = -1;
+                /* the first touched node, in node order, that passes FindNode's stages on its working record */
+                uint64_t best = ~0ULL;
+                int best_k = -1;
                 for (int k = lane; k < n_touched; k += 32) {
                     RecU u;
 #pragma unroll
                     for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)k * REC_CHUNKS + c];
                     const int node = work_node[k];
-                    if (node < best && (pass == 1 || u.r.n_gpus == 0) && !sorted_contains(ex, n_ex, node) &&
+                    const uint64_t key = node < a.n_nodes ? ((uint64_t)node << 32) | 0xFFFFFFFFu
+                                                          : ((uint64_t)a.add_at[node - a.n_nodes] << 32) | (uint32_t)(node - a.n_nodes);
+                    if (key < best && (pass == 1 || u.r.n_gpus == 0) && !sorted_contains(ex, n_ex, node) &&
                         explain_node(u.r, t, a.pod_groups ? gm : t.pod.group_mask, now, a.min_busy, a.cap) == NHD_WHY_COUNT) {
-                        best = node;
+                        best = key;
                         best_k = k;
                     }
                 }
                 for (int o = 16; o; o >>= 1) {
-                    const int ob = __shfl_sync(0xFFFFFFFFu, best, lane ^ o), ok = __shfl_sync(0xFFFFFFFFu, best_k, lane ^ o);
+                    const uint64_t ob = __shfl_sync(0xFFFFFFFFu, best, lane ^ o);
+                    const int ok = __shfl_sync(0xFFFFFFFFu, best_k, lane ^ o);
                     if (ob < best) { best = ob; best_k = ok; }
                 }
-                /* the first untouched candidate, only where it can come before that node */
+                /* the first untouched candidate, only where it comes before that node: untouched node n before key
+                 * (pos, sub) exactly when n < pos */
+                const long long best_pos = (long long)(best >> 32);
                 int first = -1;
-                for (int base = 0; base < W && first < 0 && (long long)base * 64 < best; base += 32) {
+                for (int base = 0; base < W && first < 0 && (long long)base * 64 < best_pos; base += 32) {
                     const int w = base + lane;
                     int mine = -1;
                     if (w < W) {
@@ -2915,7 +2936,7 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
                         }
                         for (; word; word &= word - 1) {
                             const int node = w * 64 + ctz64(word);
-                            if (node >= best) break;
+                            if (node >= best_pos) break;
                             if (sorted_contains(ex, n_ex, node)) continue;
                             bool touched = false;
                             for (int k = 0; k < n_touched && !touched; k++) touched = work_node[k] == node;
@@ -2933,7 +2954,11 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
                     if (m) first = __shfl_sync(0xFFFFFFFFu, mine, ctz32(m));
                 }
                 if (first >= 0) { chosen = first; slot = n_touched; }
-                else if (best_k >= 0) { chosen = best; slot = best_k; }
+                else if (best_k >= 0) {
+                    const uint32_t sub = (uint32_t)best;
+                    chosen = sub == 0xFFFFFFFFu ? (int)best_pos : a.n_nodes + (int)sub;
+                    slot = best_k;
+                }
             }
             if (lane == 0) {
                 union { nhd_binding b; uint4 q[8]; } bu;

@@ -237,15 +237,20 @@ class Solver:
         ``lift`` (None: never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits``
         (None: none): ``(nodes, records)``, node indices and a ``wire.NODE_DTYPE`` array, the records those nodes have
         for the whole scenario.  With either, the bindings are those of ``solve_batch`` on a scratch copy of the records
-        with the edits applied, the excluded nodes in maintenance for the pods before ``lift`` and back after."""
+        with the edits applied, the excluded nodes in maintenance for the pods before ``lift`` and back after.
+        ``adds`` (sixth element, None: none): ``(at, records)``, int positions and a ``wire.NODE_DTYPE`` array: nodes
+        added for the whole scenario, each right before source node ``at[k]`` (``n_nodes``: at the end), ``at`` never
+        going down (``nhd_plan_scenarios_grown``).  A pod placed on one gets node ``n_nodes + a``, ``a`` its index among
+        the added records of the whole call, in scenario order."""
         src = _source(source)
         # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
         # would cost more than the call itself)
-        exs, podb, nowl, lifts, ednodes, edrecs = [], [], [], [], [], []
+        exs, podb, nowl, lifts, ednodes, edrecs, n_adds, adats, adrecs = [], [], [], [], [], [], [], [], []
         for sc in scenarios:
             exclude, pods, now = sc[:3]
             lift = sc[3] if len(sc) > 3 else None
             edits = sc[4] if len(sc) > 4 else None
+            adds = sc[5] if len(sc) > 5 else None
             pods = np.asarray(pods)
             if pods.dtype != wire.POD_DTYPE:
                 pods = pods.astype(wire.POD_DTYPE)
@@ -262,6 +267,15 @@ class Solver:
                 recs = np.asarray(recs, dtype=wire.NODE_DTYPE).reshape(-1)
                 assert len(recs) == len(ednodes[-1])
                 edrecs.append(recs.tobytes())
+            if adds is None:
+                n_adds.append(0)
+            else:
+                at, recs = adds
+                adats.append(np.asarray(at, dtype='<i4').reshape(-1))
+                recs = np.asarray(recs, dtype=wire.NODE_DTYPE).reshape(-1)
+                assert len(recs) == len(adats[-1])
+                adrecs.append(recs.tobytes())
+                n_adds.append(len(recs))
         n = len(podb)
         excl_start = np.zeros(n + 1, dtype='<i4')
         pod_start = np.zeros(n + 1, dtype='<i4')
@@ -278,18 +292,36 @@ class Solver:
         out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
         status = np.zeros(n, dtype='<i4')
         which = np.zeros(n, dtype='<i4')
-        args = (self._h, src, n, excl_start.ctypes.data, ex.ctypes.data if len(ex) else None,
+        head = (self._h, src, n, excl_start.ctypes.data, ex.ctypes.data if len(ex) else None,
                 lift.ctypes.data if n else None, edit_start.ctypes.data, ednode.ctypes.data if len(ednode) else None,
-                edrec.ctypes.data if len(edrec) else None, pod_start.ctypes.data,
-                pods.ctypes.data if len(pods) else None, now.ctypes.data if len(pods) else None,
+                edrec.ctypes.data if len(edrec) else None)
+        tail = (pod_start.ctypes.data, pods.ctypes.data if len(pods) else None, now.ctypes.data if len(pods) else None,
                 out.ctypes.data if len(pods) else None, status.ctypes.data, which.ctypes.data)
+        if any(n_adds):
+            add_start = np.zeros(n + 1, dtype='<i4')
+            add_start[1:] = np.cumsum(n_adds)
+            adat = np.ascontiguousarray(np.concatenate(adats), dtype='<i4')
+            adrec = np.frombuffer(b''.join(adrecs), dtype=wire.NODE_DTYPE)
+            counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
+            self._ck(self._L.nhd_plan_scenarios_grown(*head, add_start.ctypes.data, adat.ctypes.data,
+                                                      adrec.ctypes.data, *tail,
+                                                      counts.ctypes.data if explain and len(pods) else None))
+            return self._scenario_results(status, which, pod_start, out, counts)
+        args = head + tail
         if not explain:
             self._ck(self._L.nhd_plan_scenarios_edited(*args))
+            return self._scenario_results(status, which, pod_start, out, None)
+        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4')
+        self._ck(self._L.nhd_plan_scenarios_explained(*args, counts.ctypes.data if len(pods) else None))
+        return self._scenario_results(status, which, pod_start, out, counts)
+
+    @staticmethod
+    def _scenario_results(status, which, pod_start, out, counts):
+        """``plan_scenarios``' per-scenario tuples: ``(code, pod, bindings[, counts])``."""
+        if counts is None:
             return [(code, pod, out[a:b] if code == 0 else None)
                     for code, pod, a, b in zip(status.tolist(), which.tolist(), pod_start[:-1].tolist(),
                                                pod_start[1:].tolist())]
-        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4')
-        self._ck(self._L.nhd_plan_scenarios_explained(*args, counts.ctypes.data if len(pods) else None))
         return [(code, pod, out[a:b], counts[a:b]) if code == 0 else (code, pod, None, None)
                 for code, pod, a, b in zip(status.tolist(), which.tolist(), pod_start[:-1].tolist(), pod_start[1:].tolist())]
 
