@@ -424,6 +424,39 @@ int32_t nhd_plan_scenarios_grown(nhd_handle* h, int32_t source, int32_t n_scenar
                                  nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
                                  uint32_t* why_counts);
 
+/*
+ * nhd_plan_scenarios_grown over several pending scans: "which pods get in at a later scan, and which never do?".  The
+ * scheduler retries every pod still pending at each scan, and a GPU node that took a pod (or failed an assignment) less
+ * than min_busy_secs earlier takes no GPU pod, so one scan cannot tell "never fits" from "fits at the next scan".
+ * Scenario s has R_s = round_start[s+1] - round_start[s] later rounds; round r >= 1 runs at clock
+ * round_clock[round_start[s] + r - 1].  After the five steps of nhd_plan_scenarios_grown (round 0), for r = 1 .. R_s
+ * the pods of s whose latest binding is not NHD_PLACED are solved in scenario order as one nhd_solve_batch at that
+ * round's clock, on the records the previous round left; a round with no such pod does nothing.
+ *   - exclusions still held for the last pod of round 0 (lift_at NULL or lift_at[s] == n_s) stay held in every later
+ *     round; exclusions lifted during round 0 stay lifted; edits and added nodes hold for the whole scenario;
+ *   out            byte for byte each pod's last attempt, node indices mapped back as for nhd_plan_scenarios_grown;
+ *   pod_round      (may be NULL) pod_start[n_scenarios] entries: the round that placed the pod, or R_s if none did;
+ *   why_counts     (may be NULL) for a pod whose last attempt is NHD_NO_CANDIDATE, the row nhd_explain_batch would give
+ *                  at the start of that attempt, at that round's clock, over the scenario's grown node list; other rows
+ *                  zero.
+ * Besides nhd_plan_scenarios_grown's malformed arguments, the whole call is NHD_ERR_INVALID for round offsets that do
+ * not start at 0 or go down, a non-finite round clock, round clocks that go down inside a scenario, and a round clock
+ * earlier than a now[] of its scenario (a monotonic clock never goes back).  The busy test is now - busy_time <
+ * min_busy_secs in fp64: give the clocks exactly as the caller's clock would read them, each the previous one plus the
+ * period, not t0 + r * period.  round_start == NULL means no rounds (round_clock is not read): the call is
+ * nhd_plan_scenarios_grown and pod_round, if given, is all zero.  Refusals per scenario, tuple limits, side effects
+ * (none observable), collectives and waiting as for nhd_plan_scenarios_grown.  Each scenario's pods may touch up to
+ * min(n_s * (1 + R_s), n_nodes) nodes besides its edited and added ones: device scratch grows with that bound.
+ */
+int32_t nhd_plan_scenarios_rounds(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                  const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                  const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                                  const int32_t* add_start, const int32_t* add_at, const nhd_node_rec* add_rec,
+                                  const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                  const int32_t* round_start, const double* round_clock,
+                                  nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                  uint32_t* why_counts, int32_t* pod_round);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

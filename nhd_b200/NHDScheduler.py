@@ -266,6 +266,9 @@ class DeviceCluster:
         scenario.  ``adds`` (eighth element, None: none): ``[(before, node)]``, Node-like objects in service for the
         whole scenario, each joining the node order right before the node named ``before`` (None: after the last
         node), packed by ``pack_candidates`` before any pod (a pod may request a group name only a candidate carries).
+        ``rounds`` (ninth element, None: none): the clocks of later pending scans, at which the scenario's pods not
+        placed yet are retried (``Solver.plan_scenarios``); with any, each result gains the per-pod round that placed
+        the pod.
         Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
         when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods; ``explain=True``: one
         ``(code, pod, bindings, counts)``, ``counts`` the per-reason node counts of the NO_CANDIDATE pods.  A pod
@@ -290,13 +293,15 @@ class DeviceCluster:
             if edits:
                 edits = (self._indices(edits, 'edit'), self._pack(list(edits.values())))
             adds = None
+            rounds = sc[8] if len(sc) > 8 else None
             if recs is not None:
                 at = np.asarray([len(self._names) if b is None else self._index[b] for b, _ in sc[7]], dtype='<i4')
                 order = np.argsort(at, kind='stable')
                 adds = (at[order], recs[order])
                 perm.extend((len(perm) + order).tolist())
             args.append((idx, self._pods(tops, pod_groups, packed), self._clocks(len(tops), now)) +
-                        ((lift, edits or None, adds) if lift is not None or edits or adds else ()))
+                        ((lift, edits or None, adds, rounds)
+                         if lift is not None or edits or adds or rounds is not None else ()))
         res = fn(args, source=source, explain=True) if explain else fn(args, source=source)
         if perm and sorted(perm) != perm:
             n, back = len(self._names), np.asarray(perm, dtype=np.int64)
@@ -914,6 +919,38 @@ class NHDScheduler:
         A candidate named like an existing node or like another candidate of its scenario, an unknown ``before`` and
         an active candidate outside the packed limits are ValueErrors.  Only reads happen, as ``PlanDrains``: each pod
         is read from Kubernetes once; ``pod_state``, the ``Node`` objects and the counters stay as they are."""
+        result = self._grown_plans(additions, keys, reasons, None)
+        return result if reasons else [p for p, _ in result]
+
+    def ForecastPending(self, scans: int, keys: Sequence = None, period: float = None, additions: Sequence = None,
+                        reasons: bool = False):
+        """Which pending pods get in at a later scan, and which never do?  ``run()`` retries every pod still pending
+        each ``idle_thresh x block_secs`` seconds, and a GPU node that took a pod less than ``MIN_BUSY_SECS`` earlier
+        takes no GPU pod, so one scan places at most one GPU pod per node.  This plans ``scans`` pending scans in a row
+        without placing anything: scan 0 at the current clock, each later scan ``period`` seconds after the one before
+        (the clock advanced step by step, as the scheduler's clock advances), each retrying in order the pods of
+        ``keys`` that no earlier scan placed, on the cluster the earlier scans left.  ``period`` defaults to ``run()``'s
+        ``idle_thresh x block_secs`` (30 s); ``keys`` (``(ns, name[, uid])``) to the pods the next ``CheckPendingPods``
+        would attempt, in its order.
+        ``additions`` None: the cluster as it is, and the result is ``{(ns, name): (scan, node name) or None}``.  Else a
+        sequence of scenarios as ``PlanExpansion`` takes them, all side by side in one GPU call, and the result is one
+        such dict per scenario, an added node named by its own name.  None: no scan placed the pod (a pod beyond the
+        solver's tuple limits included).  ``reasons=True``: ``(placement, reasons)``, ``reasons[(ns, name)]`` being
+        ``{reason name: nodes}`` for each pod no scan placed that found no node at its last scan, at that scan's state.
+        Names and reads as ``PlanExpansion``: only reads happen; ``pod_state``, the ``Node`` objects and the counters
+        stay as they are."""
+        scans = int(scans)
+        if scans < 1:
+            raise ValueError(f'scans must be at least 1, not {scans}')
+        period = float(60 * 0.5 if period is None else period)     # run()'s idle_thresh x block_secs
+        result = self._grown_plans([[]] if additions is None else additions, keys, reasons, [period] * (scans - 1))
+        out = [(p, why) if reasons else p for p, why in result]
+        return out[0] if additions is None else out
+
+    def _grown_plans(self, additions: Sequence[Sequence], keys: Sequence, reasons: bool, periods: Sequence[float]):
+        """``PlanExpansion``'s plans, with a later scan after each of ``periods`` seconds: per scenario ``(placement,
+        reasons)``, a placed pod mapped to its node name, or with ``periods`` (even an empty list) to ``(scan, node
+        name)``.  ``periods`` None: one scan, through the call without rounds."""
         scens = [[(node, before) for node, before in sc] for sc in additions]
         for sc in scens:
             names = [node.name for node, _ in sc]
@@ -933,12 +970,19 @@ class NHDScheduler:
                 self.cluster.pack_candidates([node for node, _ in sc])
             self._sync()
             now = float(self._clock())
+            clocks = None
+            if periods is not None:                 # each scan's clock from the one before, as the clock advances
+                clocks = [now]
+                for p in periods:
+                    clocks.append(clocks[-1] + float(p))
+                clocks = clocks[1:]
             todo = [(j, entries) for j in range(len(scens))]
             while todo:
                 res = self._supported(
                     self.cluster.plan_scenarios([((), [e.top for e in ok], [e.groups for e in ok], now,
                                                   [e.rec for e in ok], None, None,
-                                                  [(before, node) for node, before in scens[j]]) for j, ok in todo],
+                                                  [(before, node) for node, before in scens[j]])
+                                                 + ((clocks,) if clocks is not None else ()) for j, ok in todo],
                                                 explain=reasons),
                     'plan scenarios (no plan_scenarios)')
                 added = [node.name for j, _ in todo for node, _ in scens[j]]
@@ -955,14 +999,15 @@ class NHDScheduler:
                             retry.append((j, ok))
                         continue
                     placement, why = result[j]
-                    for e, b in zip(ok, out):
+                    for k, (e, b) in enumerate(zip(ok, out)):
                         if int(b['status']) == wire.PLACED:
                             n = int(b['node'])
-                            placement[(e.key[0], e.key[1])] = self.cluster.name_of(n) if n < n_nodes else added[n - n_nodes]
+                            name = self.cluster.name_of(n) if n < n_nodes else added[n - n_nodes]
+                            placement[(e.key[0], e.key[1])] = name if clocks is None else (int(r[-1][k]), name)
                     if reasons:
                         why.update(self._reasons(ok, out, r[3]))
                 todo = retry
-        return result if reasons else [p for p, _ in result]
+        return result
 
     @staticmethod
     def _defrag_scenario(g, moved, tail, edits, now, delay):

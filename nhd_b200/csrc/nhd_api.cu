@@ -1085,14 +1085,15 @@ static int32_t explain_prepare(nhd_handle* h, const Workspace& w, int* n_failed)
     return NHD_OK;
 }
 
-/* one (failed pod x node) pass over w's solve, which started from the records nodes; counts and/or reasons may be null */
+/* one (failed pod x node) pass over w's solve, which started from the records nodes; counts and/or reasons may be null;
+ * d_now (device, per pod) replaces the staged clocks when given */
 static int32_t explain_launch(nhd_handle* h, const Workspace& w, const uint8_t* nodes, int n_failed, uint32_t* d_counts,
-                              uint8_t* d_reasons)
+                              uint8_t* d_reasons, const double* d_now = nullptr)
 {
     const int N = h->n_nodes, P = w.n_pods;
     if (n_failed == 0 || N == 0) return NHD_OK;
     ExplainArgs xa;
-    xa.snapshot = nodes; xa.types = w.types; xa.pod_type = w.pod_type(); xa.now = w.now(); xa.out = w.out;
+    xa.snapshot = nodes; xa.types = w.types; xa.pod_type = w.pod_type(); xa.now = d_now ? d_now : w.now(); xa.out = w.out;
     xa.pod_groups = w.pod_groups();
     xa.node_start = h->d_xnode + N; xa.node_pods = h->d_xpod; xa.failed = h->d_xpod + P;
     xa.n_failed = (const int32_t*)h->d_xsmall.p;
@@ -1281,18 +1282,22 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
  * limits are judged against the whole cluster's NUMA counts and those of the edit and added records: the shared filter
  * enumerates the tuples of every node, the excluded ones included, and an edited or added node is evaluated on its own
  * record.  Added nodes (nhd_plan_scenarios_grown) live only in the working slots, after the edited ones; a binding on
- * one names it n_nodes + its call-wide index.
+ * one names it n_nodes + its call-wide index.  With rounds (nhd_plan_scenarios_rounds) the same warp walks the
+ * scenario's unplaced pods again at each round clock (scenario_plan_kernel<., true>); scenario s's slots then start at
+ * slot_start[s] and hold n_edits + n_adds + min(n_s * (1 + R_s), n_nodes) records, and the reasons' base pass reads
+ * each pod's clock of its last attempt instead of the staged clocks.
  */
 /*
  * why_counts of the scenario call just run on w (its bindings b, its pods and clocks run_pods / run_now, its correction
- * rows in d_xpod + 2 * n_run): the NO_CANDIDATE pods' keys (pod type, clock, node-group mask) de-duplicated, one
+ * rows in d_xpod + 2 * n_run; with rounds, run_now and its device copy d_now are the clocks of each pod's last attempt,
+ * else d_now is null and the staged clocks serve): the NO_CANDIDATE pods' keys (pod type, clock, node-group mask) de-duplicated, one
  * explain_kernel pass per key over the source records with no bindings (empty per-node lists), then
  * scenario_why_combine_kernel adds each pod's correction to its key's row.  rows: n_run * NHD_WHY_COUNT host entries.
  * Buffers were sized before the scenario kernel; one host wait.
  */
 static int32_t scenario_reasons(nhd_handle* h, const Workspace& w, const uint8_t* records, int n_run,
-                                const nhd_pod* run_pods, const double* run_now, const nhd_binding* b, uint32_t* rows,
-                                const char* what)
+                                const nhd_pod* run_pods, const double* run_now, const double* d_now,
+                                const nhd_binding* b, uint32_t* rows, const char* what)
 {
     const int N = h->n_nodes;
     std::vector<int32_t> idx(2 * (size_t)n_run, -1);              /* base_row | key representatives */
@@ -1319,7 +1324,7 @@ static int32_t scenario_reasons(nhd_handle* h, const Workspace& w, const uint8_t
     CK(cudaMemsetAsync(base, 0, (size_t)n_run * NHD_WHY_COUNT * 4, h->stream));
     /* the key's row on the source records: the representative pod with nothing bound before it; nodes that pass
      * every stage land in survivors, which is not read (pass bucket = n_nodes - row sum) */
-    int32_t rc = explain_launch(h, w, records, n_keys, base, nullptr);
+    int32_t rc = explain_launch(h, w, records, n_keys, base, nullptr, d_now);
     if (rc != NHD_OK) return rc;
     scenario_why_combine_kernel<<<(unsigned)((n_run + 255) / 256), 256, 0, h->stream>>>(
         base, h->d_xpod, h->d_xpod + 2 * (size_t)n_run, n_run, N, d_rows, h->d_xsmall + 2);
@@ -1337,22 +1342,39 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
                               const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
                               const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
                               const int32_t* add_start, const int32_t* add_at, const nhd_node_rec* add_rec,
-                              const int32_t* pod_start, const nhd_pod* pods, const double* now, nhd_binding* out,
-                              int32_t* scenario_status, int32_t* scenario_pod, uint32_t* why_counts)
+                              const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                              const int32_t* round_start, const double* round_clock, nhd_binding* out,
+                              int32_t* scenario_status, int32_t* scenario_pod, uint32_t* why_counts, int32_t* pod_round)
 {
     if (!h || n_scenarios < 0 || !excl_start || !pod_start || (n_scenarios > 0 && (!scenario_status || !scenario_pod)))
         return NHD_ERR_INVALID;
-    if (excl_start[0] != 0 || pod_start[0] != 0 || (edit_start && edit_start[0] != 0) || (add_start && add_start[0] != 0))
+    if (excl_start[0] != 0 || pod_start[0] != 0 || (edit_start && edit_start[0] != 0) || (add_start && add_start[0] != 0) ||
+        (round_start && round_start[0] != 0))
         return fail(h, NHD_ERR_INVALID, "scenario offsets must start at 0");
     for (int s = 0; s < n_scenarios; s++)
         if (excl_start[s + 1] < excl_start[s] || pod_start[s + 1] < pod_start[s] ||
-            (edit_start && edit_start[s + 1] < edit_start[s]) || (add_start && add_start[s + 1] < add_start[s]))
+            (edit_start && edit_start[s + 1] < edit_start[s]) || (add_start && add_start[s + 1] < add_start[s]) ||
+            (round_start && round_start[s + 1] < round_start[s]))
             return fail(h, NHD_ERR_INVALID, "scenario %d: offsets go down", s);
     const int n_excl = excl_start[n_scenarios], n_pods = pod_start[n_scenarios];
     const int n_edit = edit_start ? edit_start[n_scenarios] : 0, n_add = add_start ? add_start[n_scenarios] : 0;
+    const int n_round = round_start ? round_start[n_scenarios] : 0;
     if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)) || (n_edit > 0 && (!edit_node || !edit_rec)) ||
-        (n_add > 0 && (!add_at || !add_rec)))
+        (n_add > 0 && (!add_at || !add_rec)) || (n_round > 0 && !round_clock))
         return NHD_ERR_INVALID;
+    for (int s = 0; s < n_scenarios && n_round > 0; s++)
+        for (int r = round_start[s]; r < round_start[s + 1]; r++) {
+            if (!std::isfinite(round_clock[r]))
+                return fail(h, NHD_ERR_INVALID, "scenario %d: round clock %d is not finite", s, r);
+            if (r > round_start[s] && round_clock[r] < round_clock[r - 1])
+                return fail(h, NHD_ERR_INVALID, "scenario %d: round clocks go down at %d", s, r);
+            if (r == round_start[s])                     /* a monotonic clock never goes back */
+                for (int i = pod_start[s]; i < pod_start[s + 1]; i++)
+                    if (round_clock[r] < now[i])
+                        return fail(h, NHD_ERR_INVALID, "scenario %d: round clock %d is earlier than the clock of pod %d",
+                                    s, r, i - pod_start[s]);
+        }
+    if (pod_round && !round_start && n_pods > 0) memset(pod_round, 0, (size_t)n_pods * 4);
     const uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
     if (rc != NHD_OK) return rc;
@@ -1395,9 +1417,12 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
 
     /* per scenario: its refusal, or its place among the accepted ones (pods, exclusions and edits compacted, the
      * exclusions sorted and each once).  idx = pod offsets | exclusion offsets | exclusions | edit offsets | edited
-     * nodes | lift indices | add offsets | add positions of the accepted scenarios. */
-    std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex, ed_off{0}, ed_node, lift, ad_off{0}, ad_at;
+     * nodes | lift indices | add offsets | add positions of the accepted scenarios, and with rounds | round offsets |
+     * first working slots. */
+    std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex, ed_off{0}, ed_node, lift, ad_off{0}, ad_at, rd_off{0}, sl_start;
     std::vector<nhd_node_rec> ed_rec, ad_rec;
+    std::vector<double> rd_clock;
+    size_t n_slots = 0;
     for (int s = 0; s < n_scenarios; s++) {
         scenario_status[s] = NHD_OK;
         scenario_pod[s] = -1;
@@ -1424,7 +1449,18 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
             ad_rec.insert(ad_rec.end(), add_rec + add_start[s], add_rec + add_start[s + 1]);
         }
         ad_off.push_back((int32_t)ad_at.size());
+        const int64_t n_s = pod_start[s + 1] - pod_start[s];
+        int64_t touches = n_s;                 /* without rounds: one slot per pod, as scenario_plan_kernel<., false> */
+        if (round_start) {
+            rd_clock.insert(rd_clock.end(), round_clock + round_start[s], round_clock + round_start[s + 1]);
+            rd_off.push_back((int32_t)rd_clock.size());
+            sl_start.push_back((int32_t)n_slots);
+            touches = std::min(n_s * (1 + (int64_t)(round_start[s + 1] - round_start[s])), (int64_t)h->n_nodes);
+        }
+        n_slots += (size_t)(touches + (edit_start ? edit_start[s + 1] - edit_start[s] : 0) +
+                            (add_start ? add_start[s + 1] - add_start[s] : 0));
     }
+    if (n_slots > (size_t)INT32_MAX) return fail(h, NHD_ERR_INVALID, "%zu working slots exceed the int32 range", n_slots);
     const int n_acc = (int)acc.size(), n_run = pod_off.back(), n_ed = ed_off.back(), n_ad = ad_off.back();
     if (n_run == 0) return NHD_OK;
     const bool compact = n_run != n_pods;
@@ -1444,24 +1480,32 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
 
     std::vector<int32_t> idx;
     idx.reserve(pod_off.size() + ex_off.size() + ex.size() + ed_off.size() + ed_node.size() + lift.size() +
-                ad_off.size() + ad_at.size());
-    for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift, &ad_off, &ad_at})
+                ad_off.size() + ad_at.size() + rd_off.size() + sl_start.size());
+    for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift, &ad_off, &ad_at, &rd_off, &sl_start})
         idx.insert(idx.end(), v->begin(), v->end());
     const size_t off_ex_off = pod_off.size(), off_ex = off_ex_off + ex_off.size(), off_ed_off = off_ex + ex.size();
     const size_t off_ed_node = off_ed_off + ed_off.size(), off_lift = off_ed_node + ed_node.size();
     const size_t off_ad_off = off_lift + lift.size(), off_ad_at = off_ad_off + ad_off.size();
-    const size_t n_slots = (size_t)n_run + n_ed + n_ad, off_nodes = idx.size(), off_bad = off_nodes + n_slots;
-    /* d_swork: the working slots, then the edit records and the added records the kernel seeds them from */
-    CK(h->d_sidx.grow((off_bad + 1) * 4));
-    CK(h->d_swork.grow((n_slots + n_ed + n_ad) * sizeof(nhd_node_rec)));
+    const size_t off_rd_off = off_ad_at + ad_at.size(), off_sl = off_rd_off + rd_off.size();
+    const size_t off_nodes = idx.size(), off_bad = off_nodes + n_slots, off_round = off_bad + 1;
+    const bool rounds = round_start != nullptr;
+    /* d_swork: the working slots, then the edit records and the added records the kernel seeds them from, then (with
+     * rounds) the round clocks and the clocks of each pod's last attempt (reasons' base pass), 16-byte chunks */
+    const size_t rd_chunks = rounds ? (rd_clock.size() + 1) / 2 : 0, last_chunks = rounds && why_counts ? ((size_t)n_run + 1) / 2 : 0;
+    CK(h->d_sidx.grow((off_round + (rounds ? n_run : 0)) * 4));
+    CK(h->d_swork.grow((n_slots + n_ed + n_ad) * sizeof(nhd_node_rec) + (rd_chunks + last_chunks) * 16));
     CK(cudaMemcpyAsync(h->d_sidx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(h->d_sidx + off_bad, 0, 4, h->stream));
     uint4* d_edit_rec = h->d_swork + n_slots * REC_CHUNKS;
     uint4* d_add_rec = d_edit_rec + (size_t)n_ed * REC_CHUNKS;
+    double* d_round_clock = reinterpret_cast<double*>(d_add_rec + (size_t)n_ad * REC_CHUNKS);
+    double* d_last_now = d_round_clock + 2 * rd_chunks;
     if (n_ed > 0)
         CK(cudaMemcpyAsync(d_edit_rec, ed_rec.data(), (size_t)n_ed * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
     if (n_ad > 0)
         CK(cudaMemcpyAsync(d_add_rec, ad_rec.data(), (size_t)n_ad * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
+    if (!rd_clock.empty())
+        CK(cudaMemcpyAsync(d_round_clock, rd_clock.data(), rd_clock.size() * 8, cudaMemcpyHostToDevice, h->stream));
     if (why_counts) {       /* scenario_reasons' buffers: base rows | rows, base_row | keys | corrections, node lists */
         CK(h->d_xcounts.grow((size_t)2 * n_run * NHD_WHY_COUNT * 4));
         CK(h->d_xpod.grow((size_t)n_run * (NHD_WHY_COUNT + 3) * 4));
@@ -1484,15 +1528,23 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     sa.min_busy = h->params.min_busy_secs;
     memcpy(sa.cap, h->cap, sizeof(sa.cap));
     sa.why_delta = why_counts ? h->d_xpod + 2 * (size_t)n_run : nullptr;
+    sa.round_start = h->d_sidx + off_rd_off; sa.round_clock = d_round_clock; sa.slot_start = h->d_sidx + off_sl;
+    sa.pod_round = h->d_sidx + off_round;
     const int warps_per_cta = SCENARIO_THREADS / 32;
     const int grid = std::min((n_acc + warps_per_cta - 1) / warps_per_cta, h->sm_count * 16);
-    if (why_counts)
-        scenario_plan_kernel<true><<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
-    else
-        scenario_plan_kernel<false><<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
+    /* through a pointer: the CPU emulation (tests/emu) rewrites a launch into a macro call, whose argument list would
+     * split a kernel name with two template arguments */
+    void (*const kernel)(ScenarioArgs) = rounds ? (why_counts ? scenario_plan_kernel<true, true> : scenario_plan_kernel<false, true>)
+                                                : (why_counts ? scenario_plan_kernel<true, false> : scenario_plan_kernel<false, false>);
+    kernel<<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
     CK(cudaGetLastError());
     uint32_t bad = 0;
     CK(cudaMemcpyAsync(&bad, h->d_sidx + off_bad, 4, cudaMemcpyDeviceToHost, h->stream));
+    std::vector<int32_t> run_round;
+    if (rounds) {
+        run_round.resize(n_run);
+        CK(cudaMemcpyAsync(run_round.data(), h->d_sidx + off_round, (size_t)n_run * 4, cudaMemcpyDeviceToHost, h->stream));
+    }
     std::vector<nhd_binding> run;
     if (compact) run.resize(n_run);
     if ((rc = fetch_bindings(h, w, n_run, compact ? run.data() : out)) != NHD_OK) return rc;
@@ -1500,10 +1552,22 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     std::vector<uint32_t> run_rows;
     if (why_counts) {
         if (compact) run_rows.resize((size_t)n_run * NHD_WHY_COUNT);
-        if ((rc = scenario_reasons(h, w, records, n_run, compact ? cpods.data() : pods, compact ? cnow.data() : now,
-                                   compact ? run.data() : out, compact ? run_rows.data() : why_counts, what)) != NHD_OK)
+        const double* run_now = compact ? cnow.data() : now;
+        std::vector<double> last_now;
+        if (rounds) {            /* the base pass evaluates each pod at the clock of its last attempt */
+            last_now.resize(n_run);
+            for (int k = 0; k < n_acc; k++)
+                for (int i = pod_off[k]; i < pod_off[k + 1]; i++)
+                    last_now[i] = run_round[i] == 0 ? run_now[i] : rd_clock[rd_off[k] + run_round[i] - 1];
+            CK(cudaMemcpyAsync(d_last_now, last_now.data(), (size_t)n_run * 8, cudaMemcpyHostToDevice, h->stream));
+            run_now = last_now.data();
+        }
+        if ((rc = scenario_reasons(h, w, records, n_run, compact ? cpods.data() : pods, run_now,
+                                   rounds ? d_last_now : nullptr, compact ? run.data() : out,
+                                   compact ? run_rows.data() : why_counts, what)) != NHD_OK)
             return rc;
     }
+    if (rounds && !compact && pod_round) memcpy(pod_round, run_round.data(), (size_t)n_run * 4);
     if (compact)
         for (int k = 0; k < n_acc; k++) {
             const size_t n_k = (size_t)(pod_off[k + 1] - pod_off[k]);
@@ -1515,6 +1579,7 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
             if (why_counts)
                 memcpy(why_counts + (size_t)pod_start[acc[k]] * NHD_WHY_COUNT,
                        run_rows.data() + (size_t)pod_off[k] * NHD_WHY_COUNT, n_k * NHD_WHY_COUNT * 4);
+            if (rounds && pod_round) memcpy(pod_round + pod_start[acc[k]], run_round.data() + pod_off[k], n_k * 4);
         }
     return NHD_OK;
 }
@@ -1525,8 +1590,8 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
                                       int32_t* scenario_pod)
 {
     return plan_scenarios(h, "nhd_plan_scenarios", source, n_scenarios, excl_start, excluded, nullptr, nullptr, nullptr,
-                          nullptr, nullptr, nullptr, nullptr, pod_start, pods, now, out, scenario_status, scenario_pod,
-                          nullptr);
+                          nullptr, nullptr, nullptr, nullptr, pod_start, pods, now, nullptr, nullptr, out,
+                          scenario_status, scenario_pod, nullptr, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1537,8 +1602,8 @@ extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int3
                                              int32_t* scenario_pod)
 {
     return plan_scenarios(h, "nhd_plan_scenarios_edited", source, n_scenarios, excl_start, excluded, lift_at,
-                          edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, out,
-                          scenario_status, scenario_pod, nullptr);
+                          edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, nullptr,
+                          nullptr, out, scenario_status, scenario_pod, nullptr, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1550,8 +1615,8 @@ extern "C" int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, i
                                                 uint32_t* why_counts)
 {
     return plan_scenarios(h, "nhd_plan_scenarios_explained", source, n_scenarios, excl_start, excluded, lift_at,
-                          edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, out,
-                          scenario_status, scenario_pod, why_counts);
+                          edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, nullptr,
+                          nullptr, out, scenario_status, scenario_pod, why_counts, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_grown(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1564,8 +1629,23 @@ extern "C" int32_t nhd_plan_scenarios_grown(nhd_handle* h, int32_t source, int32
                                             uint32_t* why_counts)
 {
     return plan_scenarios(h, "nhd_plan_scenarios_grown", source, n_scenarios, excl_start, excluded, lift_at,
-                          edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now, out,
-                          scenario_status, scenario_pod, why_counts);
+                          edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now, nullptr,
+                          nullptr, out, scenario_status, scenario_pod, why_counts, nullptr);
+}
+
+extern "C" int32_t nhd_plan_scenarios_rounds(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                             const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                             const int32_t* edit_start, const int32_t* edit_node,
+                                             const nhd_node_rec* edit_rec, const int32_t* add_start,
+                                             const int32_t* add_at, const nhd_node_rec* add_rec,
+                                             const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                             const int32_t* round_start, const double* round_clock, nhd_binding* out,
+                                             int32_t* scenario_status, int32_t* scenario_pod, uint32_t* why_counts,
+                                             int32_t* pod_round)
+{
+    return plan_scenarios(h, "nhd_plan_scenarios_rounds", source, n_scenarios, excl_start, excluded, lift_at,
+                          edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now,
+                          round_start, round_clock, out, scenario_status, scenario_pod, why_counts, pod_round);
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

@@ -2794,6 +2794,11 @@ struct ScenarioArgs {
     int32_t* why_delta;            /* scenario_plan_kernel<true>: [n_pods][NHD_WHY_COUNT + 1], written for NO_CANDIDATE
                                       pods only: per reason (pass last), the nodes of C(i) counted on the scenario's
                                       records minus those counted on the source records */
+    /* scenario_plan_kernel<., true> only (nhd_plan_scenarios_rounds) */
+    const int32_t* round_start;    /* [n_scenarios + 1] into round_clock */
+    const double* round_clock;     /* each scenario's later rounds' clocks */
+    const int32_t* slot_start;     /* [n_scenarios]: scenario s's first working slot (replaces the fixed layout) */
+    int32_t* pod_round;            /* [n_pods]: the round that placed the pod, or the scenario's round count */
 };
 
 constexpr int SCENARIO_THREADS = 128;
@@ -2861,8 +2866,14 @@ __device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const Pod
  * nodes), GPU-less pass first for a pod without GPUs (Matcher.py:412-421);
  * then lane 0 runs the mapping and the assignment (query_assign_kernel's body) on that node's working record, keeps
  * the result as the node's working record and writes the binding.  WHY: at a NO_CANDIDATE pod, before any later pod
- * overwrites the working set, the pod's correction row (scenario_why_delta). */
-template <bool WHY>
+ * overwrites the working set, the pod's correction row (scenario_why_delta).
+ * ROUNDS (nhd_plan_scenarios_rounds): then each later round r of the scenario walks its pods again, skipping those
+ * already placed, at the round's clock, on the working set the previous round left; exclusions held at the scenario's
+ * last pod stay held.  The touched set stays exact across rounds (a round only adds the nodes its own attempts reach),
+ * but an attempt that fails its assignment can reach a new node in every round, so the scenario's slots start at
+ * slot_start[s], sized by the host for n_edits + n_adds + min(n_pods * (1 + rounds), n_nodes) touched nodes: at most
+ * one new node per attempt, and each source node at most once. */
+template <bool WHY, bool ROUNDS>
 __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const __grid_constant__ ScenarioArgs a)
 {
     const int lane = threadIdx.x & 31, W = a.words;
@@ -2875,8 +2886,16 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
         const int n_ex_held = a.excl_start[s + 1] - a.excl_start[s], lift = a.lift[s];
         const int e0 = a.edit_start[s], n_edits = a.edit_start[s + 1] - e0;
         const int a0 = a.add_start[s], n_adds = a.add_start[s + 1] - a0;
-        uint4* work = a.work + (size_t)(p0 + e0 + a0) * REC_CHUNKS;
-        int32_t* work_node = a.work_node + p0 + e0 + a0;
+        const int r0 = ROUNDS ? a.round_start[s] : 0, n_rounds = ROUNDS ? a.round_start[s + 1] - r0 : 0;
+        uint4* work;
+        int32_t* work_node;
+        if constexpr (ROUNDS) {
+            work = a.work + (size_t)a.slot_start[s] * REC_CHUNKS;
+            work_node = a.work_node + a.slot_start[s];
+        } else {
+            work = a.work + (size_t)(p0 + e0 + a0) * REC_CHUNKS;
+            work_node = a.work_node + p0 + e0 + a0;
+        }
         for (int k = lane; k < n_edits * REC_CHUNKS; k += 32) work[k] = a.edit_rec[(size_t)e0 * REC_CHUNKS + k];
         for (int k = lane; k < n_edits; k += 32) work_node[k] = a.edit_node[e0 + k];
         for (int k = lane; k < n_adds * REC_CHUNKS; k += 32)
@@ -2884,114 +2903,122 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
         for (int k = lane; k < n_adds; k += 32) work_node[n_edits + k] = a.n_nodes + a0 + k;
         __syncwarp();                                    /* the edited nodes are the first touched ones, then the added */
         int n_touched = n_edits + n_adds;
-        for (int i = p0; i < p1; i++) {
-            const int n_ex = i - p0 < lift ? n_ex_held : 0;           /* back in service from pod lift on */
-            const int ti = a.pod_type[i];
-            const PodType& t = a.types[ti];
-            uint4* bout = reinterpret_cast<uint4*>(&a.out[i]);
-            if (!t.valid_map) {                                        /* Matcher.py:45-47 */
-                if (lane < 8) bout[lane] = make_uint4(lane == 0 ? NHD_BAD_MAP_TYPE : 0, lane == 0 ? 0xFFFFFFFFu : 0, lane == 0 ? t.G : 0, 0);
-                continue;
-            }
-            const uint64_t* F = a.bitmaps + (size_t)ti * W;
-            const uint64_t gm = a.pod_groups ? a.pod_groups[i] : 0;
-            const double now = a.now[i];
-            int chosen = -1, slot = -1;
-            for (int pass = t.needs_gpu ? 1 : 0; pass < 2 && chosen < 0; pass++) {
-                /* the first touched node, in node order, that passes FindNode's stages on its working record */
-                uint64_t best = ~0ULL;
-                int best_k = -1;
-                for (int k = lane; k < n_touched; k += 32) {
-                    RecU u;
-#pragma unroll
-                    for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)k * REC_CHUNKS + c];
-                    const int node = work_node[k];
-                    const uint64_t key = node < a.n_nodes ? ((uint64_t)node << 32) | 0xFFFFFFFFu
-                                                          : ((uint64_t)a.add_at[node - a.n_nodes] << 32) | (uint32_t)(node - a.n_nodes);
-                    if (key < best && (pass == 1 || u.r.n_gpus == 0) && !sorted_contains(ex, n_ex, node) &&
-                        explain_node(u.r, t, a.pod_groups ? gm : t.pod.group_mask, now, a.min_busy, a.cap) == NHD_WHY_COUNT) {
-                        best = key;
-                        best_k = k;
-                    }
+        for (int r = 0; r <= n_rounds; r++) {
+            for (int i = p0; i < p1; i++) {
+                if constexpr (ROUNDS) {                                    /* lane 0 wrote the pod's last binding */
+                    if (r > 0 && __shfl_sync(0xFFFFFFFFu, lane == 0 ? a.out[i].status : 0, 0) == NHD_PLACED) continue;
                 }
-                for (int o = 16; o; o >>= 1) {
-                    const uint64_t ob = __shfl_sync(0xFFFFFFFFu, best, lane ^ o);
-                    const int ok = __shfl_sync(0xFFFFFFFFu, best_k, lane ^ o);
-                    if (ob < best) { best = ob; best_k = ok; }
+                /* back in service from pod lift on; a later round sees what the scenario's last pod saw */
+                const int n_ex = (r == 0 ? i - p0 : p1 - p0 - 1) < lift ? n_ex_held : 0;
+                const int ti = a.pod_type[i];
+                const PodType& t = a.types[ti];
+                uint4* bout = reinterpret_cast<uint4*>(&a.out[i]);
+                if (!t.valid_map) {                                        /* Matcher.py:45-47 */
+                    if (lane < 8) bout[lane] = make_uint4(lane == 0 ? NHD_BAD_MAP_TYPE : 0, lane == 0 ? 0xFFFFFFFFu : 0, lane == 0 ? t.G : 0, 0);
+                    if (ROUNDS && lane == 0) a.pod_round[i] = n_rounds;
+                    continue;
                 }
-                /* the first untouched candidate, only where it comes before that node: untouched node n before key
-                 * (pos, sub) exactly when n < pos */
-                const long long best_pos = (long long)(best >> 32);
-                int first = -1;
-                for (int base = 0; base < W && first < 0 && (long long)base * 64 < best_pos; base += 32) {
-                    const int w = base + lane;
-                    int mine = -1;
-                    if (w < W) {
-                        uint64_t word = F[w] & (pass == 0 ? NOGPU[w] : ~0ULL);
-                        if (a.pod_groups && word) {                    /* InitialNodeFilter per group name (NHDScheduler.py:241) */
-                            uint64_t e = 0;
-                            for (uint64_t g = gm; g; g &= g - 1)
-                                e |= GB[(size_t)popc64(a.names_used & ((1ULL << ctz64(g)) - 1)) * W + w];
-                            word &= e;
+                const uint64_t* F = a.bitmaps + (size_t)ti * W;
+                const uint64_t gm = a.pod_groups ? a.pod_groups[i] : 0;
+                const double now = ROUNDS && r > 0 ? a.round_clock[r0 + r - 1] : a.now[i];
+                int chosen = -1, slot = -1;
+                for (int pass = t.needs_gpu ? 1 : 0; pass < 2 && chosen < 0; pass++) {
+                    /* the first touched node, in node order, that passes FindNode's stages on its working record */
+                    uint64_t best = ~0ULL;
+                    int best_k = -1;
+                    for (int k = lane; k < n_touched; k += 32) {
+                        RecU u;
+    #pragma unroll
+                        for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)k * REC_CHUNKS + c];
+                        const int node = work_node[k];
+                        const uint64_t key = node < a.n_nodes ? ((uint64_t)node << 32) | 0xFFFFFFFFu
+                                                              : ((uint64_t)a.add_at[node - a.n_nodes] << 32) | (uint32_t)(node - a.n_nodes);
+                        if (key < best && (pass == 1 || u.r.n_gpus == 0) && !sorted_contains(ex, n_ex, node) &&
+                            explain_node(u.r, t, a.pod_groups ? gm : t.pod.group_mask, now, a.min_busy, a.cap) == NHD_WHY_COUNT) {
+                            best = key;
+                            best_k = k;
                         }
-                        for (; word; word &= word - 1) {
-                            const int node = w * 64 + ctz64(word);
-                            if (node >= best_pos) break;
-                            if (sorted_contains(ex, n_ex, node)) continue;
-                            bool touched = false;
-                            for (int k = 0; k < n_touched && !touched; k++) touched = work_node[k] == node;
-                            if (touched) continue;
-                            if (t.needs_gpu) {
-                                nhd_node_rec r;
-                                r.busy_time = *reinterpret_cast<const double*>(a.nodes + chunk_off(node, 3));
-                                if (node_busy(r, now, a.min_busy)) continue;
+                    }
+                    for (int o = 16; o; o >>= 1) {
+                        const uint64_t ob = __shfl_sync(0xFFFFFFFFu, best, lane ^ o);
+                        const int ok = __shfl_sync(0xFFFFFFFFu, best_k, lane ^ o);
+                        if (ob < best) { best = ob; best_k = ok; }
+                    }
+                    /* the first untouched candidate, only where it comes before that node: untouched node n before key
+                     * (pos, sub) exactly when n < pos */
+                    const long long best_pos = (long long)(best >> 32);
+                    int first = -1;
+                    for (int base = 0; base < W && first < 0 && (long long)base * 64 < best_pos; base += 32) {
+                        const int w = base + lane;
+                        int mine = -1;
+                        if (w < W) {
+                            uint64_t word = F[w] & (pass == 0 ? NOGPU[w] : ~0ULL);
+                            if (a.pod_groups && word) {                    /* InitialNodeFilter per group name (NHDScheduler.py:241) */
+                                uint64_t e = 0;
+                                for (uint64_t g = gm; g; g &= g - 1)
+                                    e |= GB[(size_t)popc64(a.names_used & ((1ULL << ctz64(g)) - 1)) * W + w];
+                                word &= e;
                             }
-                            mine = node;
-                            break;
+                            for (; word; word &= word - 1) {
+                                const int node = w * 64 + ctz64(word);
+                                if (node >= best_pos) break;
+                                if (sorted_contains(ex, n_ex, node)) continue;
+                                bool touched = false;
+                                for (int k = 0; k < n_touched && !touched; k++) touched = work_node[k] == node;
+                                if (touched) continue;
+                                if (t.needs_gpu) {
+                                    nhd_node_rec r;
+                                    r.busy_time = *reinterpret_cast<const double*>(a.nodes + chunk_off(node, 3));
+                                    if (node_busy(r, now, a.min_busy)) continue;
+                                }
+                                mine = node;
+                                break;
+                            }
                         }
+                        const unsigned m = __ballot_sync(0xFFFFFFFFu, mine >= 0);
+                        if (m) first = __shfl_sync(0xFFFFFFFFu, mine, ctz32(m));
                     }
-                    const unsigned m = __ballot_sync(0xFFFFFFFFu, mine >= 0);
-                    if (m) first = __shfl_sync(0xFFFFFFFFu, mine, ctz32(m));
-                }
-                if (first >= 0) { chosen = first; slot = n_touched; }
-                else if (best_k >= 0) {
-                    const uint32_t sub = (uint32_t)best;
-                    chosen = sub == 0xFFFFFFFFu ? (int)best_pos : a.n_nodes + (int)sub;
-                    slot = best_k;
-                }
-            }
-            if (lane == 0) {
-                union { nhd_binding b; uint4 q[8]; } bu;
-                for (int c = 0; c < 8; c++) bu.q[c] = make_uint4(0, 0, 0, 0);
-                if (chosen < 0) {
-                    bu.q[0] = make_uint4(NHD_NO_CANDIDATE, 0xFFFFFFFFu, t.G, 0);
-                } else {
-                    RecU u;
-                    if (slot < n_touched) {
-                        for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)slot * REC_CHUNKS + c];
-                    } else {
-                        load_rec(a.nodes, chosen, u);
+                    if (first >= 0) { chosen = first; slot = n_touched; }
+                    else if (best_k >= 0) {
+                        const uint32_t sub = (uint32_t)best;
+                        chosen = sub == 0xFFFFFFFFu ? (int)best_pos : a.n_nodes + (int)sub;
+                        slot = best_k;
                     }
-                    Mapping m;
-                    if (evaluate_mapping(u.r, t, a.cap, &m)) {
-                        bu.b.node = chosen;
-                        assign_pod(u.r, t, m, now, &bu.b);             /* the reference's unwind on a failed assignment */
-                    } else {
-                        atomicAdd(a.bad, 1u);                          /* the candidate test said feasible */
+                }
+                if (lane == 0) {
+                    union { nhd_binding b; uint4 q[8]; } bu;
+                    for (int c = 0; c < 8; c++) bu.q[c] = make_uint4(0, 0, 0, 0);
+                    if (chosen < 0) {
                         bu.q[0] = make_uint4(NHD_NO_CANDIDATE, 0xFFFFFFFFu, t.G, 0);
+                    } else {
+                        RecU u;
+                        if (slot < n_touched) {
+                            for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)slot * REC_CHUNKS + c];
+                        } else {
+                            load_rec(a.nodes, chosen, u);
+                        }
+                        Mapping m;
+                        if (evaluate_mapping(u.r, t, a.cap, &m)) {
+                            bu.b.node = chosen;
+                            assign_pod(u.r, t, m, now, &bu.b);             /* the reference's unwind on a failed assignment */
+                        } else {
+                            atomicAdd(a.bad, 1u);                          /* the candidate test said feasible */
+                            bu.q[0] = make_uint4(NHD_NO_CANDIDATE, 0xFFFFFFFFu, t.G, 0);
+                        }
+                        for (int c = 0; c < REC_CHUNKS; c++) work[(size_t)slot * REC_CHUNKS + c] = u.q[c];
+                        work_node[slot] = chosen;
                     }
-                    for (int c = 0; c < REC_CHUNKS; c++) work[(size_t)slot * REC_CHUNKS + c] = u.q[c];
-                    work_node[slot] = chosen;
+                    for (int c = 0; c < 8; c++) bout[c] = bu.q[c];
+                    if constexpr (ROUNDS) a.pod_round[i] = bu.b.status == NHD_PLACED ? r : n_rounds;
                 }
-                for (int c = 0; c < 8; c++) bout[c] = bu.q[c];
+                if constexpr (WHY) {
+                    if (chosen < 0)                                        /* warp-uniform */
+                        scenario_why_delta(a, t, a.pod_groups ? gm : t.pod.group_mask, now, ex, n_ex, work, work_node,
+                                           n_touched, a.why_delta + (size_t)i * (NHD_WHY_COUNT + 1));
+                }
+                if (chosen >= 0 && slot == n_touched) n_touched++;
+                __syncwarp();                                              /* the slot is read by every lane from here on */
             }
-            if constexpr (WHY) {
-                if (chosen < 0)                                        /* warp-uniform */
-                    scenario_why_delta(a, t, a.pod_groups ? gm : t.pod.group_mask, now, ex, n_ex, work, work_node,
-                                       n_touched, a.why_delta + (size_t)i * (NHD_WHY_COUNT + 1));
-            }
-            if (chosen >= 0 && slot == n_touched) n_touched++;
-            __syncwarp();                                              /* the slot is read by every lane from here on */
         }
     }
 }

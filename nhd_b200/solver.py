@@ -241,16 +241,22 @@ class Solver:
         ``adds`` (sixth element, None: none): ``(at, records)``, int positions and a ``wire.NODE_DTYPE`` array: nodes
         added for the whole scenario, each right before source node ``at[k]`` (``n_nodes``: at the end), ``at`` never
         going down (``nhd_plan_scenarios_grown``).  A pod placed on one gets node ``n_nodes + a``, ``a`` its index among
-        the added records of the whole call, in scenario order."""
+        the added records of the whole call, in scenario order.
+        ``rounds`` (seventh element, None: none): the clocks of later pending scans, never going down and none before
+        the scenario's pod clocks (``nhd_plan_scenarios_rounds``).  At each, the scenario's pods not placed yet are
+        solved again in order on the records the previous scan left; ``bindings`` hold each pod's last attempt.  When
+        any scenario has rounds, each result gains a last element: the ``(n_s,)`` int32 round that placed each pod, or
+        ``len(rounds)`` if none did (None when refused)."""
         src = _source(source)
         # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
         # would cost more than the call itself)
-        exs, podb, nowl, lifts, ednodes, edrecs, n_adds, adats, adrecs = [], [], [], [], [], [], [], [], []
+        exs, podb, nowl, lifts, ednodes, edrecs, n_adds, adats, adrecs, rounds = [], [], [], [], [], [], [], [], [], []
         for sc in scenarios:
             exclude, pods, now = sc[:3]
             lift = sc[3] if len(sc) > 3 else None
             edits = sc[4] if len(sc) > 4 else None
             adds = sc[5] if len(sc) > 5 else None
+            rounds.append(sc[6] if len(sc) > 6 else None)
             pods = np.asarray(pods)
             if pods.dtype != wire.POD_DTYPE:
                 pods = pods.astype(wire.POD_DTYPE)
@@ -297,14 +303,30 @@ class Solver:
                 edrec.ctypes.data if len(edrec) else None)
         tail = (pod_start.ctypes.data, pods.ctypes.data if len(pods) else None, now.ctypes.data if len(pods) else None,
                 out.ctypes.data if len(pods) else None, status.ctypes.data, which.ctypes.data)
+        adds = (None, None, None)
         if any(n_adds):
             add_start = np.zeros(n + 1, dtype='<i4')
             add_start[1:] = np.cumsum(n_adds)
             adat = np.ascontiguousarray(np.concatenate(adats), dtype='<i4')
             adrec = np.frombuffer(b''.join(adrecs), dtype=wire.NODE_DTYPE)
+            adds = (add_start.ctypes.data, adat.ctypes.data, adrec.ctypes.data)
+        if any(r is not None for r in rounds):
+            clocks = [np.asarray(() if r is None else r, dtype='<f8').reshape(-1) for r in rounds]
+            round_start = np.zeros(n + 1, dtype='<i4')
+            round_start[1:] = np.cumsum([len(c) for c in clocks])
+            round_clock = np.ascontiguousarray(np.concatenate(clocks), dtype='<f8')
             counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
-            self._ck(self._L.nhd_plan_scenarios_grown(*head, add_start.ctypes.data, adat.ctypes.data,
-                                                      adrec.ctypes.data, *tail,
+            pod_round = np.zeros(len(pods), dtype='<i4')
+            self._ck(self._L.nhd_plan_scenarios_rounds(*head, *adds, *tail[:3], round_start.ctypes.data,
+                                                       round_clock.ctypes.data if len(round_clock) else None, *tail[3:],
+                                                       counts.ctypes.data if explain and len(pods) else None,
+                                                       pod_round.ctypes.data if len(pods) else None))
+            res = self._scenario_results(status, which, pod_start, out, counts)
+            return [r + (pod_round[a:b] if r[0] == 0 else None,)
+                    for r, a, b in zip(res, pod_start[:-1].tolist(), pod_start[1:].tolist())]
+        if any(n_adds):
+            counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
+            self._ck(self._L.nhd_plan_scenarios_grown(*head, *adds, *tail,
                                                       counts.ctypes.data if explain and len(pods) else None))
             return self._scenario_results(status, which, pod_start, out, counts)
         args = head + tail
