@@ -457,6 +457,35 @@ int32_t nhd_plan_scenarios_rounds(nhd_handle* h, int32_t source, int32_t n_scena
                                   nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
                                   uint32_t* why_counts, int32_t* pod_round);
 
+/*
+ * nhd_plan_batch over several pending scans: "the queue I have now, on the cluster I have now: which pods get in at a
+ * later scan, and which never do?".  One large batch, solved by the batch path at every scan (nhd_plan_scenarios_rounds
+ * runs each scenario on one warp and is meant for many small ones).  Round 0 is nhd_plan_batch(h, source, n_excluded,
+ * excluded, n_pods, pods, now, ...).  For r = 1 .. n_rounds the pods whose latest binding is not NHD_PLACED are solved
+ * in their original order as one nhd_solve_batch at clock round_clock[r-1], on the records the previous round left
+ * (placements, and the busy stamp of a failed assignment, committed to the plan's own copy); a round with no such pod
+ * does nothing.  The excluded nodes stay in maintenance in every round.
+ *   out[i]         byte for byte pod i's last attempt;
+ *   pod_round      (may be NULL) n_pods entries: the round that placed the pod, or n_rounds if none did;
+ *   why_counts     (may be NULL) n_pods * NHD_WHY_COUNT entries: for a pod whose last attempt is NHD_NO_CANDIDATE, the
+ *                  row nhd_explain_batch would give for that attempt (the records at the start of that round plus that
+ *                  round's earlier pods, at the round's clock); all other rows zero.
+ * Bindings, pod_round and why_counts equal those of nhd_plan_scenarios_rounds called with this one scenario, its
+ * exclusions held to the end (lift_at NULL), no edits and no additions; the one difference is nhd_plan_batch's: the
+ * tuple limits are judged without the excluded nodes.  n_rounds == 0 is nhd_plan_batch (round_clock is not read,
+ * pod_round, if given, is all zero).
+ * Refused as nhd_plan_batch refuses, and NHD_ERR_INVALID for n_rounds < 0, a NULL round_clock with n_rounds > 0, a
+ * non-finite round clock, round clocks that go down, and a first round clock earlier than a now[] (a monotonic clock
+ * never goes back).  The busy test is now - busy_time < min_busy_secs in fp64: give the clocks exactly as the caller's
+ * clock would read them, each the previous one plus the period, not t0 + r * period.  A node passing every stage for a
+ * NO_CANDIDATE pod is NHD_ERR_STATE.  Nothing is written that a caller can observe (the list of nhd_plan_batch), no
+ * collective is entered (any rank may call alone), and the call waits for the device before returning.
+ */
+int32_t nhd_plan_batch_rounds(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                              int32_t n_pods, const nhd_pod* pods, const double* now,
+                              int32_t n_rounds, const double* round_clock,
+                              nhd_binding* out, uint32_t* why_counts, int32_t* pod_round);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

@@ -258,6 +258,21 @@ class DeviceCluster:
         return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), source=source, exclude=idx,
                   explain=explain)
 
+    def forecast(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now, round_clocks: Sequence[float],
+                 source: str = 'mirror', exclude: Iterable[str] = (), explain: bool = False, packed: Sequence = None):
+        """``plan`` over several pending scans (``Solver.plan_batch_rounds``): after the dry run at ``now``, at each
+        clock of ``round_clocks`` the pods no earlier scan placed are retried in order on the cluster the earlier scans
+        left, the nodes named in ``exclude`` in maintenance throughout.  Returns ``(bindings, pod_round)``: each pod's
+        last attempt and the scan that placed it, or ``len(round_clocks)``; ``explain=True``: also the per-reason node
+        counts of the pods whose last attempt found no node.  None when the solver in use cannot (a stand-in without
+        ``plan_batch_rounds``)."""
+        fn = getattr(self._solver, 'plan_batch_rounds', None)
+        if fn is None:
+            return None
+        idx = self._indices(exclude, 'exclude')
+        return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), round_clocks, source=source,
+                  exclude=idx, explain=explain)
+
     def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror', explain: bool = False):
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
         of ``(exclude, tops, pod_groups, now[, packed[, lift[, edits]]])`` with ``exclude`` node names.  ``lift`` (None:
@@ -938,19 +953,44 @@ class NHDScheduler:
         solver's tuple limits included).  ``reasons=True``: ``(placement, reasons)``, ``reasons[(ns, name)]`` being
         ``{reason name: nodes}`` for each pod no scan placed that found no node at its last scan, at that scan's state.
         Names and reads as ``PlanExpansion``: only reads happen; ``pod_state``, the ``Node`` objects and the counters
-        stay as they are."""
-        scans = int(scans)
-        if scans < 1:
-            raise ValueError(f'scans must be at least 1, not {scans}')
-        period = float(60 * 0.5 if period is None else period)     # run()'s idle_thresh x block_secs
-        result = self._grown_plans([[]] if additions is None else additions, keys, reasons, [period] * (scans - 1))
+        stay as they are.  One scenario without added nodes is one large batch and is solved by the batch path at every
+        scan (``DeviceCluster.forecast``); several scenarios, or added nodes, run side by side, one warp each."""
+        result = self._grown_plans([[]] if additions is None else additions, keys, reasons,
+                                   self._scan_periods(scans, period))
         out = [(p, why) if reasons else p for p, why in result]
         return out[0] if additions is None else out
 
-    def _grown_plans(self, additions: Sequence[Sequence], keys: Sequence, reasons: bool, periods: Sequence[float]):
+    def ForecastDrain(self, node_names: Sequence[str], scans: int, period: float = None, reasons: bool = False):
+        """When do the pods of drained nodes get back in?  ``PlanDrain``'s pods (the pods now on ``node_names``, nodes in
+        the given order, pods in ``Node.pod_info`` order, read as re-created pods) forecast over ``scans`` pending scans
+        as ``ForecastPending`` forecasts the pending pods, with those nodes in maintenance throughout: a GPU node takes
+        one GPU pod per busy window, so most pods of a drained GPU node find every node busy at scan 0 and place at a
+        later one.  Returns ``{(ns, name): (scan, node name) or None}``; ``reasons=True``: ``(placement, reasons)`` as
+        ``ForecastPending``.  ``ForecastDrain(names, 1)`` is ``PlanDrain(names)`` with every node as ``(0, node)``.
+        Only reads happen, as ``PlanDrain``."""
+        names = list(node_names)
+        missing = [n for n in names if n not in self.nodes]
+        if missing:
+            raise ValueError(f'unknown node(s) {missing}')
+        placement, why = self._grown_plans([[]], self._pods_on(names), reasons, self._scan_periods(scans, period),
+                                           exclude=names)[0]
+        return (placement, why) if reasons else placement
+
+    @staticmethod
+    def _scan_periods(scans: int, period: float) -> List[float]:
+        """The seconds between ``scans`` pending scans, ``period`` defaulting to ``run()``'s ``idle_thresh x
+        block_secs``."""
+        scans = int(scans)
+        if scans < 1:
+            raise ValueError(f'scans must be at least 1, not {scans}')
+        return [float(60 * 0.5 if period is None else period)] * (scans - 1)
+
+    def _grown_plans(self, additions: Sequence[Sequence], keys: Sequence, reasons: bool, periods: Sequence[float],
+                     exclude: Sequence[str] = ()):
         """``PlanExpansion``'s plans, with a later scan after each of ``periods`` seconds: per scenario ``(placement,
         reasons)``, a placed pod mapped to its node name, or with ``periods`` (even an empty list) to ``(scan, node
-        name)``.  ``periods`` None: one scan, through the call without rounds."""
+        name)``.  ``periods`` None: one scan, through the call without rounds.  ``exclude``: nodes in maintenance
+        throughout, in every scenario."""
         scens = [[(node, before) for node, before in sc] for sc in additions]
         for sc in scens:
             names = [node.name for node, _ in sc]
@@ -977,9 +1017,25 @@ class NHDScheduler:
                     clocks.append(clocks[-1] + float(p))
                 clocks = clocks[1:]
             todo = [(j, entries) for j in range(len(scens))]
+            if clocks is not None and scens == [[]]:
+                # one scenario on the cluster as it is: one batch per scan (a pod beyond the tuple limits is dropped
+                # and the rest planned again, as _plan_prepared does)
+                res, ok, _ = self._without_refused(
+                    lambda es: self.cluster.forecast([e.top for e in es], [e.groups for e in es], now, clocks,
+                                                     exclude=exclude, explain=reasons, packed=[e.rec for e in es]),
+                    entries)
+                if res is not None or not ok:
+                    todo = []
+                if res is not None:
+                    placement, why = result[0]
+                    for e, b, r in zip(ok, res[0], res[1]):
+                        if int(b['status']) == wire.PLACED:
+                            placement[(e.key[0], e.key[1])] = (int(r), self.cluster.name_of(int(b['node'])))
+                    if reasons:
+                        why.update(self._reasons(ok, res[0], res[2]))
             while todo:
                 res = self._supported(
-                    self.cluster.plan_scenarios([((), [e.top for e in ok], [e.groups for e in ok], now,
+                    self.cluster.plan_scenarios([(exclude, [e.top for e in ok], [e.groups for e in ok], now,
                                                   [e.rec for e in ok], None, None,
                                                   [(before, node) for node, before in scens[j]])
                                                  + ((clocks,) if clocks is not None else ()) for j, ok in todo],

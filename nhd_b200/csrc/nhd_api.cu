@@ -77,6 +77,7 @@ struct Buf {
     Buf& operator=(const Buf&) = delete;
     ~Buf() { release(); }
     operator T*() const { return p; }
+    void swap(Buf& o) { std::swap(p, o.p); std::swap(cap, o.cap); }
     void release()
     {
         if (p) Pinned ? cudaFreeHost(p) : cudaFree(p);
@@ -104,6 +105,7 @@ template <typename T> using PinnedBuf = Buf<T, true>;
 struct Workspace {
     /* the pod set */
     int n_pods = 0, n_types = 0, n_names = 0;
+    int pod_cap = 0;                      /* pods the arrays are laid out for: n_pods as staged (a plan's later rounds hold fewer) */
     uint64_t names_used = 0;
     double now0 = 0.0;                    /* clock of the first pod (the filter's BUSY row) */
     bool const_clock = true;
@@ -124,12 +126,12 @@ struct Workspace {
     DevBuf<nhd_binding> out;              /* n_pods + 8 (spare records for check builds) */
     PinnedBuf<nhd_binding> h_out;         /* bounce buffer of fetch_bindings */
 
-    size_t now_offset() const { return ((size_t)n_pods * 4 + 15) & ~(size_t)15; }
+    size_t now_offset() const { return ((size_t)pod_cap * 4 + 15) & ~(size_t)15; }
     const int32_t* pod_type() const { return reinterpret_cast<const int32_t*>(pod_arrays.p); }
     const double* now() const { return reinterpret_cast<const double*>(pod_arrays.p + now_offset()); }
     const uint64_t* pod_groups() const      /* per-pod node-group masks when the pods mix lists, else null */
     {
-        return n_names ? reinterpret_cast<const uint64_t*>(pod_arrays.p + now_offset() + (size_t)n_pods * 8) : nullptr;
+        return n_names ? reinterpret_cast<const uint64_t*>(pod_arrays.p + now_offset() + (size_t)pod_cap * 8) : nullptr;
     }
 };
 
@@ -197,6 +199,14 @@ struct nhd_handle {
     /* a plan's copy of the records, with its excluded nodes flagged there, and their indices */
     DevBuf<uint8_t> d_pnodes;
     DevBuf<int32_t> d_pidx;
+    /* a plan's rounds (nhd_plan_batch_rounds): the other half of the scratch pod arrays, both caller-row maps | the round
+     * that placed each pod | survivors per CTA, every pod's last attempt, the last round's reason rows, and the word the
+     * device leaves the next round's pod count in */
+    DevBuf<uint8_t> d_rpods;
+    DevBuf<int32_t> d_ridx;
+    DevBuf<nhd_binding> d_rout;
+    DevBuf<uint32_t> d_rwhy;
+    PinnedBuf<int32_t> h_rcount;
     /* scenario plans: pod offsets | exclusion offsets | exclusions | edit offsets | edited nodes | lift indices | slot
      * nodes | the failed-mapping word, and one working record per slot followed by the edit records */
     DevBuf<int32_t> d_sidx;
@@ -747,7 +757,7 @@ static int32_t stage_pods(nhd_handle* h, Workspace& w, int n, const nhd_pod* pod
     if (rc != NHD_OK) return rc;
     CK(cudaSetDevice(h->params.device));
     const int T = (int)types.size();
-    w.n_pods = n;
+    w.n_pods = w.pod_cap = n;
     w.n_types = T;
     w.n_names = multi_group ? __builtin_popcountll(names_used) : 0;
     w.names_used = multi_group ? names_used : 0;
@@ -806,12 +816,12 @@ extern "C" int32_t nhd_run_filter_only(nhd_handle* h)
 
 /*
  * The launches of a solve of w's pod set on the records nodes: direct-path tables, filter, sweep, resolve, core ids.
- * batch = the handle's staged batch on the mirror: its timing events, the node-sharded filter + exchange when
- * world_size > 1, and commit_kernel, which folds the bindings into the mirror.  Without it (a plan, or a query's
- * filter) none of the three: every rank filters the whole cluster and the records are only read.  filter_only stops
- * after the filter.
+ * batch = the handle's staged batch on the mirror: its timing events and the node-sharded filter + exchange when
+ * world_size > 1.  Without it (a plan, or a query's filter) neither: every rank filters the whole cluster.  commit =
+ * commit_kernel folds the bindings into nodes (the mirror for the batch, a plan's own copy between its rounds);
+ * without it the records are only read.  filter_only stops after the filter.
  */
-static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, bool batch, bool filter_only)
+static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, bool batch, bool commit, bool filter_only)
 {
     const int T = w.n_types, W = h->words;
     int launches = 0;
@@ -884,7 +894,7 @@ static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, b
 
     /* 3. sequential select + assign sweep (replicated on every rank) */
     if (w.n_pods > 0 && !filter_only) {
-        /* (the sweep's and the finishing kernels' record pointer is writable for commit_kernel, which only a batch runs) */
+        /* (the sweep's and the finishing kernels' record pointer is writable for commit_kernel) */
         uint8_t* const records = const_cast<uint8_t*>(nodes);
         SweepArgs sa;
         sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type(); sa.now = w.now(); sa.out = w.out;
@@ -929,7 +939,7 @@ static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, b
         assign_cores_kernel<<<fgrid, fthreads, 0, h->stream>>>(fin);
         CK(cudaGetLastError());
         launches += 3;
-        if (batch) {
+        if (commit) {
             commit_kernel<<<fgrid, fthreads, 0, h->stream>>>(fin);
             CK(cudaGetLastError());
             launches++;
@@ -951,19 +961,20 @@ static int32_t solve_staged(nhd_handle* h, bool filter_only)
     h->gen++;
     h->explain_gen = explainable ? h->gen : 0;
     CK(cudaSetDevice(h->params.device));
-    const int32_t rc = launch_solve(h, h->batch, h->d_nodes, true, filter_only);
+    const int32_t rc = launch_solve(h, h->batch, h->d_nodes, true, !filter_only, filter_only);
     if (rc != NHD_OK) return rc;
     h->solved = true;
     return NHD_OK;
 }
 
-/* device -> host: the first n bindings of w, through its bounce buffer unless out is pinned; waits for the device */
-static int32_t fetch_bindings(nhd_handle* h, Workspace& w, int n, nhd_binding* out)
+/* device -> host: the first n bindings of w (or of from, when given), through w's bounce buffer unless out is pinned;
+ * waits for the device */
+static int32_t fetch_bindings(nhd_handle* h, Workspace& w, int n, nhd_binding* out, const nhd_binding* from = nullptr)
 {
     const size_t bytes = (size_t)n * sizeof(nhd_binding);
     const bool direct = bytes == 0 || is_pinned_host(out);
     if (!direct) CK(w.h_out.grow(bytes));
-    if (bytes) CK(cudaMemcpyAsync(direct ? (void*)out : (void*)w.h_out.p, w.out, bytes, cudaMemcpyDeviceToHost, h->stream));
+    if (bytes) CK(cudaMemcpyAsync(direct ? (void*)out : (void*)w.h_out.p, from ? from : w.out.p, bytes, cudaMemcpyDeviceToHost, h->stream));
     CK(cudaStreamSynchronize(h->stream));
     if (!direct) memcpy(out, w.h_out, bytes);
     return NHD_OK;
@@ -1117,18 +1128,26 @@ static int32_t explain_survivors(nhd_handle* h, const char* what)
     return NHD_OK;
 }
 
-/* per-reason node counts of every NO_CANDIDATE pod of w's solve from the records nodes into the host array counts
- * (n_pods * NHD_WHY_COUNT) */
-static int32_t explain_counts(nhd_handle* h, const Workspace& w, const uint8_t* nodes, uint32_t* counts, const char* what)
+/* per-reason node counts of every NO_CANDIDATE pod of w's solve from the records nodes into d_xcounts (n_pods > 0 rows
+ * of NHD_WHY_COUNT, zero for the other pods) */
+static int32_t explain_rows(nhd_handle* h, const Workspace& w, const uint8_t* nodes)
 {
     const size_t bytes = (size_t)w.n_pods * NHD_WHY_COUNT * 4;
-    if (bytes == 0) return NHD_OK;
     int nf = 0;
     int32_t rc;
     if ((rc = explain_prepare(h, w, &nf)) != NHD_OK) return rc;
     CK(h->d_xcounts.grow(bytes));
     CK(cudaMemsetAsync(h->d_xcounts, 0, bytes, h->stream));
-    if ((rc = explain_launch(h, w, nodes, nf, h->d_xcounts, nullptr)) != NHD_OK) return rc;
+    return explain_launch(h, w, nodes, nf, h->d_xcounts, nullptr);
+}
+
+/* ... into the host array counts (n_pods * NHD_WHY_COUNT) */
+static int32_t explain_counts(nhd_handle* h, const Workspace& w, const uint8_t* nodes, uint32_t* counts, const char* what)
+{
+    const size_t bytes = (size_t)w.n_pods * NHD_WHY_COUNT * 4;
+    if (bytes == 0) return NHD_OK;
+    const int32_t rc = explain_rows(h, w, nodes);
+    if (rc != NHD_OK) return rc;
     CK(cudaMemcpyAsync(counts, h->d_xcounts, bytes, cudaMemcpyDeviceToHost, h->stream));
     return explain_survivors(h, what);
 }
@@ -1202,7 +1221,7 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
     if ((rc = stage_pods(h, w, n_pods, pods, now, h->max_numa)) != NHD_OK) return rc;
 
     /* the candidate bitmaps of the query's pod types on the chosen records */
-    if ((rc = launch_solve(h, w, nodes, false, true)) != NHD_OK) return rc;
+    if ((rc = launch_solve(h, w, nodes, false, false, true)) != NHD_OK) return rc;
 
     /* each pod on its own: the node, then the mapping and the assignment on a copy of its record */
     QueryArgs qa;
@@ -1222,15 +1241,31 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
 /*
  * The bindings nhd_solve_batch would return on the chosen records with the excluded nodes in maintenance, and
  * optionally nhd_explain_batch's counts after it, with nothing written but the scratch: the solve's own launches
- * (launch_solve) on the scratch workspace, without the commit and without sharding.  With exclusions the records are first copied into a plan-owned array and the excluded
- * nodes flagged there (exclude_nodes_kernel); without, the source records are read in place.
+ * (launch_solve) on the scratch workspace, without the commit and without sharding.  With exclusions the records are
+ * first copied into a plan-owned array and the excluded nodes flagged there (exclude_nodes_kernel); without, the source
+ * records are read in place.
+ * With rounds (nhd_plan_batch_rounds, n_rounds > 0) the records are always copied, and every round but the last commits
+ * to the copy; round r >= 1 is the same launches on the pods round r - 1 left unplaced, at round_clock[r - 1].  The pod
+ * types are staged once; round_advance_kernel hands the unplaced pods (type, group mask, caller row) to the other half
+ * of the double-buffered pod arrays and every binding to its caller's row, and the host reads one word per round, the
+ * next round's pod count.  Only the last round can leave a NO_CANDIDATE last attempt (an unplaced pod is retried in
+ * every round), so only it is explained, on the records it started from: it runs no commit.
  */
-extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
-                                  int32_t n_pods, const nhd_pod* pods, const double* now, nhd_binding* out,
-                                  uint32_t* why_counts)
+static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                          int32_t n_pods, const nhd_pod* pods, const double* now, int32_t n_rounds,
+                          const double* round_clock, nhd_binding* out, uint32_t* why_counts, int32_t* pod_round)
 {
     if (!h || n_pods < 0 || n_excluded < 0 || (n_excluded > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)))
         return NHD_ERR_INVALID;
+    if (n_rounds < 0) return fail(h, NHD_ERR_INVALID, "%d rounds", n_rounds);
+    if (n_rounds > 0 && !round_clock) return fail(h, NHD_ERR_INVALID, "%d rounds without round clocks", n_rounds);
+    for (int r = 0; r < n_rounds; r++) {
+        if (!std::isfinite(round_clock[r])) return fail(h, NHD_ERR_INVALID, "round clock %d is not finite", r);
+        if (r > 0 && round_clock[r] < round_clock[r - 1]) return fail(h, NHD_ERR_INVALID, "round clocks go down at %d", r);
+    }
+    for (int i = 0; i < n_pods && n_rounds > 0; i++)         /* a monotonic clock never goes back */
+        if (round_clock[0] < now[i])
+            return fail(h, NHD_ERR_INVALID, "round clock 0 is earlier than the clock of pod %d", i);
     const uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
     if (rc != NHD_OK) return rc;
@@ -1259,18 +1294,89 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
     Workspace& w = h->scratch;
     if ((rc = stage_pods(h, w, n_pods, pods, now, max_numa)) != NHD_OK) return rc;
     const uint8_t* nodes = records;
-    if (!ex.empty()) {
+    if (!ex.empty() || n_rounds > 0) {
         CK(h->d_pnodes.grow(h->nodes_bytes));
-        CK(h->d_pidx.grow(ex.size() * 4));
         CK(cudaMemcpyAsync(h->d_pnodes, records, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
+        nodes = h->d_pnodes;
+    }
+    if (!ex.empty()) {
+        CK(h->d_pidx.grow(ex.size() * 4));
         CK(cudaMemcpyAsync(h->d_pidx, ex.data(), ex.size() * 4, cudaMemcpyHostToDevice, h->stream));
         exclude_nodes_kernel<<<(unsigned)((ex.size() + 255) / 256), 256, 0, h->stream>>>(h->d_pnodes, h->d_pidx, (int)ex.size());
         CK(cudaGetLastError());
-        nodes = h->d_pnodes;
     }
-    if ((rc = launch_solve(h, w, nodes, false, false)) != NHD_OK) return rc;
-    if (why_counts && (rc = explain_counts(h, w, nodes, why_counts, "nhd_plan_batch")) != NHD_OK) return rc;
-    return fetch_bindings(h, w, n_pods, out);
+    if (n_rounds == 0) {
+        if (pod_round) memset(pod_round, 0, (size_t)n_pods * 4);
+        if ((rc = launch_solve(h, w, nodes, false, false, false)) != NHD_OK) return rc;
+        if (why_counts && (rc = explain_counts(h, w, nodes, why_counts, what)) != NHD_OK) return rc;
+        return fetch_bindings(h, w, n_pods, out);
+    }
+
+    const size_t P = (size_t)n_pods, grid0 = (P + ROUND_THREADS - 1) / ROUND_THREADS, why_bytes = P * NHD_WHY_COUNT * 4;
+    const size_t off_now = w.now_offset(), off_gm = off_now + P * 8;
+    CK(h->d_rpods.grow(off_gm + (w.n_names ? P * 8 : 0)));
+    CK(h->d_ridx.grow((3 * P + grid0) * 4));
+    CK(h->d_rout.grow(P * sizeof(nhd_binding)));
+    CK(h->h_rcount.grow(4));
+    if (why_counts) {
+        CK(h->d_rwhy.grow(why_bytes));
+        CK(cudaMemsetAsync(h->d_rwhy, 0, why_bytes, h->stream));
+    }
+    int32_t* const rows[2] = {h->d_ridx, h->d_ridx + P};
+    RoundArgs ra;
+    ra.result = h->d_rout; ra.pod_round = h->d_ridx + 2 * P; ra.block_cnt = h->d_ridx + 3 * P;
+    ra.n_rounds = n_rounds; ra.survivors = h->h_rcount;
+    int n = n_pods, cur = 0;
+    for (int r = 0; r <= n_rounds && n > 0; r++) {
+        const bool last = r == n_rounds;
+        w.n_pods = n;
+        if (r > 0) { w.now0 = round_clock[r - 1]; w.const_clock = true; }
+        if ((rc = launch_solve(h, w, nodes, false, !last, false)) != NHD_OK) return rc;
+        ra.out = w.out; ra.pod_type = w.pod_type(); ra.pod_groups = w.pod_groups(); ra.row = r ? rows[cur] : nullptr;
+        ra.n_pods = n; ra.round = r;
+        ra.next_pod_type = last ? nullptr : reinterpret_cast<int32_t*>(h->d_rpods.p);
+        ra.next_now = last ? nullptr : reinterpret_cast<double*>(h->d_rpods.p + off_now);
+        ra.next_pod_groups = last || !w.n_names ? nullptr : reinterpret_cast<uint64_t*>(h->d_rpods.p + off_gm);
+        ra.next_row = last ? nullptr : rows[cur ^ 1];
+        ra.next_clock = last ? 0.0 : round_clock[r];
+        const int grid = (n + ROUND_THREADS - 1) / ROUND_THREADS;
+        if (!last) round_count_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(ra);
+        round_advance_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(ra);
+        CK(cudaGetLastError());
+        if (last) {
+            if (why_counts) {
+                if ((rc = explain_rows(h, w, nodes)) != NHD_OK) return rc;
+                round_why_kernel<<<(n * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, ra.row, n, h->d_rwhy);
+                CK(cudaGetLastError());
+            }
+            break;
+        }
+        CK(cudaStreamSynchronize(h->stream));
+        n = *h->h_rcount;
+        w.pod_arrays.swap(h->d_rpods);
+        cur ^= 1;
+    }
+    if (why_counts) CK(cudaMemcpyAsync(why_counts, h->d_rwhy, why_bytes, cudaMemcpyDeviceToHost, h->stream));
+    if (pod_round) CK(cudaMemcpyAsync(pod_round, ra.pod_round, P * 4, cudaMemcpyDeviceToHost, h->stream));
+    if ((rc = fetch_bindings(h, w, n_pods, out, h->d_rout)) != NHD_OK) return rc;
+    return why_counts && n > 0 ? explain_survivors(h, what) : NHD_OK;
+}
+
+extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                                  int32_t n_pods, const nhd_pod* pods, const double* now, nhd_binding* out,
+                                  uint32_t* why_counts)
+{
+    return plan_batch(h, "nhd_plan_batch", source, n_excluded, excluded, n_pods, pods, now, 0, nullptr, out, why_counts,
+                      nullptr);
+}
+
+extern "C" int32_t nhd_plan_batch_rounds(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                                         int32_t n_pods, const nhd_pod* pods, const double* now, int32_t n_rounds,
+                                         const double* round_clock, nhd_binding* out, uint32_t* why_counts,
+                                         int32_t* pod_round)
+{
+    return plan_batch(h, "nhd_plan_batch_rounds", source, n_excluded, excluded, n_pods, pods, now, n_rounds, round_clock,
+                      out, why_counts, pod_round);
 }
 
 /*
@@ -1514,7 +1620,7 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     }
 
     /* the candidate bitmaps of the call's pod types on the unchanged source records */
-    if ((rc = launch_solve(h, w, records, false, true)) != NHD_OK) return rc;
+    if ((rc = launch_solve(h, w, records, false, false, true)) != NHD_OK) return rc;
 
     ScenarioArgs sa;
     sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type(); sa.now = w.now();

@@ -22,8 +22,9 @@
  *                   parallel, from the snapshot core masks and per-socket prefix offsets
  *   commit_kernel   folds the batch into the node records
  * Outside a solve: explain_* (why a pod found no node), query_select / query_assign_kernel (where each pod
- * of a query would go on its own, nhd_query_batch), exclude_nodes_kernel (a plan's excluded nodes, nhd_plan_batch)
- * and scenario_plan_kernel (many independent small plans side by side, nhd_plan_scenarios).
+ * of a query would go on its own, nhd_query_batch), exclude_nodes_kernel (a plan's excluded nodes, nhd_plan_batch),
+ * round_count / round_advance_kernel (the unplaced pods of a plan's round handed to its next round,
+ * nhd_plan_batch_rounds) and scenario_plan_kernel (many independent small plans side by side, nhd_plan_scenarios).
  *
  * Device layout of the node array ("tiled AoSoA"): tiles of 32 nodes, 4 KB each:
  *     byte offset(node n, 16-byte chunk c) = (n / 32) * 4096 + c * 512 + (n % 32) * 16
@@ -2741,6 +2742,98 @@ __global__ void exclude_nodes_kernel(uint8_t* nodes, const int32_t* __restrict__
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     nodes[chunk_off(idx[i], 2) + REC_FLAGS_BYTE] |= (uint8_t)NHD_NODE_MAINTENANCE;
+}
+
+/* ------------------------------------------------------------------ rounds of a plan (nhd_plan_batch_rounds) */
+
+/*
+ * Not part of a solve: between two rounds of a plan.  Round r solved its pods (the pods no earlier round placed, in
+ * caller order) into out[]; the next round needs those of them that are still not NHD_PLACED, in the same order, at the
+ * next round's clock, and the caller needs every pod's last attempt in its own row.  Both happen on the device, so that
+ * the host reads one word per round (the survivor count: it sizes the next round's grids) and nothing else until the
+ * end.  Two launches of the same grid, one CTA per ROUND_THREADS pods: round_count_kernel leaves each CTA's survivor
+ * count, round_advance_kernel sums the counts of the CTAs before it (an order-preserving compaction: CTA prefix, warp
+ * prefix, ballot rank) and scatters.  No CTA waits for another.
+ */
+struct RoundArgs {
+    const nhd_binding* out;        /* the round's bindings, its pods in order */
+    const int32_t* pod_type;       /* the round's pod -> pod type */
+    const uint64_t* pod_groups;    /* ... -> node-group lists when the batch mixes them, else null */
+    const int32_t* row;            /* ... -> caller row; null in round 0 (pod i is row i) */
+    int n_pods, round, n_rounds;
+    nhd_binding* result;           /* [caller row] each pod's last attempt */
+    int32_t* pod_round;            /* [caller row] the round that placed the pod, or n_rounds */
+    int32_t* block_cnt;            /* [grid] survivors per CTA */
+    /* the next round's pod set (the other half of the double buffers); all null after the last round */
+    int32_t* next_pod_type;
+    double* next_now;
+    uint64_t* next_pod_groups;
+    int32_t* next_row;
+    double next_clock;
+    int32_t* survivors;            /* pods of the next round: one word the host reads (page-locked host memory) */
+};
+
+constexpr int ROUND_THREADS = 256;
+
+__global__ void __launch_bounds__(ROUND_THREADS) round_count_kernel(const RoundArgs a)
+{
+    __shared__ int32_t cnt;
+    const int tid = threadIdx.x, i = blockIdx.x * ROUND_THREADS + tid;
+    if (tid == 0) cnt = 0;
+    __syncthreads();
+    const unsigned m = __ballot_sync(0xFFFFFFFFu, i < a.n_pods && a.out[i].status != NHD_PLACED);
+    if ((tid & 31) == 0 && m) atomicAdd(&cnt, __popc(m));
+    __syncthreads();
+    if (tid == 0) a.block_cnt[blockIdx.x] = cnt;
+}
+
+__global__ void __launch_bounds__(ROUND_THREADS) round_advance_kernel(const RoundArgs a)
+{
+    __shared__ int32_t s_before[ROUND_THREADS / 32], s_mine[ROUND_THREADS / 32];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int i = blockIdx.x * ROUND_THREADS + tid;
+    const bool live = i < a.n_pods;
+    const int row = live ? (a.row ? a.row[i] : i) : 0;
+    const bool pending = live && a.out[i].status != NHD_PLACED;
+    if (live) a.pod_round[row] = pending ? a.n_rounds : a.round;
+    if (a.next_row) {
+        int32_t part = 0;                                            /* survivors of the CTAs before this one */
+        for (int b = tid; b < (int)blockIdx.x; b += ROUND_THREADS) part += a.block_cnt[b];
+        for (int off = 16; off; off >>= 1) part += __shfl_sync(0xFFFFFFFFu, part, lane ^ off);
+        const unsigned m = __ballot_sync(0xFFFFFFFFu, pending);
+        if (lane == 0) { s_before[wid] = part; s_mine[wid] = __popc(m); }
+        __syncthreads();
+        int32_t pos = 0, total = 0;
+        for (int k = 0; k < ROUND_THREADS / 32; k++) {
+            pos += s_before[k] + (k < wid ? s_mine[k] : 0);
+            total += s_before[k] + s_mine[k];
+        }
+        if (pending) {
+            pos += __popc(m & ((1u << lane) - 1u));
+            a.next_pod_type[pos] = a.pod_type[i];
+            a.next_now[pos] = a.next_clock;
+            if (a.next_pod_groups) a.next_pod_groups[pos] = a.pod_groups[i];
+            a.next_row[pos] = row;
+        }
+        if (blockIdx.x == gridDim.x - 1 && tid == 0) *a.survivors = total;
+    }
+    /* each binding to its caller row: 8 lanes per binding, a warp's 32 bindings in 8 steps of 512 contiguous bytes read */
+    const int p0 = blockIdx.x * ROUND_THREADS + wid * 32;
+    for (int k = 0; k < 8; k++) {
+        const int p = k * 4 + (lane >> 3), c = lane & 7;
+        const int r = __shfl_sync(0xFFFFFFFFu, row, p);
+        if (p0 + p < a.n_pods)
+            reinterpret_cast<uint4*>(a.result)[(size_t)r * 8 + c] = reinterpret_cast<const uint4*>(a.out)[(size_t)(p0 + p) * 8 + c];
+    }
+}
+
+/* the last round's reason rows (explain_kernel's counts, one row per pod of that round) to the callers' rows */
+__global__ void round_why_kernel(const uint32_t* __restrict__ rows, const int32_t* __restrict__ row, int n_pods,
+                                 uint32_t* __restrict__ out)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= n_pods * NHD_WHY_COUNT) return;
+    out[(size_t)row[k / NHD_WHY_COUNT] * NHD_WHY_COUNT + k % NHD_WHY_COUNT] = rows[k];
 }
 
 /* ------------------------------------------------------------------ independent plans (nhd_plan_scenarios) */

@@ -224,6 +224,29 @@ class Solver:
                                         counts.ctypes.data if explain else None))
         return (out, counts) if explain else out
 
+    def plan_batch_rounds(self, pods, now, round_clocks, source='mirror', exclude=(), explain=False):
+        """``plan_batch`` over several pending scans (``nhd_plan_batch_rounds``): after the dry run of the batch, at each
+        clock of ``round_clocks`` (never going down, none before a pod clock) the pods not placed yet are solved again
+        in order on the records the previous scan left, the nodes ``exclude`` in maintenance throughout.  Returns
+        ``(bindings, pod_round)``: each pod's last attempt and the round that placed it, or ``len(round_clocks)`` if
+        none did; ``explain=True``: ``(bindings, pod_round, counts)``, ``counts`` the per-reason node counts of the pods
+        whose last attempt found no node, at that attempt.  The same answer as ``plan_scenarios`` with this one scenario
+        and rounds, from the batch path: meant for one large pending set.  Nothing is placed."""
+        src = _source(source)
+        pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
+        now = np.ascontiguousarray(now, dtype='<f8')
+        assert len(pods) == len(now)
+        ex = np.ascontiguousarray(exclude, dtype='<i4').reshape(-1)
+        clocks = np.ascontiguousarray(round_clocks, dtype='<f8').reshape(-1)
+        out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
+        pod_round = np.zeros(len(pods), dtype='<i4')
+        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
+        self._ck(self._L.nhd_plan_batch_rounds(self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods),
+                                               pods.ctypes.data, now.ctypes.data, len(clocks),
+                                               clocks.ctypes.data if len(clocks) else None, out.ctypes.data,
+                                               counts.ctypes.data if explain else None, pod_round.ctypes.data))
+        return (out, pod_round, counts) if explain else (out, pod_round)
+
     def plan_scenarios(self, scenarios, source='mirror', explain=False):
         """Many independent dry runs in one call (``nhd_plan_scenarios_edited``).  ``scenarios``: a sequence of
         ``(exclude, pods, now[, lift[, edits]])``.  Returns one ``(code, pod, bindings)`` per scenario: ``code`` 0 and
