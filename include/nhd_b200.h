@@ -486,6 +486,58 @@ int32_t nhd_plan_batch_rounds(nhd_handle* h, int32_t source, int32_t n_excluded,
                               int32_t n_rounds, const double* round_clock,
                               nhd_binding* out, uint32_t* why_counts, int32_t* pod_round);
 
+/* One deployed pod given back between two scans of a forecast (ReleasePodResources, NHDScheduler.py:174-205), 88 bytes. */
+typedef struct nhd_release {
+    int32_t  node;                        /* node index in load order                                         */
+    int32_t  round;                       /* 1 .. n_rounds: lands after round - 1 and before round             */
+    double   clock;                       /* time.monotonic() at the release; Node.SetBusy stamps it (:205)   */
+    uint64_t cores[4];                    /* bit c: Node.cores[c].used = False (Node.py:590-619)              */
+    uint16_t gpus;                        /* bit i: Node.gpus[i].used = False                                 */
+    uint8_t  pad_[2];
+    int32_t  hugepages_gb;                /* added to free_hugepages_gb when > 0 (Node.py:634-635)            */
+    uint8_t  nic_pairings[NHD_MAX_NICS];  /* per Node.nics[i]: nic_core_pairing entries, each pods_used -= 1  */
+} nhd_release;
+
+/*
+ * nhd_plan_batch_rounds with running pods finishing between the scans: "these deployed pods end at about these times:
+ * when does each pending pod get in, and on which node?".  Rounds, pods, exclusions and clocks are those of
+ * nhd_plan_batch_rounds.  Before round r >= 1 the releases with round == r are applied, in array order, to the plan's
+ * own copy of the records: their core and GPU bits cleared, hugepages_gb added when > 0, the NIC counters lowered by
+ * nic_pairings, and busy_time = clock (a freed GPU node takes no GPU pod for min_busy_secs after the release).
+ * The records carry one in-use bit per NIC; the reference carries a signed counter, NodeNic.pods_used, which a release
+ * lowers once per RX/TX pairing (Node.py:621-631) and a claim raises once per distinct NIC (Node.py:644-646), so after a
+ * pod with two pairings on one NIC ends the counter sits at -1 and the next claim leaves the NIC free (Node.py:292).
+ * The call carries those counters for the nodes tracked[0..n_tracked): pods_used[t * NHD_MAX_NICS + i] is the counter
+ * of NIC i of node tracked[t] at plan start.  Every release's node must be tracked; a caller also tracks every node
+ * with a negative counter.  On a tracked node a NIC's in-use bit is count > 0 after every release, and every placement
+ * raises the count of each NIC in its claimed_nics by 1.
+ *   out, pod_round, why_counts   as for nhd_plan_batch_rounds: byte for byte what the reference's scheduler gives,
+ *                  every round solved one pod at a time on the records and counters, the releases played between rounds.
+ * The batch path differs from that only where a placement claims a tracked NIC whose count is <= -1 before the claim
+ * (the solve's commit sets a bit the reference leaves clear).  The call then cuts the round right after that pod: it
+ * restores the records the round's segment started from, solves that prefix again with its commit (the solve is
+ * deterministic), clears the bit from the count and solves the rest of the round as a new segment at the same clock.
+ * Each cut uses up one unit of negative count, so a call makes at most sum(|negative pods_used|) + sum(nic_pairings)
+ * cuts, each one more solve of its prefix and one host read.  Only the last round's last attempts are explained, each
+ * on the records its segment started from.
+ * With n_releases == 0 and n_tracked == 0 the call is nhd_plan_batch_rounds (tracked, pods_used and releases are not
+ * read).  Refused as nhd_plan_batch_rounds refuses, and, before anything is placed on the plan's copy, NHD_ERR_INVALID
+ * for: n_tracked or n_releases < 0 or their arrays NULL; a tracked node outside [0, n_nodes) or tracked twice; a
+ * release round outside [1, n_rounds]; release clocks that go down in array order, are not finite, lie before the
+ * clock of the round before theirs (before every now[] for round 1) or after their own round's clock; a release on an
+ * untracked node; and, checked on the device against the source records (one word read back), a tracked count whose
+ * sign disagrees with the NIC's in-use bit (> 0 exactly when set), a NIC at or beyond n_nics with a non-zero count, a
+ * core bit at or beyond the node's logical core count, a GPU bit at or beyond n_gpus, or a pairing on a NIC at or
+ * beyond n_nics.  Nothing is written that a caller can observe (the list of nhd_plan_batch), no collective is entered,
+ * and the call waits for the device before returning.
+ */
+int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                                int32_t n_pods, const nhd_pod* pods, const double* now,
+                                int32_t n_rounds, const double* round_clock,
+                                int32_t n_tracked, const int32_t* tracked, const int16_t* pods_used,
+                                int32_t n_releases, const nhd_release* releases,
+                                nhd_binding* out, uint32_t* why_counts, int32_t* pod_round);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

@@ -111,6 +111,7 @@ class DeviceCluster:
         self._last = None
         self.stubs = set()
         self.unsupported_nodes: Dict[str, str] = {}
+        self._nodes: Dict[str, object] = {}
 
     @property
     def layout(self):
@@ -156,6 +157,7 @@ class DeviceCluster:
         """Make the device copy equal to ``nodes``; ``dirty`` names the nodes the host changed since
         the last call."""
         names = list(nodes)
+        self._nodes = nodes
         min_busy = float(getattr(type(nodes[names[0]]), 'MIN_BUSY_SECS', 30.0)) if names else 30.0
         full = self._solver is None or names != self._names or min_busy != self._min_busy
         recs = idx = None
@@ -259,19 +261,74 @@ class DeviceCluster:
                   explain=explain)
 
     def forecast(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now, round_clocks: Sequence[float],
-                 source: str = 'mirror', exclude: Iterable[str] = (), explain: bool = False, packed: Sequence = None):
+                 source: str = 'mirror', exclude: Iterable[str] = (), explain: bool = False, packed: Sequence = None,
+                 releases: Sequence = None):
         """``plan`` over several pending scans (``Solver.plan_batch_rounds``): after the dry run at ``now``, at each
         clock of ``round_clocks`` the pods no earlier scan placed are retried in order on the cluster the earlier scans
         left, the nodes named in ``exclude`` in maintenance throughout.  Returns ``(bindings, pod_round)``: each pod's
         last attempt and the scan that placed it, or ``len(round_clocks)``; ``explain=True``: also the per-reason node
         counts of the pods whose last attempt found no node.  None when the solver in use cannot (a stand-in without
-        ``plan_batch_rounds``)."""
+        ``plan_batch_rounds``).
+        ``releases`` (``Solver.plan_batch_releases``): ``(node name, topology, clock)`` of deployed pods that end between
+        the scans, each given back as ``ReleasePodResources`` gives it back (``AddResourcesFromTopology``, then the node
+        busy from ``clock``) right before the first scan whose clock is not earlier than ``clock``; one after the last
+        scan changes nothing and is left out, one at or before ``now`` is a ValueError.  The nodes' signed NIC pod
+        counters are those of the synced ``Node`` objects; every node with a release or a negative counter is tracked.
+        None when the solver in use cannot (a stand-in without ``plan_batch_releases``)."""
+        if releases is not None:
+            fn = getattr(self._solver, 'plan_batch_releases', None)
+            if fn is None:
+                return None
+            idx = self._indices(exclude, 'exclude')
+            tracked, used, rels = self._releases(releases, float(now if np.isscalar(now) else np.max(now)), round_clocks)
+            return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), round_clocks, tracked, used,
+                      rels, source=source, exclude=idx, explain=explain)
         fn = getattr(self._solver, 'plan_batch_rounds', None)
         if fn is None:
             return None
         idx = self._indices(exclude, 'exclude')
         return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), round_clocks, source=source,
                   exclude=idx, explain=explain)
+
+    def _releases(self, releases: Sequence, now: float, round_clocks: Sequence[float]):
+        """``(tracked, pods_used, records)`` of ``forecast``'s releases: per release the core bits of the topology's
+        logical core ids, the GPU bits of its device ids and its pairings per NIC by MAC, as
+        ``Node.AddResourcesFromTopology`` walks them; the round from the round clocks; array order = clock order."""
+        clocks = [float(c) for c in round_clocks]
+        items = []
+        for name, top, clock in releases:
+            clock = float(clock)
+            if not clock > now:
+                raise ValueError(f'release on {name} at {clock} is not after the first scan ({now})')
+            rnd = next((r for r, c in enumerate(clocks, 1) if clock <= c), None)
+            if rnd is not None:
+                items.append((clock, rnd, name, top))
+        items.sort(key=lambda x: x[0])
+        rels = np.zeros(len(items), dtype=wire.RELEASE_DTYPE)
+        for k, (clock, rnd, name, top) in enumerate(items):
+            node = self._nodes[name]
+            rl = rels[k]
+            rl['node'], rl['round'], rl['clock'] = self._indices([name], 'release pods on')[0], rnd, clock
+            for c in node._topology_cores(top):
+                rl['cores'][c.core >> 6] |= np.uint64(1) << np.uint64(c.core & 63)
+            for pv in top.proc_groups:
+                for g in pv.group_gpus:
+                    dev = node.GetGPU(g.device_id)
+                    if dev is not None:
+                        rl['gpus'] |= 1 << node.gpus.index(dev)
+            for pair in top.nic_core_pairing:
+                nic = node.GetNIC(pair.mac)
+                if nic is not None:
+                    rl['nic_pairings'][node.nics.index(nic)] += 1
+            rl['hugepages_gb'] = max(int(top.hugepages_gb), 0)
+        names = set(items[k][2] for k in range(len(items)))
+        tracked = [i for i, n in enumerate(self._names)
+                   if n in names or any(x.pods_used < 0 for x in getattr(self._nodes[n], 'nics', ()))]
+        used = np.zeros((len(tracked), wire.MAX_NICS), dtype='<i2')
+        for t, i in enumerate(tracked):
+            for j, x in enumerate(self._nodes[self._names[i]].nics[:wire.MAX_NICS]):
+                used[t, j] = x.pods_used
+        return tracked, used, rels
 
     def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror', explain: bool = False):
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
@@ -938,7 +995,7 @@ class NHDScheduler:
         return result if reasons else [p for p, _ in result]
 
     def ForecastPending(self, scans: int, keys: Sequence = None, period: float = None, additions: Sequence = None,
-                        reasons: bool = False):
+                        reasons: bool = False, departures: Dict = None):
         """Which pending pods get in at a later scan, and which never do?  ``run()`` retries every pod still pending
         each ``idle_thresh x block_secs`` seconds, and a GPU node that took a pod less than ``MIN_BUSY_SECS`` earlier
         takes no GPU pod, so one scan places at most one GPU pod per node.  This plans ``scans`` pending scans in a row
@@ -954,9 +1011,35 @@ class NHDScheduler:
         ``{reason name: nodes}`` for each pod no scan placed that found no node at its last scan, at that scan's state.
         Names and reads as ``PlanExpansion``: only reads happen; ``pod_state``, the ``Node`` objects and the counters
         stay as they are.  One scenario without added nodes is one large batch and is solved by the batch path at every
-        scan (``DeviceCluster.forecast``); several scenarios, or added nodes, run side by side, one warp each."""
+        scan (``DeviceCluster.forecast``); several scenarios, or added nodes, run side by side, one warp each.
+        ``departures``: ``{(ns, name): seconds after the first scan}``, deployed pods expected to end by then.  Each is
+        given back as its delete would give it back (``ReleasePodResources``: what ``_release_target`` reads, the node
+        busy from the delete) before the first scan at or after it; a pod that would give nothing back is left out, as
+        the delete leaves it, and one after the last scan changes nothing.  A pod never annotated (its delete re-scans
+        every node), a departure that is also among ``keys``, an offset <= 0, and ``departures`` together with
+        ``additions`` are ValueErrors.  Releases need the batch path (``Solver.plan_batch_releases``)."""
+        rel = None
+        if departures is not None:
+            if additions is not None:
+                raise ValueError('departures are planned on the cluster as it is, not with additions')
+            if keys is None:
+                phase = self._service_pods()
+                keys = [k for k in phase if self._wanted(phase)(k)]
+            pending = {(k[0], k[1]) for k in keys}
+            rel = []
+            for (ns, name), offset in departures.items():
+                offset = float(offset)
+                if (ns, name) in pending:
+                    raise ValueError(f'pod {ns}.{name} is pending and cannot depart')
+                if not offset > 0.0:
+                    raise ValueError(f'departure of {ns}.{name} at {offset} s is not after the first scan')
+                target = self._release_target(name, ns)
+                if target is None:
+                    raise ValueError(f'pod {ns}.{name} was never annotated: its delete re-scans every node')
+                if target[0] is not None:
+                    rel.append((target[0], target[1], offset))
         result = self._grown_plans([[]] if additions is None else additions, keys, reasons,
-                                   self._scan_periods(scans, period))
+                                   self._scan_periods(scans, period), departures=rel)
         out = [(p, why) if reasons else p for p, why in result]
         return out[0] if additions is None else out
 
@@ -986,7 +1069,7 @@ class NHDScheduler:
         return [float(60 * 0.5 if period is None else period)] * (scans - 1)
 
     def _grown_plans(self, additions: Sequence[Sequence], keys: Sequence, reasons: bool, periods: Sequence[float],
-                     exclude: Sequence[str] = ()):
+                     exclude: Sequence[str] = (), departures: Sequence = None):
         """``PlanExpansion``'s plans, with a later scan after each of ``periods`` seconds: per scenario ``(placement,
         reasons)``, a placed pod mapped to its node name, or with ``periods`` (even an empty list) to ``(scan, node
         name)``.  ``periods`` None: one scan, through the call without rounds.  ``exclude``: nodes in maintenance
@@ -1016,14 +1099,27 @@ class NHDScheduler:
                 for p in periods:
                     clocks.append(clocks[-1] + float(p))
                 clocks = clocks[1:]
+            releases = None
+            if departures is not None:              # seconds after the first scan -> clocks (a scan's own when equal)
+                offs, releases = [], []
+                for p in periods:
+                    offs.append((offs[-1] if offs else 0.0) + float(p))
+                for node, top, off in departures:
+                    if offs and off <= offs[-1]:
+                        k = next(k for k, o in enumerate(offs) if off <= o)
+                        at = clocks[k] if off == offs[k] else max(now + off, clocks[k - 1] if k else now)
+                        releases.append((node, top, min(at, clocks[k])))
             todo = [(j, entries) for j in range(len(scens))]
             if clocks is not None and scens == [[]]:
                 # one scenario on the cluster as it is: one batch per scan (a pod beyond the tuple limits is dropped
                 # and the rest planned again, as _plan_prepared does)
                 res, ok, _ = self._without_refused(
                     lambda es: self.cluster.forecast([e.top for e in es], [e.groups for e in es], now, clocks,
-                                                     exclude=exclude, explain=reasons, packed=[e.rec for e in es]),
+                                                     exclude=exclude, explain=reasons, packed=[e.rec for e in es],
+                                                     releases=releases),
                     entries)
+                if releases is not None and res is None and ok:
+                    self._supported(None, 'forecast releases (no plan_batch_releases)')
                 if res is not None or not ok:
                     todo = []
                 if res is not None:

@@ -63,6 +63,7 @@ struct NcclApi {
 static NcclApi g_nccl;
 
 static_assert(offsetof(nhd_node_rec, flags) == 2 * 16 + REC_FLAGS_BYTE, "exclude_nodes_kernel's flags byte");
+static_assert(sizeof(nhd_release) == 88 && offsetof(nhd_release, nic_pairings) == 56, "nhd_release is 88 bytes");
 
 /* ------------------------------------------------------------------ buffers */
 
@@ -106,6 +107,7 @@ struct Workspace {
     /* the pod set */
     int n_pods = 0, n_types = 0, n_names = 0;
     int pod_cap = 0;                      /* pods the arrays are laid out for: n_pods as staged (a plan's later rounds hold fewer) */
+    int seg = 0;                          /* first pod of the solve: a plan with releases solves a round in segments */
     uint64_t names_used = 0;
     double now0 = 0.0;                    /* clock of the first pod (the filter's BUSY row) */
     bool const_clock = true;
@@ -127,12 +129,13 @@ struct Workspace {
     PinnedBuf<nhd_binding> h_out;         /* bounce buffer of fetch_bindings */
 
     size_t now_offset() const { return ((size_t)pod_cap * 4 + 15) & ~(size_t)15; }
-    const int32_t* pod_type() const { return reinterpret_cast<const int32_t*>(pod_arrays.p); }
-    const double* now() const { return reinterpret_cast<const double*>(pod_arrays.p + now_offset()); }
+    const int32_t* pod_type() const { return reinterpret_cast<const int32_t*>(pod_arrays.p) + seg; }
+    const double* now() const { return reinterpret_cast<const double*>(pod_arrays.p + now_offset()) + seg; }
     const uint64_t* pod_groups() const      /* per-pod node-group masks when the pods mix lists, else null */
     {
-        return n_names ? reinterpret_cast<const uint64_t*>(pod_arrays.p + now_offset() + (size_t)pod_cap * 8) : nullptr;
+        return n_names ? reinterpret_cast<const uint64_t*>(pod_arrays.p + now_offset() + (size_t)pod_cap * 8) + seg : nullptr;
     }
+    nhd_binding* bindings() const { return out.p + seg; }
 };
 
 /* ------------------------------------------------------------------ handle */
@@ -207,6 +210,11 @@ struct nhd_handle {
     DevBuf<nhd_binding> d_rout;
     DevBuf<uint32_t> d_rwhy;
     PinnedBuf<int32_t> h_rcount;
+    /* a plan's releases (nhd_plan_batch_releases): the records a segment started from, the releases, and counts |
+     * node -> tracked slot | release -> slot | releases by round and node | node starts | the check word */
+    DevBuf<uint8_t> d_pseg;
+    DevBuf<nhd_release> d_rels;
+    DevBuf<int32_t> d_rel;
     /* scenario plans: pod offsets | exclusion offsets | exclusions | edit offsets | edited nodes | lift indices | slot
      * nodes | the failed-mapping word, and one working record per slot followed by the edit records */
     DevBuf<int32_t> d_sidx;
@@ -758,6 +766,7 @@ static int32_t stage_pods(nhd_handle* h, Workspace& w, int n, const nhd_pod* pod
     CK(cudaSetDevice(h->params.device));
     const int T = (int)types.size();
     w.n_pods = w.pod_cap = n;
+    w.seg = 0;
     w.n_types = T;
     w.n_names = multi_group ? __builtin_popcountll(names_used) : 0;
     w.names_used = multi_group ? names_used : 0;
@@ -897,7 +906,7 @@ static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, b
         /* (the sweep's and the finishing kernels' record pointer is writable for commit_kernel) */
         uint8_t* const records = const_cast<uint8_t*>(nodes);
         SweepArgs sa;
-        sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type(); sa.now = w.now(); sa.out = w.out;
+        sa.nodes = records; sa.types = w.types; sa.pod_type = w.pod_type(); sa.now = w.now(); sa.out = w.bindings();
         sa.n_pods = w.n_pods; sa.n_types = T; sa.n_nodes = h->n_nodes; sa.words = W;
         sa.n_names = w.n_names; sa.names_used = w.names_used; sa.pod_groups = w.pod_groups();
         /* reserved_ (test knobs; every setting gives the same bindings): low byte 0 = default, 1 = the general one-warp
@@ -931,7 +940,7 @@ static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, b
         }
         CK(cudaGetLastError());
         FinishArgs fin;
-        fin.nodes = records; fin.types = w.types; fin.pod_type = w.pod_type(); fin.out = w.out;
+        fin.nodes = records; fin.types = w.types; fin.pod_type = w.pod_type(); fin.out = w.bindings();
         fin.dyn = w.dyn; fin.n_pods = w.n_pods;
         const int fthreads = 128, fgrid = (w.n_pods + fthreads - 1) / fthreads;
         resolve_kernel<<<(w.n_pods + 63) / 64, 64, 0, h->stream>>>(sa);
@@ -1062,7 +1071,7 @@ static int32_t explain_ready(nhd_handle* h)
 static int32_t explain_prepare(nhd_handle* h, const Workspace& w, int* n_failed)
 {
     const int N = h->n_nodes, P = w.n_pods;
-    const nhd_binding* out = w.out;
+    const nhd_binding* out = w.bindings();
     CK(h->d_xnode.grow(((size_t)3 * N + 2) * 4));
     CK(h->d_xpod.grow(((size_t)2 * P + 1) * 4));
     CK(h->d_xsmall.grow(16));
@@ -1104,7 +1113,7 @@ static int32_t explain_launch(nhd_handle* h, const Workspace& w, const uint8_t* 
     const int N = h->n_nodes, P = w.n_pods;
     if (n_failed == 0 || N == 0) return NHD_OK;
     ExplainArgs xa;
-    xa.snapshot = nodes; xa.types = w.types; xa.pod_type = w.pod_type(); xa.now = d_now ? d_now : w.now(); xa.out = w.out;
+    xa.snapshot = nodes; xa.types = w.types; xa.pod_type = w.pod_type(); xa.now = d_now ? d_now : w.now(); xa.out = w.bindings();
     xa.pod_groups = w.pod_groups();
     xa.node_start = h->d_xnode + N; xa.node_pods = h->d_xpod; xa.failed = h->d_xpod + P;
     xa.n_failed = (const int32_t*)h->d_xsmall.p;
@@ -1250,10 +1259,20 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
  * of the double-buffered pod arrays and every binding to its caller's row, and the host reads one word per round, the
  * next round's pod count.  Only the last round can leave a NO_CANDIDATE last attempt (an unplaced pod is retried in
  * every round), so only it is explained, on the records it started from: it runs no commit.
+ * With releases or tracked NIC counts (nhd_plan_batch_releases) release_kernel applies a round's releases to the copy
+ * before its solve, and a round is solved in segments while a cut is still possible (the negative count the call can
+ * hold, from its start and its releases so far, less the cuts made): each segment saves the records it starts from,
+ * solves and commits, and claim_cut_kernel leaves the first pod that claimed a tracked NIC at <= -1 in the second
+ * page-locked word.  On a cut the records are restored and the prefix up to that pod solved again with its commit; the
+ * rest of the round is the next segment, at the same clock (Workspace::seg).  claim_count_kernel then adds the
+ * segment's claims to the counts and clears the bits the counts leave at <= 0.  A last-round segment is explained on
+ * the records it started from.
  */
 static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32_t n_excluded, const int32_t* excluded,
                           int32_t n_pods, const nhd_pod* pods, const double* now, int32_t n_rounds,
-                          const double* round_clock, nhd_binding* out, uint32_t* why_counts, int32_t* pod_round)
+                          const double* round_clock, int32_t n_tracked, const int32_t* tracked, const int16_t* pods_used,
+                          int32_t n_releases, const nhd_release* releases, nhd_binding* out, uint32_t* why_counts,
+                          int32_t* pod_round)
 {
     if (!h || n_pods < 0 || n_excluded < 0 || (n_excluded > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)))
         return NHD_ERR_INVALID;
@@ -1266,9 +1285,94 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
     for (int i = 0; i < n_pods && n_rounds > 0; i++)         /* a monotonic clock never goes back */
         if (round_clock[0] < now[i])
             return fail(h, NHD_ERR_INVALID, "round clock 0 is earlier than the clock of pod %d", i);
+    if (n_tracked < 0 || n_releases < 0 || (n_tracked > 0 && (!tracked || !pods_used)) || (n_releases > 0 && !releases))
+        return fail(h, NHD_ERR_INVALID, "%d tracked nodes, %d releases", n_tracked, n_releases);
+    double t0 = -INFINITY;
+    for (int i = 0; i < n_pods; i++) t0 = std::max(t0, now[i]);
+    for (int k = 0; k < n_releases; k++) {
+        const nhd_release& rl = releases[k];
+        if (rl.round < 1 || rl.round > n_rounds)
+            return fail(h, NHD_ERR_INVALID, "release %d: round %d outside [1, %d]", k, rl.round, n_rounds);
+        if (!std::isfinite(rl.clock)) return fail(h, NHD_ERR_INVALID, "release %d: clock is not finite", k);
+        if (k > 0 && rl.clock < releases[k - 1].clock) return fail(h, NHD_ERR_INVALID, "release clocks go down at %d", k);
+        if (rl.clock < (rl.round > 1 ? round_clock[rl.round - 2] : t0) || rl.clock > round_clock[rl.round - 1])
+            return fail(h, NHD_ERR_INVALID, "release %d: clock outside the gap before round %d", k, rl.round);
+    }
     const uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
     if (rc != NHD_OK) return rc;
+    const bool track = n_tracked > 0 || n_releases > 0;
+
+    /* the tracked nodes' slots, the releases grouped by round and node (array order kept), the counts; the checks that
+     * need the records run on the device */
+    const int N = h->n_nodes, T = n_tracked, R = n_releases;
+    std::vector<int32_t> rel_area;
+    std::vector<int> group_first(n_rounds + 2, 0);
+    long long neg0 = 0;
+    std::vector<long long> pairs_by_round(n_rounds + 1, 0);
+    size_t off_slot = 0, off_rslot = 0, off_nrel = 0, off_nstart = 0, off_bad = 0;
+    if (track) {
+        off_slot = (size_t)T * NHD_MAX_NICS; off_rslot = off_slot + N; off_nrel = off_rslot + R; off_nstart = off_nrel + R;
+        rel_area.assign(off_nstart, 0);
+        for (int t = 0; t < T; t++)
+            for (int i = 0; i < NHD_MAX_NICS; i++) {
+                const int c = pods_used[(size_t)t * NHD_MAX_NICS + i];
+                rel_area[(size_t)t * NHD_MAX_NICS + i] = c;
+                neg0 += c < 0 ? -c : 0;
+            }
+        int32_t* slot = rel_area.data() + off_slot;
+        for (int n = 0; n < N; n++) slot[n] = -1;
+        for (int t = 0; t < T; t++) {
+            const int32_t n = tracked[t];
+            if (n < 0 || n >= N) return fail(h, NHD_ERR_INVALID, "tracked node %d outside the %d loaded nodes", n, N);
+            if (slot[n] >= 0) return fail(h, NHD_ERR_INVALID, "node %d tracked twice", n);
+            slot[n] = t;
+        }
+        std::vector<int32_t> order((size_t)R);
+        for (int k = 0; k < R; k++) {
+            const int32_t n = releases[k].node;
+            if (n < 0 || n >= N || slot[n] < 0) return fail(h, NHD_ERR_INVALID, "release %d: node %d is not tracked", k, n);
+            rel_area[off_rslot + k] = slot[n];
+            order[k] = k;
+            for (int i = 0; i < NHD_MAX_NICS; i++) pairs_by_round[releases[k].round] += releases[k].nic_pairings[i];
+        }
+        std::stable_sort(order.begin(), order.end(), [&](int32_t a, int32_t b) {
+            return std::make_pair(releases[a].round, slot[releases[a].node]) < std::make_pair(releases[b].round, slot[releases[b].node]);
+        });
+        for (int k = 0; k < R; k++) {
+            rel_area[off_nrel + k] = order[k];
+            const nhd_release& rl = releases[order[k]];
+            if (k == 0 || rl.round != releases[order[k - 1]].round || rl.node != releases[order[k - 1]].node) {
+                group_first[rl.round + 1]++;
+                rel_area.push_back(k);
+            }
+        }
+        rel_area.push_back(R);
+        for (int r = 1; r <= n_rounds + 1; r++) group_first[r] += group_first[r - 1];
+        off_bad = rel_area.size();
+        rel_area.push_back(0x7FFFFFFF);
+        CK(cudaSetDevice(h->params.device));
+        CK(h->d_rel.grow(rel_area.size() * 4));
+        CK(h->d_rels.grow((size_t)std::max(R, 1) * sizeof(nhd_release)));
+        CK(h->d_pidx.grow((size_t)std::max(T, 1) * (4 + NHD_MAX_NICS * 2)));
+        CK(cudaMemcpyAsync(h->d_rel, rel_area.data(), rel_area.size() * 4, cudaMemcpyHostToDevice, h->stream));
+        if (R) CK(cudaMemcpyAsync(h->d_rels, releases, (size_t)R * sizeof(nhd_release), cudaMemcpyHostToDevice, h->stream));
+        if (T) {
+            CK(cudaMemcpyAsync(h->d_pidx, tracked, (size_t)T * 4, cudaMemcpyHostToDevice, h->stream));
+            CK(cudaMemcpyAsync(h->d_pidx + T, pods_used, (size_t)T * NHD_MAX_NICS * 2, cudaMemcpyHostToDevice, h->stream));
+        }
+        release_check_kernel<<<(R + T + 255) / 256, 256, 0, h->stream>>>(records, h->d_rels, R, h->d_pidx,
+                                                                          reinterpret_cast<const int16_t*>(h->d_pidx + T), T,
+                                                                          h->d_rel + off_bad);
+        CK(cudaGetLastError());
+        int32_t bad = 0;
+        CK(cudaMemcpyAsync(&bad, h->d_rel + off_bad, 4, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+        if (bad < R)
+            return fail(h, NHD_ERR_INVALID, "release %d: a core, GPU or NIC beyond node %d's own", bad, releases[bad].node);
+        if (bad != 0x7FFFFFFF)
+            return fail(h, NHD_ERR_INVALID, "tracked node %d: pods_used disagrees with its NIC bits", tracked[bad - R]);
+    }
 
     /* the excluded nodes, each once; the tuple limits are judged as the equivalent solve would, on the largest NUMA
      * count among the nodes the filter could accept once they are in maintenance */
@@ -1294,7 +1398,7 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
     Workspace& w = h->scratch;
     if ((rc = stage_pods(h, w, n_pods, pods, now, max_numa)) != NHD_OK) return rc;
     const uint8_t* nodes = records;
-    if (!ex.empty() || n_rounds > 0) {
+    if (!ex.empty() || n_rounds > 0 || track) {
         CK(h->d_pnodes.grow(h->nodes_bytes));
         CK(cudaMemcpyAsync(h->d_pnodes, records, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
         nodes = h->d_pnodes;
@@ -1305,7 +1409,7 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
         exclude_nodes_kernel<<<(unsigned)((ex.size() + 255) / 256), 256, 0, h->stream>>>(h->d_pnodes, h->d_pidx, (int)ex.size());
         CK(cudaGetLastError());
     }
-    if (n_rounds == 0) {
+    if (n_rounds == 0 && !track) {
         if (pod_round) memset(pod_round, 0, (size_t)n_pods * 4);
         if ((rc = launch_solve(h, w, nodes, false, false, false)) != NHD_OK) return rc;
         if (why_counts && (rc = explain_counts(h, w, nodes, why_counts, what)) != NHD_OK) return rc;
@@ -1317,12 +1421,23 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
     CK(h->d_rpods.grow(off_gm + (w.n_names ? P * 8 : 0)));
     CK(h->d_ridx.grow((3 * P + grid0) * 4));
     CK(h->d_rout.grow(P * sizeof(nhd_binding)));
-    CK(h->h_rcount.grow(4));
+    CK(h->h_rcount.grow(8));
     if (why_counts) {
         CK(h->d_rwhy.grow(why_bytes));
         CK(cudaMemsetAsync(h->d_rwhy, 0, why_bytes, h->stream));
     }
     int32_t* const rows[2] = {h->d_ridx, h->d_ridx + P};
+    if (track) {
+        /* round 0's caller rows are the pods' own (its reason rows are scattered per segment) */
+        std::vector<int32_t> iota(P);
+        for (size_t i = 0; i < P; i++) iota[i] = (int32_t)i;
+        CK(cudaMemcpyAsync(rows[0], iota.data(), P * 4, cudaMemcpyHostToDevice, h->stream));
+        CK(h->d_pseg.grow(h->nodes_bytes));
+    }
+    int32_t* const d_count = h->d_rel;
+    const int32_t* const d_slot = h->d_rel + off_slot;
+    uint8_t* const pnodes = h->d_pnodes;
+    long long cut_room = neg0;                /* negative count the plan's copy may hold: an upper bound on cuts */
     RoundArgs ra;
     ra.result = h->d_rout; ra.pod_round = h->d_ridx + 2 * P; ra.block_cnt = h->d_ridx + 3 * P;
     ra.n_rounds = n_rounds; ra.survivors = h->h_rcount;
@@ -1331,8 +1446,74 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
         const bool last = r == n_rounds;
         w.n_pods = n;
         if (r > 0) { w.now0 = round_clock[r - 1]; w.const_clock = true; }
-        if ((rc = launch_solve(h, w, nodes, false, !last, false)) != NHD_OK) return rc;
-        ra.out = w.out; ra.pod_type = w.pod_type(); ra.pod_groups = w.pod_groups(); ra.row = r ? rows[cur] : nullptr;
+        int32_t* const row = r || track ? rows[cur] : nullptr;
+        if (!track) {
+            if ((rc = launch_solve(h, w, nodes, false, !last, false)) != NHD_OK) return rc;
+        } else {
+            const int groups = group_first[r + 1] - group_first[r];
+            if (groups > 0) {
+                ReleaseArgs rla;
+                rla.nodes = pnodes; rla.rel = h->d_rels; rla.rel_slot = h->d_rel + off_rslot;
+                rla.node_start = h->d_rel + off_nstart + group_first[r]; rla.node_rel = h->d_rel + off_nrel;
+                rla.n = groups; rla.count = d_count;
+                release_kernel<<<(groups + 127) / 128, 128, 0, h->stream>>>(rla);
+                CK(cudaGetLastError());
+            }
+            cut_room += pairs_by_round[r];
+            for (int seg = 0; seg < n;) {
+                w.seg = seg;
+                w.n_pods = n - seg;
+                if (r == 0) w.now0 = now[seg];
+                const bool may_cut = cut_room > 0;
+                const bool explain = last && why_counts;
+                if (!may_cut) {
+                    /* no claim can meet a negative count: the rest of the round is one segment, as without releases */
+                    const int m = w.n_pods;
+                    nhd_binding* const b = w.bindings();
+                    if ((rc = launch_solve(h, w, nodes, false, !last, false)) != NHD_OK) return rc;
+                    if (!last) {
+                        claim_count_kernel<<<(m + 127) / 128, 128, 0, h->stream>>>(b, m, d_slot, d_count, pnodes);
+                        CK(cudaGetLastError());
+                    }
+                    if (explain) {
+                        if ((rc = explain_rows(h, w, nodes)) != NHD_OK) return rc;
+                        round_why_kernel<<<(m * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, row + seg, m,
+                                                                                                 h->d_rwhy);
+                        CK(cudaGetLastError());
+                    }
+                    break;
+                }
+                nhd_binding* const b = w.bindings();
+                int32_t* const cut_word = h->h_rcount + 1;
+                uint8_t* const seg_nodes = h->d_pseg;
+                CK(cudaMemcpyAsync(seg_nodes, pnodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
+                if ((rc = launch_solve(h, w, nodes, false, true, false)) != NHD_OK) return rc;
+                int m = w.n_pods;
+                claim_cut_kernel<<<1, CUT_THREADS, 0, h->stream>>>(b, m, d_slot, d_count, cut_word);
+                CK(cudaGetLastError());
+                CK(cudaStreamSynchronize(h->stream));
+                const int cut = *cut_word;
+                if (cut >= 0) {
+                    CK(cudaMemcpyAsync(pnodes, seg_nodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
+                    w.n_pods = m = cut + 1;
+                    if ((rc = launch_solve(h, w, nodes, false, true, false)) != NHD_OK) return rc;
+                    cut_room--;
+                }
+                claim_count_kernel<<<(m + 127) / 128, 128, 0, h->stream>>>(b, m, d_slot, d_count, pnodes);
+                CK(cudaGetLastError());
+                if (explain) {
+                    if ((rc = explain_rows(h, w, seg_nodes)) != NHD_OK) return rc;
+                    round_why_kernel<<<(m * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, row + seg, m,
+                                                                                             h->d_rwhy);
+                    CK(cudaGetLastError());
+                    if ((rc = explain_survivors(h, what)) != NHD_OK) return rc;
+                }
+                seg += m;
+            }
+            w.seg = 0;
+            w.n_pods = n;
+        }
+        ra.out = w.out; ra.pod_type = w.pod_type(); ra.pod_groups = w.pod_groups(); ra.row = row;
         ra.n_pods = n; ra.round = r;
         ra.next_pod_type = last ? nullptr : reinterpret_cast<int32_t*>(h->d_rpods.p);
         ra.next_now = last ? nullptr : reinterpret_cast<double*>(h->d_rpods.p + off_now);
@@ -1344,7 +1525,7 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
         round_advance_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(ra);
         CK(cudaGetLastError());
         if (last) {
-            if (why_counts) {
+            if (why_counts && !track) {
                 if ((rc = explain_rows(h, w, nodes)) != NHD_OK) return rc;
                 round_why_kernel<<<(n * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, ra.row, n, h->d_rwhy);
                 CK(cudaGetLastError());
@@ -1366,8 +1547,8 @@ extern "C" int32_t nhd_plan_batch(nhd_handle* h, int32_t source, int32_t n_exclu
                                   int32_t n_pods, const nhd_pod* pods, const double* now, nhd_binding* out,
                                   uint32_t* why_counts)
 {
-    return plan_batch(h, "nhd_plan_batch", source, n_excluded, excluded, n_pods, pods, now, 0, nullptr, out, why_counts,
-                      nullptr);
+    return plan_batch(h, "nhd_plan_batch", source, n_excluded, excluded, n_pods, pods, now, 0, nullptr, 0, nullptr,
+                      nullptr, 0, nullptr, out, why_counts, nullptr);
 }
 
 extern "C" int32_t nhd_plan_batch_rounds(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
@@ -1376,7 +1557,17 @@ extern "C" int32_t nhd_plan_batch_rounds(nhd_handle* h, int32_t source, int32_t 
                                          int32_t* pod_round)
 {
     return plan_batch(h, "nhd_plan_batch_rounds", source, n_excluded, excluded, n_pods, pods, now, n_rounds, round_clock,
-                      out, why_counts, pod_round);
+                      0, nullptr, nullptr, 0, nullptr, out, why_counts, pod_round);
+}
+
+extern "C" int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                                           int32_t n_pods, const nhd_pod* pods, const double* now, int32_t n_rounds,
+                                           const double* round_clock, int32_t n_tracked, const int32_t* tracked,
+                                           const int16_t* pods_used, int32_t n_releases, const nhd_release* releases,
+                                           nhd_binding* out, uint32_t* why_counts, int32_t* pod_round)
+{
+    return plan_batch(h, "nhd_plan_batch_releases", source, n_excluded, excluded, n_pods, pods, now, n_rounds,
+                      round_clock, n_tracked, tracked, pods_used, n_releases, releases, out, why_counts, pod_round);
 }
 
 /*

@@ -24,7 +24,8 @@
  * Outside a solve: explain_* (why a pod found no node), query_select / query_assign_kernel (where each pod
  * of a query would go on its own, nhd_query_batch), exclude_nodes_kernel (a plan's excluded nodes, nhd_plan_batch),
  * round_count / round_advance_kernel (the unplaced pods of a plan's round handed to its next round,
- * nhd_plan_batch_rounds) and scenario_plan_kernel (many independent small plans side by side, nhd_plan_scenarios).
+ * nhd_plan_batch_rounds), release_kernel / release_check_kernel / claim_cut_kernel / claim_count_kernel (deployed pods
+ * ending between a plan's rounds and the signed NIC counters, nhd_plan_batch_releases) and scenario_plan_kernel (many independent small plans side by side, nhd_plan_scenarios).
  *
  * Device layout of the node array ("tiled AoSoA"): tiles of 32 nodes, 4 KB each:
  *     byte offset(node n, 16-byte chunk c) = (n / 32) * 4096 + c * 512 + (n % 32) * 16
@@ -2834,6 +2835,138 @@ __global__ void round_why_kernel(const uint32_t* __restrict__ rows, const int32_
     const int k = blockIdx.x * blockDim.x + threadIdx.x;
     if (k >= n_pods * NHD_WHY_COUNT) return;
     out[(size_t)row[k / NHD_WHY_COUNT] * NHD_WHY_COUNT + k % NHD_WHY_COUNT] = rows[k];
+}
+
+/* ------------------------------------------------------------------ releases between rounds (nhd_plan_batch_releases) */
+
+/*
+ * Not part of a solve either.  The reference counts a NIC's pods (NodeNic.pods_used, signed: a release lowers it once
+ * per RX/TX pairing, a claim raises it once per NIC), the records hold one bit per NIC.  On the tracked nodes the plan
+ * keeps the counts (count[slot * NHD_MAX_NICS + nic], slot[node] = the node's tracked slot or -1) and derives the bit
+ * from them: bit = count > 0.
+ */
+struct ReleaseArgs {
+    uint8_t* nodes;                /* the plan's copy of the records (tiled) */
+    const nhd_release* rel;        /* the call's releases */
+    const int32_t* rel_slot;       /* [release] its node's tracked slot */
+    const int32_t* node_start;     /* [k + 1] CSR of this round: releases node_rel[node_start[k] .. node_start[k+1]) */
+    const int32_t* node_rel;       /* ... release indices, array order within a node */
+    int n;                         /* tracked nodes with releases in this round */
+    int32_t* count;                /* [n_tracked][NHD_MAX_NICS] */
+};
+
+/* one thread per tracked node with releases in the round: apply them in array order (AddResourcesFromTopology +
+ * SetBusy, NHDScheduler.py:201-205), then rewrite the node's NIC bits from its counts */
+__global__ void release_kernel(const ReleaseArgs a)
+{
+    const int k = blockIdx.x * blockDim.x + threadIdx.x;
+    if (k >= a.n) return;
+    const int first = a.node_start[k], last = a.node_start[k + 1];
+    const int node = a.rel[a.node_rel[first]].node, slot = a.rel_slot[a.node_rel[first]];
+    uint64_t used[4];
+    for (int w = 0; w < 4; w++) used[w] = *reinterpret_cast<const uint64_t*>(a.nodes + chunk_off(node, w >> 1) + (w & 1) * 8);
+    uint8_t* c2 = a.nodes + chunk_off(node, 2);
+    uint16_t gpu_used = *reinterpret_cast<const uint16_t*>(c2);
+    const int n_nics = c2[3];
+    int32_t huge = *reinterpret_cast<const int32_t*>(c2 + 8);
+    double busy = 0.0;
+    int32_t* cnt = a.count + (size_t)slot * NHD_MAX_NICS;
+    for (int j = first; j < last; j++) {
+        const nhd_release& r = a.rel[a.node_rel[j]];
+        for (int w = 0; w < 4; w++) used[w] &= ~r.cores[w];
+        gpu_used &= (uint16_t)~r.gpus;
+        if (r.hugepages_gb > 0) huge += r.hugepages_gb;
+        for (int i = 0; i < n_nics; i++) cnt[i] -= r.nic_pairings[i];
+        busy = r.clock;
+    }
+    uint32_t inuse = 0;
+    for (int i = 0; i < n_nics; i++) inuse |= (cnt[i] > 0 ? 1u : 0u) << i;
+    for (int w = 0; w < 4; w++) *reinterpret_cast<uint64_t*>(a.nodes + chunk_off(node, w >> 1) + (w & 1) * 8) = used[w];
+    *reinterpret_cast<uint16_t*>(c2) = gpu_used;
+    *reinterpret_cast<uint32_t*>(c2 + 4) = inuse;
+    *reinterpret_cast<int32_t*>(c2 + 8) = huge;
+    *reinterpret_cast<double*>(a.nodes + chunk_off(node, 3)) = busy;
+}
+
+/*
+ * The checks of a release call that need the records, before anything runs: thread i < n_rel checks release i (core
+ * bits below the logical core count, GPU bits below n_gpus, pairings on NICs below n_nics), thread n_rel + t tracked
+ * node t (count > 0 exactly where the bit is set, no count beyond n_nics).  *bad = the lowest failing thread, or
+ * untouched (0x7FFFFFFF).
+ */
+__global__ void release_check_kernel(const uint8_t* __restrict__ nodes, const nhd_release* __restrict__ rel, int n_rel,
+                                     const int32_t* __restrict__ tracked, const int16_t* __restrict__ count0,
+                                     int n_tracked, int32_t* bad)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_rel + n_tracked) return;
+    const int node = i < n_rel ? rel[i].node : tracked[i - n_rel];
+    const uint4 q = *reinterpret_cast<const uint4*>(nodes + chunk_off(node, 2));
+    const int n_gpus = (q.x >> 16) & 0xFF, n_nics = q.x >> 24, lcores = (q.w >> 16) << (((q.w >> 8) & NHD_NODE_SMT) ? 1 : 0);
+    const uint32_t inuse = q.y;
+    bool ok = true;
+    if (i < n_rel) {
+        const nhd_release& r = rel[i];
+        for (int w = 0; w < 4; w++) {
+            const int lo = w * 64;
+            const uint64_t allowed = lcores >= lo + 64 ? ~0ULL : lcores <= lo ? 0ULL : (1ULL << (lcores - lo)) - 1ULL;
+            ok &= (r.cores[w] & ~allowed) == 0;
+        }
+        ok &= (r.gpus >> n_gpus) == 0;
+        for (int k = n_nics; k < NHD_MAX_NICS; k++) ok &= r.nic_pairings[k] == 0;
+    } else {
+        const int16_t* c = count0 + (size_t)(i - n_rel) * NHD_MAX_NICS;
+        for (int k = 0; k < NHD_MAX_NICS; k++)
+            ok &= k < n_nics ? ((c[k] > 0) == (((inuse >> k) & 1u) != 0)) : c[k] == 0;
+    }
+    if (!ok) atomicMin(bad, i);
+}
+
+/*
+ * After a segment's solve with its commit: the first of its pods (lowest index) whose placement claims a tracked NIC
+ * whose count is <= -1 (the commit set that NIC's bit; the reference's count reaches at most 0, so it reads the NIC as
+ * free).  One CTA; *cut (page-locked host word) = that index or -1.
+ */
+constexpr int CUT_THREADS = 1024;
+
+__global__ void __launch_bounds__(CUT_THREADS) claim_cut_kernel(const nhd_binding* __restrict__ out, int n_pods,
+                                                                const int32_t* __restrict__ slot,
+                                                                const int32_t* __restrict__ count, int32_t* cut)
+{
+    __shared__ int32_t first;
+    if (threadIdx.x == 0) first = 0x7FFFFFFF;
+    __syncthreads();
+    for (int i = threadIdx.x; i < n_pods; i += CUT_THREADS) {
+        if (out[i].status != NHD_PLACED) continue;
+        const int s = slot[out[i].node];
+        if (s < 0) continue;
+        const int nc = out[i].n_claimed;
+        for (int j = 0; j < nc; j++)
+            if (count[(size_t)s * NHD_MAX_NICS + out[i].claimed_nics[j]] <= -1) { atomicMin(&first, i); break; }
+    }
+    __syncthreads();
+    if (threadIdx.x == 0) *cut = first == 0x7FFFFFFF ? -1 : first;
+}
+
+/*
+ * The count pass after a segment's last commit: every placement on a tracked node raises the counts of its claimed
+ * NICs (ClaimPodNICResources, Node.py:644-646), and a NIC whose count is still <= 0 gets its bit cleared (the commit
+ * set it).  A segment ends at its first claim of a NIC at <= -1, so no two of its pods claim one NIC; the atomics keep
+ * the pass exact regardless.
+ */
+__global__ void claim_count_kernel(const nhd_binding* __restrict__ out, int n_pods, const int32_t* __restrict__ slot,
+                                   int32_t* count, uint8_t* nodes)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i >= n_pods || out[i].status != NHD_PLACED) return;
+    const int node = out[i].node, s = slot[node];
+    if (s < 0) return;
+    const int nc = out[i].n_claimed;
+    for (int j = 0; j < nc; j++) {
+        const int nic = out[i].claimed_nics[j];
+        if (atomicAdd(&count[(size_t)s * NHD_MAX_NICS + nic], 1) + 1 <= 0)
+            atomicAnd(reinterpret_cast<unsigned int*>(nodes + chunk_off(node, 2) + 4), ~(1u << nic));
+    }
 }
 
 /* ------------------------------------------------------------------ independent plans (nhd_plan_scenarios) */

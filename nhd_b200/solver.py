@@ -247,6 +247,34 @@ class Solver:
                                                counts.ctypes.data if explain else None, pod_round.ctypes.data))
         return (out, pod_round, counts) if explain else (out, pod_round)
 
+    def plan_batch_releases(self, pods, now, round_clocks, tracked, pods_used, releases, source='mirror', exclude=(),
+                            explain=False):
+        """``plan_batch_rounds`` with deployed pods ending between the scans (``nhd_plan_batch_releases``).
+        ``releases``: ``wire.RELEASE_DTYPE`` records, each applied before its ``round`` (1 .. ``len(round_clocks)``),
+        in array order, clocks never going down.  ``tracked``: the node indices whose signed NIC pod counters the plan
+        carries, every released node among them; ``pods_used``: ``(len(tracked), MAX_NICS)`` counters at plan start.
+        Returns what ``plan_batch_rounds`` returns.  Nothing is placed."""
+        src = _source(source)
+        pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
+        now = np.ascontiguousarray(now, dtype='<f8')
+        assert len(pods) == len(now)
+        ex = np.ascontiguousarray(exclude, dtype='<i4').reshape(-1)
+        clocks = np.ascontiguousarray(round_clocks, dtype='<f8').reshape(-1)
+        tr = np.ascontiguousarray(tracked, dtype='<i4').reshape(-1)
+        used = np.ascontiguousarray(pods_used, dtype='<i2').reshape(len(tr), wire.MAX_NICS)
+        rel = np.ascontiguousarray(releases, dtype=wire.RELEASE_DTYPE).reshape(-1)
+        out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
+        pod_round = np.zeros(len(pods), dtype='<i4')
+        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
+        self._ck(self._L.nhd_plan_batch_releases(self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods),
+                                                 pods.ctypes.data, now.ctypes.data, len(clocks),
+                                                 clocks.ctypes.data if len(clocks) else None, len(tr),
+                                                 tr.ctypes.data if len(tr) else None,
+                                                 used.ctypes.data if len(tr) else None, len(rel),
+                                                 rel.ctypes.data if len(rel) else None, out.ctypes.data,
+                                                 counts.ctypes.data if explain else None, pod_round.ctypes.data))
+        return (out, pod_round, counts) if explain else (out, pod_round)
+
     def plan_scenarios(self, scenarios, source='mirror', explain=False):
         """Many independent dry runs in one call (``nhd_plan_scenarios_edited``).  ``scenarios``: a sequence of
         ``(exclude, pods, now[, lift[, edits]])``.  Returns one ``(code, pod, bindings)`` per scenario: ``code`` 0 and

@@ -74,6 +74,13 @@ BINDING_DTYPE = np.dtype([
 ], align=False)
 assert BINDING_DTYPE.itemsize == 128
 
+# nhd_release: one deployed pod given back between two scans of a forecast (nhd_plan_batch_releases)
+RELEASE_DTYPE = np.dtype([
+    ('node', '<i4'), ('round', '<i4'), ('clock', '<f8'), ('cores', '<u8', (4,)), ('gpus', '<u2'), ('pad_', 'u1', (2,)),
+    ('hugepages_gb', '<i4'), ('nic_pairings', 'u1', (MAX_NICS,)),
+], align=False)
+assert RELEASE_DTYPE.itemsize == 88
+
 # nhd_node_aux: what nhd_ingest_node reads from the labels besides the packed record
 NODE_AUX_DTYPE = np.dtype([
     ('data_vlan', '<i4'), ('res_hugepages_gb', '<i4'), ('n_reserved_cores', '<i4'), ('gw_label', '<i4'),
