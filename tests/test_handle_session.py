@@ -8,10 +8,13 @@ pinned here: a seeded session generator and a runner that drives one ``Solver`` 
 call, compares it
 
   * with the oracle (``oracle.binding.solve``, ``test_query.oracle_alone``, ``test_plan.oracle_plan``,
-    ``test_defrag.oracle_defrag``, ``tests/explain_oracle.py``), byte for byte;
+    ``test_defrag.oracle_defrag``, ``tests/explain_oracle.py``; for the forecasts ``test_plan_reasons.oracle_explained``,
+    ``test_expand.oracle_grown``, ``test_forecast.oracle_rounds``, ``test_forecast_releases.oracle_releases``), byte
+    for byte;
   * with a fresh handle in the same sweep mode, loaded with the records the call reads (a snapshot source is asked of
     the fresh handle as its mirror), refusals included: the same code, naming the same pod;
-  * with the runner's own model of the records, the snapshot and the legality rules (DESIGN §8.6 - §8.10).
+  * with the runner's own model of the records, the snapshot, the deployed pods and the legality rules (DESIGN §8.6 -
+    §8.15), refusals in the order the library checks them.
 
 A session is plain data, a list of ``(op, args)``; ``make_session(seed, ...)`` rebuilds it from its seed, so a failure
 names ``seed / step / op`` and replays alone.  ``tools/session_fuzz.py`` runs the same generator over many seeds."""
@@ -71,6 +74,65 @@ def pod_refusal(pods, now, k):
         if not tuple_ok(k, int(pods[i]['n_groups'])):
             return wire.ERR_UNSUPPORTED, i
     return None
+
+
+def scenario_call_refusal(scs, src_ref, n_classes):
+    """(code, pod, rule) refusing a whole scenario call, in the order nhd_api.cu's plan_scenarios checks: every
+    scenario's first round clock against its pods' clocks (before the source is read), the source, then the added
+    records (a NIC speed class the handle lacks).  ``scs``: 7-tuples."""
+    for ex, pods, now, lift, edits, adds, rounds in scs:
+        if rounds is not None and len(rounds):
+            late = np.flatnonzero(np.asarray(now) > rounds[0])
+            if len(late):
+                return wire.ERR_INVALID, int(late[0]), 'round clock'
+    if src_ref is not None:
+        return src_ref + ('source',)
+    for sc in scs:
+        if sc[5] is not None:
+            for r in np.asarray(sc[5][1], dtype=wire.NODE_DTYPE):
+                spd = int(r['nic_speed'][0]) | int(r['nic_speed'][1]) << 64
+                if any((spd >> (4 * i)) & 0xF >= n_classes for i in range(int(r['n_nics']))):
+                    return wire.ERR_INVALID, None, 'speed class'
+    return None
+
+
+def batch_refusal(pods, now, rounds, rel, src_ref, recs, k):
+    """(code, pod, rule) of plan_batch_rounds (``rel`` None) or plan_batch_releases (``rel``: tracked, pods_used,
+    releases), in the order nhd_api.cu's plan_batch checks: round clocks and the releases' rounds and clocks, the
+    source, tracked nodes and untracked releases, the device check of pods_used against the NIC bits, then the pods
+    (non-finite clocks, the tuple limit at NUMA count k)."""
+    if len(rounds):
+        late = np.flatnonzero(np.asarray(now) > rounds[0])
+        if len(late):
+            return wire.ERR_INVALID, int(late[0]), 'round clock'
+    if rel is not None:
+        fin = now[np.isfinite(now)]
+        t0 = float(fin.max()) if len(fin) else -np.inf
+        for j, rl in enumerate(rel[2]):
+            r, c = int(rl['round']), float(rl['clock'])
+            if not (1 <= r <= len(rounds)) or not np.isfinite(c) or (j and c < rel[2][j - 1]['clock']) or \
+                    c < (t0 if r == 1 else rounds[r - 2]) or c > rounds[r - 1]:
+                return wire.ERR_INVALID, None, 'release gap'
+    if src_ref is not None:
+        return src_ref + ('source',)
+    if rel is not None:
+        tracked, used, rels = rel
+        if len(set(tracked)) != len(tracked) or any(t < 0 or t >= len(recs) for t in tracked):
+            return wire.ERR_INVALID, None, 'tracked'
+        if any(int(n) not in tracked for n in rels['node']):
+            return wire.ERR_INVALID, None, 'untracked'
+        for t, node in enumerate(tracked):
+            nn, inuse = int(recs['n_nics'][node]), int(recs['nic_inuse'][node])
+            if any(((used[t, i] > 0) != bool(inuse >> i & 1)) if i < nn else used[t, i] != 0
+                   for i in range(wire.MAX_NICS)):
+                return wire.ERR_INVALID, None, 'pods_used sign'
+    ref = pod_refusal(pods, now, k)
+    return None if ref is None else ref + ('pod',)
+
+
+def _result_bytes(res):
+    """A call's result, arrays as bytes, to compare two handles' answers."""
+    return None if res is None else tuple(x.tobytes() if isinstance(x, np.ndarray) else x for x in res)
 
 
 def static_key(r):
@@ -171,14 +233,70 @@ class Draw:
         return cluster_records(self.rng, self.layout, n)
 
 
-def make_session(seed, n_steps=30, sizes=SIZES):
+    def added(self, k):
+        """k records for a grown scenario: the cluster's kinds, some replaced by a 4-NUMA huge_node, made GPU-less, put
+        in maintenance or given a node-group bit no loaded node has."""
+        rng = self.rng
+        recs = self.nodes(k)
+        for j in range(k):
+            kind = int(rng.integers(0, 7))
+            if kind == 0:
+                recs[j] = self.four_numa()
+            elif kind == 1:
+                for f in ('n_gpus', 'gpu_used', 'gpu_numa_mask', 'gpu_sw'):
+                    recs[j][f] = 0
+            elif kind == 2:
+                recs[j]['flags'] |= wire.NODE_ACTIVE | wire.NODE_MAINTENANCE
+            elif kind == 3:
+                recs[j]['group_mask'] = np.uint64(1) << np.uint64(62)
+        return recs
+
+    def four_numa(self):
+        if not hasattr(self, '_four'):
+            while True:
+                r = special_nodes(self.rng, self.layout, 1, 'h')
+                if r['n_numa'][0] == 4:
+                    break
+            r['flags'] |= wire.NODE_ACTIVE
+            r['flags'] &= np.uint8(0xFF ^ wire.NODE_MAINTENANCE)
+            self._four = r[0]
+        return self._four
+
+    def rounds(self, now, lo=1, hi=6, early=False):
+        """Later scan clocks from the pods' last clock, periods around the busy window; ``early``: the first is before
+        the clock of one of the pods (a malformed call)."""
+        rng = self.rng
+        fin = now[np.isfinite(now)]
+        t = float(fin.max()) if len(fin) else self.t
+        k = int(rng.integers(lo, hi + 1))
+        out = list(t + np.cumsum(rng.choice([0.0, BUSY / 3.0, BUSY, BUSY + 1.0, 7.0], k)))
+        if early and k and len(fin):
+            out[0] = float(fin[int(rng.integers(0, len(fin)))]) - 1.0
+        return out
+
+
+# the ops of the sessions before the forecast calls, with their weights: the default of make_session, so that every
+# seed still generates the session it always did
+BASIC_WEIGHTS = {'load_nodes': 2, 'update_nodes': 5, 'snapshot': 2, 'restore': 1.5, 'solve_batch': 6, 'query_batch': 3,
+                 'plan_batch': 3, 'plan_scenarios': 3, 'explain_batch': 1, 'explain_pod': 1, 'explain_macro': 2}
+BASIC = tuple(BASIC_WEIGHTS)
+# the scenario and batch forecasts: explained, grown and round scenario calls, plan_batch_rounds, plan_batch_releases
+FORECAST_WEIGHTS = {'plan_explained': 2, 'plan_grown': 2, 'plan_rounds': 2, 'batch_rounds': 2, 'batch_releases': 3}
+FORECASTS = tuple(FORECAST_WEIGHTS)
+# the share of scenario forecasts and plan_batch_rounds calls malformed on purpose (with every fourth
+# plan_batch_releases call: some 3 % of the calls of a session with the forecasts)
+MALFORMED = 0.22
+
+
+def make_session(seed, n_steps=30, sizes=SIZES, kinds=BASIC):
     """A random session: ``{'seed', 'steps': [(op, args), ...]}``.  Ops and arguments only depend on the seed (node
-    counts are tracked here so that indices stay in range); what they do to the records is the runner's business."""
+    counts are tracked here so that indices stay in range); what they do to the records is the runner's business.
+    ``kinds``: the ops drawn (``BASIC``, the default, or with ``FORECASTS``); the explanation sequence also mixes in
+    the forecast ops drawn."""
     rng = np.random.default_rng(seed)
     d = Draw(rng, new_layout())
     steps = []
-    weights = {'load_nodes': 2, 'update_nodes': 5, 'snapshot': 2, 'restore': 1.5, 'solve_batch': 6, 'query_batch': 3,
-               'plan_batch': 3, 'plan_scenarios': 3, 'explain_batch': 1, 'explain_pod': 1, 'explain_macro': 2}
+    weights = {k: v for k, v in {**BASIC_WEIGHTS, **FORECAST_WEIGHTS}.items() if k in kinds}
     names = list(weights)
     p = np.array([weights[k] for k in names])
     p = p / p.sum()
@@ -218,6 +336,68 @@ def make_session(seed, n_steps=30, sizes=SIZES):
                 out.append((ex, pods, now, lift, edits))
         return ('plan_scenarios', {'scenarios': out, 'source': src()})
 
+    def bad():
+        return rng.random() < MALFORMED
+    made = []
+
+    def forecast_scen(op):
+        """Scenarios of 0 to 8 pods (32 at most per call) with lifts and edits; grown: added records, an unknown speed
+        class on one of them now and then; rounds: mixed with scenarios of no rounds (None) and empty ones."""
+        out = []
+        wrong = bad()
+        for _ in range(int(rng.integers(1, 5))):
+            pods, now = d.pods(0, 8)
+            ex = some(int(rng.integers(0, 4)))
+            lift = int(rng.integers(0, len(pods) + 1)) if rng.random() < 0.5 else None
+            edits = None
+            if rng.random() < 0.4:
+                at = some(int(rng.integers(1, 3)))
+                edits = (at, d.nodes(len(at)))
+            adds = None
+            if op != 'plan_explained' and (op == 'plan_grown' or rng.random() < 0.4) and rng.random() < 0.85:
+                k = int(rng.integers(1, 4))
+                adds = (np.sort(rng.integers(0, n + 1, k)).astype(np.int32), d.added(k))
+                if op == 'plan_grown' and wrong and (adds[1]['n_nics'] > 0).any():
+                    j = int(np.flatnonzero(adds[1]['n_nics'] > 0)[0])
+                    adds[1][j]['nic_speed'][0] = (int(adds[1][j]['nic_speed'][0]) & ~0xF) | 0xF
+                    wrong = False
+            rounds = None
+            if op == 'plan_rounds':
+                kind = rng.random()
+                rounds = d.rounds(now, early=wrong) if kind < 0.7 else ([] if kind < 0.85 else None)
+                wrong = wrong and not rounds
+            out.append((ex, pods, now, lift, edits, adds, rounds))
+        return (op, {'scenarios': out, 'source': src()})
+
+    def batch_forecast(op):
+        """plan_batch_rounds / plan_batch_releases of up to 32 pods over up to 6 rounds; the releases and the tracked
+        free-NIC nodes as fractions of the deployed pods and nodes the runner knows of."""
+        pods, now = d.pods(1, 32)
+        if rng.random() < 0.4 and np.isfinite(now).any():                 # one descriptor at one clock: the nodes
+            pods[:] = pods[int(rng.integers(0, len(pods)))]               # that fit it are stamped busy in turn, and
+            now[:] = now[np.isfinite(now)].max()                          # the rest wait for a later round
+        wrong = bad()
+        ex = some(int(rng.integers(0, 6))) if rng.random() < 0.7 else np.zeros(0, np.int32)
+        args = {'pods': pods, 'now': now, 'source': src(), 'exclude': ex, 'explain': bool(rng.random() < 0.5)}
+        if op == 'batch_rounds':
+            args['rounds'] = d.rounds(now, 0 if rng.random() < 0.1 else 1, early=wrong)
+            return (op, args)
+        made.append(op)                                                    # every fourth one broken, the ways in turn
+        k = made.count(op)
+        how = ('gap', 'untracked', 'sign')[(seed + k // 4) % 3] if k % 4 == 0 else None
+        args['rounds'] = d.rounds(now)
+        r = len(args['rounds'])
+        args['ends'] = [(float(rng.random()), int(rng.integers(1, r + 1)), float(rng.choice([0.0, 0.5, 1.0, rng.random()])),
+                         int(rng.integers(1, 3))) for _ in range(int(rng.integers(0, 9)))]
+        args['extra'] = [(float(rng.random()), int(rng.integers(1, 1 << 32)), -1 - int(rng.integers(0, 2)))
+                         for _ in range(int(rng.integers(0, 4)))]
+        args['bad'] = how
+        return (op, args)
+
+    def forecast(op):
+        return forecast_scen(op) if op.startswith('plan_') else batch_forecast(op)
+    mix = [query, plan, scen] + [lambda op=op: forecast(op) for op in FORECASTS if op in kinds]
+
     while len(steps) < n_steps:
         op = names[int(rng.choice(len(names), p=p))]
         if op == 'load_nodes':
@@ -246,6 +426,8 @@ def make_session(seed, n_steps=30, sizes=SIZES):
             steps.append(plan())
         elif op == 'plan_scenarios':
             steps.append(scen())
+        elif op in FORECASTS:
+            steps.append(forecast(op))
         elif op in ('explain_batch', 'explain_pod'):
             steps.append((op, {'which': float(rng.random())}))
         elif op == 'explain_macro':                                         # the sequence explanations need
@@ -253,7 +435,7 @@ def make_session(seed, n_steps=30, sizes=SIZES):
             pods, now = d.pods(8, 64, four=False)
             steps.append(('solve_batch', {'pods': pods, 'now': now}))
             for _ in range(int(rng.integers(0, 3))):
-                steps.append((query, plan, scen)[int(rng.integers(0, 3))]())
+                steps.append(mix[int(rng.integers(0, len(mix)))]())
             steps.append(('explain_batch', {'which': 0.0}))
             steps.append(('explain_pod', {'which': float(rng.random())}))
         else:
@@ -289,6 +471,8 @@ class Runner:
         self.after_snap = False       # the last call that moved the generation was nhd_snapshot
         self.expl = None              # (pods, now, batch-start records, bindings) of an explainable batch
         self.history = []             # the records at the start of every batch
+        self.deployed = []            # (binding, pod) of every pod a batch placed on the records as they are
+        self.snap_deployed = []       # the same list at the snapshot
 
     def close(self):
         self.s.close()
@@ -307,18 +491,24 @@ class Runner:
             return None, _refusal(e)
 
     def expect(self, where, got_ref, want_ref):
+        """The refusal (code, pod named) the model expects, or none; a third element of ``want_ref`` names the rule
+        for the stats."""
         if got_ref is not None:
             self.stats['refusals'][got_ref[0]] = self.stats['refusals'].get(got_ref[0], 0) + 1
         if (got_ref is None) != (want_ref is None) or (want_ref is not None and
-                                                       (got_ref[0], got_ref[1]) != tuple(want_ref)):
+                                                       (got_ref[0], got_ref[1]) != tuple(want_ref[:2])):
             raise Mismatch(f'{where}: refusal {got_ref}, expected {want_ref}')
+        if want_ref is not None and len(want_ref) > 2:
+            self.stats['rules'][want_ref[2]] = self.stats['rules'].get(want_ref[2], 0) + 1
 
-    def same(self, where, got, want):
+    def same(self, where, got, want, n_nodes=None):
+        """Bindings equal byte for byte, none on a node past ``n_nodes`` (the loaded nodes and the call's added ones)."""
+        n_nodes = len(self.recs) if n_nodes is None else n_nodes
         if got.tobytes() != want.tobytes():
             from tests import helpers
             raise Mismatch(f'{where}: {helpers.first_binding_diff(want, got)}')
-        if len(got) and got['node'].max() >= len(self.recs):
-            raise Mismatch(f'{where}: a node outside the {len(self.recs)} loaded nodes (padding) was chosen')
+        if len(got) and got['node'].max() >= n_nodes:
+            raise Mismatch(f'{where}: a node outside the {n_nodes} loaded and added nodes (padding) was chosen')
         self.stats['bindings'] += len(got)
         st = self.stats['status']
         for k, v in zip(*np.unique(got['status'], return_counts=True)):
@@ -340,6 +530,7 @@ class Runner:
         self.recs = np.ascontiguousarray(recs, dtype=wire.NODE_DTYPE).copy()
         self.snap, self.snap_fresh = None, False
         self.history = []
+        self.deployed, self.snap_deployed = [], []
         self.moved()
 
     def update_nodes(self, idx, kind, recs=None, set=None, clear=None, masks=None, back=None):
@@ -356,12 +547,16 @@ class Runner:
                 new = self.history[-back][idx].copy()
         self.s.update_nodes(idx, new)
         self.recs[idx] = new
+        if kind in ('hardware', 'release'):                               # those pods are gone with the record
+            gone = {int(i) for i in idx}
+            self.deployed = [(b, p) for b, p in self.deployed if int(b['node']) not in gone]
         self.snap_fresh = False
         self.moved()
 
     def snapshot(self):
         self.s.snapshot()
         self.snap, self.snap_fresh = self.recs.copy(), True
+        self.snap_deployed = list(self.deployed)
         self.moved()
         self.after_snap = True
 
@@ -370,6 +565,7 @@ class Runner:
         self.expect('restore', ref, None if self.snap is not None else (wire.ERR_STATE, None))
         if self.snap is not None:
             self.recs = self.snap.copy()
+            self.deployed = list(self.snap_deployed)
             self.moved()
 
     def solve_batch(self, pods, now):
@@ -394,6 +590,7 @@ class Runner:
             self.same('solve_batch against a fresh handle', got, fgot)
         self.history.append(start)
         self.recs = final
+        self.deployed += [(got[i].copy(), pods[i].copy()) for i in np.flatnonzero(got['status'] == wire.PLACED)]
         if on_snap:
             self.expl = (pods.copy(), now.copy(), start, got.copy())
 
@@ -443,45 +640,202 @@ class Runner:
         if self.check_fresh:
             self.same(f'plan_batch ({source}) against a fresh handle', b, fgot[0] if explain else fgot)
 
-    def plan_scenarios(self, scenarios, source):
+    def plan_scenarios(self, scenarios, source, explain=False, what='plan_scenarios'):
+        """Any scenario call: plain, edited, explained, grown (sixth element) and with rounds (seventh), each scenario
+        against the oracle of its entry point, added nodes numbered call-wide."""
         from tests.test_defrag import oracle_defrag
+        from tests.test_expand import oracle_grown
+        from tests.test_forecast import _sc, oracle_rounds
         from tests.test_plan import oracle_plan
+        from tests.test_plan_reasons import oracle_explained
+        scs = [_sc(sc) for sc in scenarios]
         recs, want_ref = self.source(source)
-        got, ref = self.call(lambda: self.s.plan_scenarios(scenarios, source=source))
-        self.expect(f'plan_scenarios ({source})', ref, want_ref)
+        want_ref = scenario_call_refusal(scs, want_ref, self.n_classes())
+        got, ref = self.call(lambda: self.s.plan_scenarios(scenarios, source=source, explain=explain))
+        self.expect(f'{what} ({source})', ref, want_ref)
         if recs is None:
             return
-        fgot = None
+        fgot, fref = None, None
         if self.check_fresh:
             f = self.fresh(recs)
             try:
-                fgot = f.plan_scenarios(scenarios)
+                fgot, fref = self.call(lambda: f.plan_scenarios(scenarios, explain=explain))
             finally:
                 f.close()
+            self.expect(f'{what} on a fresh handle', fref, want_ref)
+        if want_ref is not None:
+            return
+        rounds = any(sc[6] is not None for sc in scs)
+        grown_call = any(sc[5] is not None for sc in scs)
         k = max_numa(self.recs)
-        for sc in scenarios:
-            if len(sc) > 4 and sc[4] is not None:
-                k = max(k, int(np.asarray(sc[4][1])['n_numa'].max()))
-        for j, sc in enumerate(scenarios):
-            ex, pods, now = sc[:3]
-            lift = sc[3] if len(sc) > 3 else None
-            edits = sc[4] if len(sc) > 4 else None
-            code, pod, b = got[j]
+        for sc in scs:
+            for change in (sc[4], sc[5]):                                  # edits and additions count, held or not
+                if change is not None and len(change[1]):
+                    k = max(k, int(np.asarray(change[1])['n_numa'].max()))
+        base, st = 0, self.stats
+        for j, (ex, pods, now, lift, edits, adds, clocks) in enumerate(scs):
+            res, where = got[j], f'{what} ({source}) scenario {j}'
+            n_add = 0 if adds is None else len(adds[0])
             want_ref = pod_refusal(pods, now, k)
-            self.expect(f'plan_scenarios ({source}) scenario {j}', None if code == 0 else (code, pod), want_ref)
-            if fgot is not None:
-                self.expect(f'plan_scenarios scenario {j} on a fresh handle',
-                            None if fgot[j][0] == 0 else fgot[j][:2], want_ref)
-            if want_ref is not None:
+            self.expect(where, None if res[0] == 0 else tuple(res[:2]), want_ref)
+            if fgot is not None and _result_bytes(fgot[j]) != _result_bytes(res):
+                raise Mismatch(f'{where}: differs from a fresh handle')
+            if want_ref is not None or not len(pods):
+                base += n_add
                 continue
-            exl = [int(i) for i in ex]
-            if lift is None and edits is None:
-                want = oracle_plan(recs, self.speed, pods, now, exl, BUSY)[0] if len(pods) else b
+            b, exl, wrows, wrnd = res[2], [int(i) for i in ex], None, None
+            if rounds:
+                want, wrnd, wrows, _ = oracle_rounds(recs, self.speed, pods, now, exl, lift, edits, adds, clocks, base,
+                                                     BUSY, explain=explain)
+            elif grown_call:
+                want = oracle_grown(recs, self.speed, pods, now, exl, lift, edits, adds, base, BUSY, explain=explain)
+                want, wrows = want if explain else (want, None)
+            elif explain:
+                want, wrows = oracle_explained(recs, self.speed, pods, now, exl, lift, edits, BUSY)
+            elif lift is None and edits is None:
+                want = oracle_plan(recs, self.speed, pods, now, exl, BUSY)[0]
             else:
                 want = oracle_defrag(recs, self.speed, pods, now, exl, lift, edits, busy=BUSY)
-            self.same(f'plan_scenarios ({source}) scenario {j} against the oracle', b, want)
-            if fgot is not None:
-                self.same(f'plan_scenarios ({source}) scenario {j} against a fresh handle', b, fgot[j][2])
+            self.same(f'{where} against the oracle', b, want, len(recs) + base + n_add)
+            if explain:
+                self.same_rows(where, res[3], wrows, b, len(recs) + n_add)
+            if rounds:
+                self.same_rounds(where, res[-1], wrnd, b)
+            placed = b['status'] == wire.PLACED
+            st['on_added'] += int((placed & (b['node'] >= len(recs))).sum())
+            base += n_add
+
+    def plan_explained(self, scenarios, source):
+        self.plan_scenarios(scenarios, source, explain=True, what='plan_explained')
+
+    def plan_grown(self, scenarios, source):
+        self.plan_scenarios(scenarios, source, explain=bool(len(scenarios) % 2), what='plan_grown')
+
+    def plan_rounds(self, scenarios, source):
+        self.plan_scenarios(scenarios, source, explain=bool(len(scenarios) % 2), what='plan_rounds')
+
+    def same_rows(self, where, rows, want, b, n_nodes):
+        """Reason rows equal the oracle's; every NO_CANDIDATE row counts each loaded and added node once."""
+        if rows.tobytes() != want.tobytes():
+            raise Mismatch(f'{where}: reason rows {np.flatnonzero((rows != want).any(1))} differ from the oracle')
+        none = b['status'] == wire.NO_CANDIDATE
+        if (rows[none].sum(1) != n_nodes).any():
+            raise Mismatch(f'{where}: a NO_CANDIDATE row does not sum to {n_nodes} nodes')
+        self.stats['rows'] += int(none.sum())
+
+    def same_rounds(self, where, rnd, want, b):
+        if rnd.tobytes() != np.asarray(want, dtype='<i4').tobytes():
+            raise Mismatch(f'{where}: pod rounds {rnd} differ from the oracle\'s {want}')
+        self.stats['later'] += int(((b['status'] == wire.PLACED) & (rnd >= 1)).sum())
+
+    def n_classes(self):
+        return max([i + 1 for i, s in enumerate(self.speed) if s != 0.0], default=0)
+
+    def batch_rounds(self, pods, now, rounds, source, exclude, explain):
+        self._batch_forecast('batch_rounds', pods, now, rounds, source, exclude, explain, None)
+
+    def batch_releases(self, pods, now, rounds, source, exclude, explain, ends, extra, bad):
+        """The releases are pods a batch of this session deployed on the source records (``ends``: fractions of that
+        list, a round, a place in the round's gap and the pairings per NIC); the tracked nodes are theirs plus free-NIC
+        nodes (``extra``) whose free NICs start at -1 or -2; ``pods_used`` from the source records' NIC bits.  ``bad``
+        breaks one argument: a release out of its gap, a release on an untracked node, a flipped pods_used sign."""
+        from tests.test_forecast_releases import release_of
+        snap = source == 'snapshot' and self.snap is not None
+        recs, dep = (self.snap, self.snap_deployed) if snap else (self.recs, self.deployed)
+        fin = now[np.isfinite(now)]
+        t0 = float(fin.max()) if len(fin) else -np.inf
+
+        def gap(rnd):
+            return (t0 if rnd == 1 else rounds[rnd - 2]), rounds[rnd - 1]
+        rels, taken = [], set()
+        for which, rnd, at, pairings in ends:
+            i = int(which * len(dep))
+            if not dep or i in taken:
+                continue
+            taken.add(i)
+            b, pod = dep[i]
+            lo, hi = gap(rnd)
+            clock = hi if at == 1.0 or not np.isfinite(lo) else min(hi, lo + at * (hi - lo))
+            rels.append(release_of(b, pod, int(b['node']), rnd, clock, pairings))
+        rels = np.array(sorted(rels, key=lambda x: (int(x['round']), float(x['clock']))), dtype=wire.RELEASE_DTYPE)
+        tracked = sorted({int(x['node']) for x in rels})
+        # free-NIC nodes the pods take when nothing ends (where a negative counter cuts), else any with NICs
+        from oracle import binding
+        from tests.test_plan import excluded
+        ok = np.isfinite(now)
+        first = binding.solve(excluded(recs, [int(i) for i in exclude]), self.speed, pods[ok], now[ok],
+                              min_busy_secs=BUSY)[0]
+        free = sorted({int(v) for v in first['node'][first['n_claimed'] > 0]} - set(tracked)) or \
+            [int(v) for v in np.flatnonzero(recs['n_nics'] > 0) if int(v) not in tracked]
+        negs = {}
+        for which, bits, neg in extra:
+            if free:
+                negs[free[int(which * len(free))]] = (bits, neg)
+        tracked += sorted(negs)
+        used = np.zeros((len(tracked), wire.MAX_NICS), dtype='<i2')
+        for t, node in enumerate(tracked):
+            inuse, bits, neg = int(recs['nic_inuse'][node]), *negs.get(node, (0, 0))
+            for i in range(int(recs['n_nics'][node])):
+                used[t, i] = 1 if inuse >> i & 1 else (neg if bits >> i & 1 else 0)
+        if bad == 'gap' and len(rels):
+            rels[0]['clock'] = gap(int(rels[0]['round']))[0] - 1.0
+        elif bad == 'untracked' and len(rels):
+            t = tracked.index(int(rels[0]['node']))
+            tracked, used = tracked[:t] + tracked[t + 1:], np.delete(used, t, axis=0)
+        elif bad == 'sign' and tracked:
+            node = tracked[0]
+            used[0, 0] = 0 if recs['n_nics'][node] and recs['nic_inuse'][node] & 1 else 1
+        self._batch_forecast('batch_releases', pods, now, rounds, source, exclude, explain, (tracked, used, rels))
+
+    def _batch_forecast(self, what, pods, now, rounds, source, exclude, explain, rel):
+        """plan_batch_rounds (``rel`` None) or plan_batch_releases (``rel``: tracked, pods_used, releases) against the
+        refusal model, a fresh handle and the oracle loop; a rounds forecast also against the scenario call of that
+        one scenario on this handle."""
+        from tests.test_forecast import oracle_rounds
+        from tests.test_forecast_releases import oracle_releases
+        recs, src_ref = self.source(source)
+        ex = [int(i) for i in exclude]
+        want_ref = batch_refusal(pods, now, rounds, rel, src_ref, recs, max_numa(self.recs, ex))
+
+        def run(s, src):
+            if rel is None:
+                return s.plan_batch_rounds(pods, now, rounds, source=src, exclude=ex, explain=explain)
+            return s.plan_batch_releases(pods, now, rounds, *rel, source=src, exclude=ex, explain=explain)
+        got, ref = self.call(lambda: run(self.s, source))
+        self.expect(f'{what} ({source})', ref, want_ref)
+        if recs is None:
+            return
+        if self.check_fresh:
+            f = self.fresh(recs)
+            try:
+                fgot, fref = self.call(lambda: run(f, 'mirror'))
+            finally:
+                f.close()
+            self.expect(f'{what} on a fresh handle', fref, want_ref)
+            if want_ref is None and _result_bytes(fgot) != _result_bytes(got):
+                raise Mismatch(f'{what} ({source}): differs from a fresh handle')
+        if want_ref is not None:
+            return
+        if rel is None:
+            want, wrnd, wrows, _ = oracle_rounds(recs, self.speed, pods, now, ex, rounds=rounds, busy=BUSY,
+                                                 explain=explain)
+        else:
+            want, wrnd, wrows, cuts = oracle_releases(recs, self.speed, pods, now, rounds, *rel, exclude=ex, busy=BUSY,
+                                                      explain=explain)
+            self.stats['cuts'] += sum(cuts)
+        b, rnd = got[:2]
+        self.same(f'{what} ({source}) against the oracle', b, want)
+        self.same_rounds(f'{what} ({source})', rnd, wrnd, b)
+        if explain:
+            self.same_rows(f'{what} ({source})', got[2], wrows, b, len(recs))
+        if rel is None:                        # the scenario call of this one scenario, on this handle
+            sres = self.s.plan_scenarios([(ex, pods, now, None, None, None, rounds)], source=source, explain=explain)[0]
+            if sres[0] == 0:
+                mine = (sres[2], sres[-1]) + ((sres[3],) if explain else ())
+                if _result_bytes(mine) != _result_bytes(got):
+                    raise Mismatch(f'{what} ({source}): differs from the scenario call')
+            elif sres[0] != wire.ERR_UNSUPPORTED or not ex:
+                raise Mismatch(f'{what} ({source}): the scenario call refused with {sres[:2]}')
 
     def _explained(self, what, fn, fresh_fn, want_fn):
         got, ref = self.call(fn)
@@ -542,7 +896,10 @@ class Runner:
 
 
 def new_stats():
-    return {'ops': {}, 'refusals': {}, 'status': {}, 'bindings': 0, 'calls': 0, 'explained': 0}
+    """``rules``: refusals by the model's rule; ``rows``: NO_CANDIDATE reason rows compared; ``later``: pods placed at a
+    round >= 1; ``on_added``: pods placed on added nodes; ``cuts``: the oracle loop's cuts in release forecasts."""
+    return {'ops': {}, 'refusals': {}, 'status': {}, 'bindings': 0, 'calls': 0, 'explained': 0, 'rules': {}, 'rows': 0,
+            'later': 0, 'on_added': 0, 'cuts': 0}
 
 
 def run_session(session, mode, stats=None):
@@ -697,7 +1054,17 @@ def test_the_tuple_limit_follows_updates(mode):
                 ('plan_batch', {'pods': pods, 'now': now + t, 'source': 'mirror', 'exclude': np.array([6]),
                                 'explain': False}),
                 ('plan_scenarios', {'scenarios': [([5], pods, now + t), ([], pods, now + t, 2, None)],
-                                    'source': 'mirror'})]
+                                    'source': 'mirror'}),
+                ('plan_explained', {'scenarios': [([5], pods, now + t), ([], pods, now + t, 2, None)],
+                                    'source': 'mirror'}),
+                ('plan_grown', {'scenarios': [([], pods, now + t, None, None, ([0], recs[[1]]))], 'source': 'mirror'}),
+                ('plan_rounds', {'scenarios': [([6], pods, now + t, None, None, None, [5100.0 + t])],
+                                 'source': 'mirror'}),
+                ('batch_rounds', {'pods': pods, 'now': now + t, 'rounds': [5100.0 + t], 'source': 'mirror',
+                                  'exclude': np.array([5]), 'explain': False}),
+                ('batch_releases', {'pods': pods, 'now': now + t, 'rounds': [5100.0 + t], 'source': 'mirror',
+                                    'exclude': np.array([6]), 'explain': True, 'ends': [(0.5, 1, 0.5, 2)],
+                                    'extra': [], 'bad': None})]
 
     def flags(set_, clear):
         return ('update_nodes', {'idx': np.array([5], np.int32), 'kind': 'flags',
@@ -772,6 +1139,7 @@ def test_explanations_after_interleaved_whatif_calls(mode):
     from tests.test_query import packed
     recs, pods, now, speed, busy = packed(explain_scenarios()[1])
     assert busy == BUSY
+    t = float(np.max(now))
     r = Runner(mode, speed=speed)
     try:
         r.run({'seed': 'explain', 'steps': [
@@ -783,6 +1151,17 @@ def test_explanations_after_interleaved_whatif_calls(mode):
             ('plan_scenarios', {'scenarios': [([1], pods, now), ([0], pods, now, 3, ([2], recs[[1]]))],
                                 'source': 'snapshot'}),
             ('plan_scenarios', {'scenarios': [([], pods[:4], now[:4])], 'source': 'mirror'}),
+            ('plan_explained', {'scenarios': [([1], pods, now), ([0], pods, now, 3, ([2], recs[[1]]))],
+                                'source': 'snapshot'}),
+            ('plan_grown', {'scenarios': [([], pods, now, None, None, ([0, len(recs)], recs[[1, 2]]))],
+                            'source': 'mirror'}),
+            ('plan_rounds', {'scenarios': [([1], pods, now, None, None, ([1], recs[[0]]), [t + 10.0, t + 40.0]),
+                                           ([], pods[:3], now[:3], None, None, None, None)], 'source': 'snapshot'}),
+            ('batch_rounds', {'pods': pods, 'now': now, 'rounds': [t + 30.0], 'source': 'snapshot', 'exclude': [0],
+                              'explain': True}),
+            ('batch_releases', {'pods': pods, 'now': now, 'rounds': [t + 30.0, t + 60.0], 'source': 'mirror',
+                                'exclude': [], 'explain': True, 'ends': [(0.1, 1, 0.5, 2), (0.6, 2, 1.0, 1)],
+                                'extra': [(0.5, 0xFF, -1)], 'bad': None}),
             ('explain_batch', {'which': 0.0}), ('explain_pod', {'which': 0.0}), ('explain_pod', {'which': 0.5}),
             ('explain_pod', {'which': 0.9}), ('restore', {}), ('explain_batch', {'which': 0.0})]})
         assert r.stats['explained'] == 4 and r.stats['refusals'] == {wire.ERR_STATE: 1}, r.stats

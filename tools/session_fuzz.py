@@ -2,7 +2,10 @@
 through loads, updates, snapshots, restores, batches, queries, plans, scenario calls and explanations, every call
 compared with a fresh handle and the oracle.  Developer tool.
 
-    python tools/session_fuzz.py [first_seed] [n_seeds] [n_steps]
+    python tools/session_fuzz.py [first_seed] [n_seeds] [n_steps] [kinds]
+
+``kinds``: ``all`` (the default: every op, the forecasts included), ``basic`` (the ops of the sessions before the
+forecasts, as ``make_session``'s default) or a comma-separated list of ops.
 
 Runs on the CPU-emulated device (tests/emu) unless NHD_B200_LIB is unset and a CUDA device exists, in which case it
 runs on the GPU.  Environment: EMU_SCHED_SEED=<n> shuffles the emulated warp schedule, EMU_LANE_ORDER=a|d sets the
@@ -33,26 +36,31 @@ if not _on_gpu():
     os.environ['NHD_B200_ALLOW_EMULATED'] = '1'
     os.environ.setdefault('EMU_LANE_ORDER', 'd')
 
-from tests.test_handle_session import (EMU_SIZES, MODES, SIZES, Mismatch, make_session, new_stats,  # noqa: E402
-                                       run_session)
+from tests.test_handle_session import (BASIC, EMU_SIZES, FORECASTS, MODES, SIZES, Mismatch,  # noqa: E402
+                                       make_session, new_stats, run_session)
 
 
 def main():
     first = int(sys.argv[1]) if len(sys.argv) > 1 else 0
     n = int(sys.argv[2]) if len(sys.argv) > 2 else 200
     steps = int(sys.argv[3]) if len(sys.argv) > 3 else 30
+    arg = sys.argv[4] if len(sys.argv) > 4 else 'all'
+    kinds = {'all': BASIC + FORECASTS, 'basic': BASIC}.get(arg) or tuple(arg.split(','))
     sizes = EMU_SIZES if os.environ.get('NHD_B200_ALLOW_EMULATED') == '1' else SIZES
     bad = 0
     stats = new_stats()
     t0 = time.time()
     for seed in range(first, first + n):
         try:
-            run_session(make_session(seed, steps, sizes), MODES[seed % len(MODES)], stats)
+            run_session(make_session(seed, steps, sizes, kinds), MODES[seed % len(MODES)], stats)
         except Mismatch as e:
             bad += 1
             print('MISMATCH', e, flush=True)
     print(f"{n} sessions, {stats['calls']} calls, {stats['bindings']} bindings compared, {bad} mismatches, "
           f'{time.time() - t0:.0f} s')
+    print('ops', stats['ops'])
+    print('refused by rule', stats['rules'], '/ reason rows', stats['rows'], '/ placed at a later round', stats['later'],
+          '/ on added nodes', stats['on_added'], '/ cuts', stats['cuts'])
 
 
 if __name__ == '__main__':
