@@ -39,12 +39,13 @@ import threading
 import time
 from enum import Enum
 from queue import Queue
-from typing import Callable, Dict, Iterable, List, Optional, Sequence
+from typing import Any, Callable, Dict, Iterable, List, NamedTuple, Optional, Sequence
 
 import numpy as np
 
 from nhd_b200 import packing, wire
 from nhd_b200.Node import Node
+from nhd_b200.solver import Scenario
 
 NHD_SCHED_NAME = "nhd-scheduler"                # NHDScheduler.py:23
 
@@ -79,6 +80,23 @@ class RpcMsgType(Enum):                         # NHDCommon.py:69-73
     TYPE_SCHEDULER_INFO = 2
     TYPE_POD_INFO = 3
     TYPE_NODE_DETAIL = 4
+
+
+class ClusterScenario(NamedTuple):
+    """One dry run of ``DeviceCluster.plan_scenarios``: ``solver.Scenario`` with node names for indices, Node-like
+    objects for records and the pods as ``plan`` takes them (``now`` one clock or one per pod).  ``edits`` (None: none):
+    ``{node name: Node-like object}``, packed as ``sync`` packs nodes.  ``adds`` (None: none): ``[(before, node)]``,
+    each joining the node order right before the node named ``before`` (None: after the last node), packed by
+    ``pack_candidates`` before any pod (a pod may request a group name only a candidate carries)."""
+    exclude: Iterable[str]
+    tops: Sequence
+    pod_groups: Sequence[Iterable[str]]
+    now: Any
+    packed: Optional[Sequence] = None
+    lift: Optional[int] = None
+    edits: Optional[Dict[str, object]] = None
+    adds: Optional[Sequence[tuple]] = None
+    rounds: Optional[Sequence[float]] = None
 
 
 def _type_name(t) -> str:
@@ -275,19 +293,12 @@ class DeviceCluster:
         scan changes nothing and is left out, one at or before ``now`` is a ValueError.  The nodes' signed NIC pod
         counters are those of the synced ``Node`` objects; every node with a release or a negative counter is tracked.
         None when the solver in use cannot (a stand-in without ``plan_batch_releases``)."""
-        if releases is not None:
-            fn = getattr(self._solver, 'plan_batch_releases', None)
-            if fn is None:
-                return None
-            idx = self._indices(exclude, 'exclude')
-            tracked, used, rels = self._releases(releases, float(now if np.isscalar(now) else np.max(now)), round_clocks)
-            return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), round_clocks, tracked, used,
-                      rels, source=source, exclude=idx, explain=explain)
-        fn = getattr(self._solver, 'plan_batch_rounds', None)
+        fn = getattr(self._solver, 'plan_batch_rounds' if releases is None else 'plan_batch_releases', None)
         if fn is None:
             return None
         idx = self._indices(exclude, 'exclude')
-        return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), round_clocks, source=source,
+        rel = () if releases is None else self._releases(releases, float(np.max(now)), round_clocks)
+        return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), round_clocks, *rel, source=source,
                   exclude=idx, explain=explain)
 
     def _releases(self, releases: Sequence, now: float, round_clocks: Sequence[float]):
@@ -332,15 +343,8 @@ class DeviceCluster:
 
     def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror', explain: bool = False):
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
-        of ``(exclude, tops, pod_groups, now[, packed[, lift[, edits]]])`` with ``exclude`` node names.  ``lift`` (None:
-        never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits`` (None: none):
-        ``{node name: Node-like object}``, packed as ``sync`` packs nodes, the records those nodes have for the whole
-        scenario.  ``adds`` (eighth element, None: none): ``[(before, node)]``, Node-like objects in service for the
-        whole scenario, each joining the node order right before the node named ``before`` (None: after the last
-        node), packed by ``pack_candidates`` before any pod (a pod may request a group name only a candidate carries).
-        ``rounds`` (ninth element, None: none): the clocks of later pending scans, at which the scenario's pods not
-        placed yet are retried (``Solver.plan_scenarios``); with any, each result gains the per-pod round that placed
-        the pod.
+        of ``ClusterScenario`` records, or plain tuples of their fields in order.  When any scenario has ``rounds``,
+        each result gains the per-pod round that placed the pod (``Solver.plan_scenarios``).
         Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
         when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods; ``explain=True``: one
         ``(code, pod, bindings, counts)``, ``counts`` the per-reason node counts of the NO_CANDIDATE pods.  A pod
@@ -350,30 +354,27 @@ class DeviceCluster:
         fn = getattr(self._solver, 'plan_scenarios', None)
         if fn is None:
             return None
+        scenarios = [ClusterScenario(*sc) for sc in scenarios]
         # every scenario's names are checked, and every candidate packed, before any pod is packed
-        self._indices(sorted({n for sc in scenarios for n in list(sc[0]) + list(sc[6] if len(sc) > 6 and sc[6] else ())} |
-                             {b for sc in scenarios if len(sc) > 7 and sc[7] for b, _ in sc[7] if b is not None}),
+        self._indices(sorted({n for sc in scenarios for n in list(sc.exclude) + list(sc.edits or ())} |
+                             {b for sc in scenarios for b, _ in sc.adds or () if b is not None}),
                       'exclude, edit or add before')
-        added = [self.pack_candidates([node for _, node in sc[7]]) if len(sc) > 7 and sc[7] else None for sc in scenarios]
+        added = [self.pack_candidates([node for _, node in sc.adds]) if sc.adds else None for sc in scenarios]
         args, perm = [], []                           # perm: the call's additions in position order -> as given
         for sc, recs in zip(scenarios, added):
-            exclude, tops, pod_groups, now = sc[:4]
-            packed = sc[4] if len(sc) > 4 else None
-            lift = sc[5] if len(sc) > 5 else None
-            edits = sc[6] if len(sc) > 6 else None
-            idx = self._indices(exclude, 'exclude')
-            if edits:
-                edits = (self._indices(edits, 'edit'), self._pack(list(edits.values())))
-            adds = None
-            rounds = sc[8] if len(sc) > 8 else None
+            idx = self._indices(sc.exclude, 'exclude')
+            edits = adds = None
+            if sc.edits:
+                edits = (self._indices(sc.edits, 'edit'), self._pack(list(sc.edits.values())))
             if recs is not None:
-                at = np.asarray([len(self._names) if b is None else self._index[b] for b, _ in sc[7]], dtype='<i4')
+                at = np.asarray([len(self._names) if b is None else self._index[b] for b, _ in sc.adds], dtype='<i4')
                 order = np.argsort(at, kind='stable')
                 adds = (at[order], recs[order])
                 perm.extend((len(perm) + order).tolist())
-            args.append((idx, self._pods(tops, pod_groups, packed), self._clocks(len(tops), now)) +
-                        ((lift, edits or None, adds, rounds)
-                         if lift is not None or edits or adds or rounds is not None else ()))
+            # a solver stand-in need take no more fields than the call uses, nor ``explain`` unless it is asked for
+            pods = (idx, self._pods(sc.tops, sc.pod_groups, sc.packed), self._clocks(len(sc.tops), sc.now))
+            args.append(Scenario(*pods, sc.lift, edits, adds, sc.rounds)
+                        if sc.lift is not None or edits or adds or sc.rounds is not None else pods)
         res = fn(args, source=source, explain=True) if explain else fn(args, source=source)
         if perm and sorted(perm) != perm:
             n, back = len(self._names), np.asarray(perm, dtype=np.int64)
@@ -873,8 +874,9 @@ class NHDScheduler:
             self._sync()
             now = float(self._clock())
             res = self._supported(
-                self.cluster.plan_scenarios([(g, [e.top for e in ok], [e.groups for e in ok], now, [e.rec for e in ok])
-                                             for g, _, ok in todo], explain=reasons),
+                self.cluster.plan_scenarios([ClusterScenario(g, [e.top for e in ok], [e.groups for e in ok], now,
+                                                             packed=[e.rec for e in ok]) for g, _, ok in todo],
+                                            explain=reasons),
                 'plan scenarios (no plan_scenarios)')
             for (g, entries, ok), r in zip(todo, res):
                 out = r[2]
@@ -945,24 +947,16 @@ class NHDScheduler:
                     edits[node] = _copy_node(self.nodes[node])
                 self._give_back(edits[node], key[1], key[0], top, now)
             todo.append((g, [e for e in moved if e.solvable], tail, edits))
-        while todo:
-            res = self._supported(self.cluster.plan_scenarios([self._defrag_scenario(g, ok, tail, edits, now, delay)
-                                                               for g, ok, tail, edits in todo], explain=reasons),
-                                  'plan scenarios (no plan_scenarios)')
-            retry = []
-            for (g, ok, tail, edits), r in zip(todo, res):
-                code, pod, out = r[:3]
-                if out is None:
-                    # a pod beyond the tuple limits (judged with the group's nodes and the edited records counted):
-                    # it gets None, as in PlanDrain, and the group is planned again without it
-                    if code != wire.ERR_UNSUPPORTED:
-                        raise RuntimeError(f'nhd_plan_scenarios_edited refused group {g}: code {code}, pod {pod}')
-                    if pod < len(ok):
-                        ok = ok[:pod] + ok[pod + 1:]
-                    else:
-                        tail = tail[:pod - len(ok)] + tail[pod - len(ok) + 1:]
-                    retry.append((g, ok, tail, edits))
-                    continue
+
+        def drop(item, pod):
+            g, ok, tail, edits = item
+            k = pod - len(ok)                                   # the pod's place in the tail
+            return (g, ok[:pod] + ok[pod + 1:], tail, edits) if k < 0 else (g, ok, tail[:k] + tail[k + 1:], edits)
+        for _, done in self._plan_refused(
+                todo, lambda item: self._defrag_scenario(*item, now, delay), drop, reasons,
+                lambda item, code, pod: f'nhd_plan_scenarios_edited refused group {item[0]}: code {code}, pod {pod}'):
+            for (g, ok, tail, edits), r in done:
+                out = r[2]
                 moved, _, why = result[g]
                 moved.update(self._placements(ok, out[:len(ok)]))
                 if reasons:
@@ -973,7 +967,6 @@ class NHDScheduler:
                     if reasons:
                         why.update(self._reasons(tail, out[len(ok):], r[3][len(ok):]))
                     result[g] = (moved, pending, why)
-            todo = retry
         return result if reasons else {g: v[:2] for g, v in result.items()}
 
     def PlanExpansion(self, additions: Sequence[Sequence], keys: Sequence = None, reasons: bool = False) -> List:
@@ -1129,27 +1122,17 @@ class NHDScheduler:
                             placement[(e.key[0], e.key[1])] = (int(r), self.cluster.name_of(int(b['node'])))
                     if reasons:
                         why.update(self._reasons(ok, res[0], res[2]))
-            while todo:
-                res = self._supported(
-                    self.cluster.plan_scenarios([(exclude, [e.top for e in ok], [e.groups for e in ok], now,
-                                                  [e.rec for e in ok], None, None,
-                                                  [(before, node) for node, before in scens[j]])
-                                                 + ((clocks,) if clocks is not None else ()) for j, ok in todo],
-                                                explain=reasons),
-                    'plan scenarios (no plan_scenarios)')
-                added = [node.name for j, _ in todo for node, _ in scens[j]]
-                n_nodes, retry = len(self.nodes), []
-                for (j, ok), r in zip(todo, res):
-                    code, pod, out = r[:3]
-                    if out is None:
-                        # a pod beyond the tuple limits: it gets None, as in PlanDefrag, and the scenario is planned
-                        # again without it
-                        if code != wire.ERR_UNSUPPORTED:
-                            raise RuntimeError(f'nhd_plan_scenarios_grown refused scenario {j}: code {code}, pod {pod}')
-                        ok = ok[:pod] + ok[pod + 1:]
-                        if ok:
-                            retry.append((j, ok))
-                        continue
+            planned = self._plan_refused(
+                todo, lambda item: ClusterScenario(exclude, [e.top for e in item[1]], [e.groups for e in item[1]], now,
+                                                   [e.rec for e in item[1]], rounds=clocks,
+                                                   adds=[(before, node) for node, before in scens[item[0]]]),
+                lambda item, pod: (item[0], item[1][:pod] + item[1][pod + 1:]) if len(item[1]) > 1 else None, reasons,
+                lambda item, code, pod: f'nhd_plan_scenarios_grown refused scenario {item[0]}: code {code}, pod {pod}')
+            n_nodes = len(self.nodes)
+            for call, done in planned:
+                added = [node.name for j, _ in call for node, _ in scens[j]]     # numbered call-wide
+                for (j, ok), r in done:
+                    out = r[2]
                     placement, why = result[j]
                     for k, (e, b) in enumerate(zip(ok, out)):
                         if int(b['status']) == wire.PLACED:
@@ -1158,15 +1141,31 @@ class NHDScheduler:
                             placement[(e.key[0], e.key[1])] = name if clocks is None else (int(r[-1][k]), name)
                     if reasons:
                         why.update(self._reasons(ok, out, r[3]))
-                todo = retry
         return result
 
     @staticmethod
     def _defrag_scenario(g, moved, tail, edits, now, delay):
         """One ``PlanDefrag`` group as a ``DeviceCluster.plan_scenarios`` scenario."""
         pods = moved + tail
-        clock = [now] * len(moved) + [now + delay] * len(tail)
-        return (g, [e.top for e in pods], [e.groups for e in pods], clock, [e.rec for e in pods], len(moved), edits)
+        return ClusterScenario(exclude=g, tops=[e.top for e in pods], pod_groups=[e.groups for e in pods],
+                               now=[now] * len(moved) + [now + delay] * len(tail), packed=[e.rec for e in pods],
+                               lift=len(moved), edits=edits)
+
+    def _plan_refused(self, items: Sequence, make: Callable, drop: Callable, reasons: bool, refused: Callable):
+        """``DeviceCluster.plan_scenarios`` of ``make(item)`` for every item; yields per GPU call ``(its items, [(item,
+        result)] of those planned)`` (added nodes are numbered across the call).  An item refused for a pod beyond the
+        tuple limits (``wire.ERR_UNSUPPORTED``) is planned in the next call as ``drop(item, pod)``, the pod getting
+        None as in ``PlanDrain``, unless that is None; any other refusal raises ``RuntimeError(refused(item, code,
+        pod))``."""
+        while items:
+            res = self._supported(self.cluster.plan_scenarios([make(item) for item in items], explain=reasons),
+                                  'plan scenarios (no plan_scenarios)')
+            for item, (code, pod, out, *_) in zip(items, res):
+                if out is None and code != wire.ERR_UNSUPPORTED:
+                    raise RuntimeError(refused(item, code, pod))
+            yield items, [(item, r) for item, r in zip(items, res) if r[2] is not None]
+            retry = [drop(item, r[1]) for item, r in zip(items, res) if r[2] is None]
+            items = [item for item in retry if item is not None]
 
     def _plan(self, keys: Sequence, exclude: Sequence[str]):
         entries = self._read(keys)

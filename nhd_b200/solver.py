@@ -3,8 +3,8 @@
 Works on packed numpy records (``nhd_b200.wire``); the object-level drop-in lives in
 ``nhd_b200.Matcher``.  All compute happens in the CUDA library."""
 import ctypes
-
 import os
+from typing import NamedTuple, Optional, Sequence
 
 import numpy as np
 
@@ -59,6 +59,26 @@ def _source(source):
     if src is None:
         raise ValueError(f"source must be 'mirror' or 'snapshot', not {source!r}")
     return src
+
+
+class Scenario(NamedTuple):
+    """One dry run of ``Solver.plan_scenarios``.
+
+    ``exclude``: node indices taken as in maintenance; ``pods``, ``now``: the scenario's ``wire.POD_DTYPE`` pods and
+    their clocks, planned in order.  ``lift`` (None: never): the excluded nodes are back in service from the scenario's
+    pod ``lift`` on.  ``edits`` (None: none): ``(nodes, records)``, node indices and a ``wire.NODE_DTYPE`` array, the
+    records those nodes have for the whole scenario.  ``adds`` (None: none): ``(at, records)``, int positions and a
+    ``wire.NODE_DTYPE`` array: nodes added for the whole scenario, each right before source node ``at[k]``
+    (``n_nodes``: at the end), ``at`` never going down.  ``rounds`` (None: none): the clocks of later pending scans,
+    never going down and none before the scenario's pod clocks; at each, the scenario's pods not placed yet are solved
+    again in order on the records the previous scan left, and the bindings hold each pod's last attempt."""
+    exclude: Sequence[int]
+    pods: np.ndarray
+    now: Sequence[float]
+    lift: Optional[int] = None
+    edits: Optional[tuple] = None
+    adds: Optional[tuple] = None
+    rounds: Optional[Sequence[float]] = None
 
 
 class Solver:
@@ -206,65 +226,54 @@ class Solver:
         return out
 
     def plan_batch(self, pods, now, source='mirror', exclude=(), explain=False, out=None):
-        """A dry run of ``solve_batch`` (``nhd_plan_batch``): the bindings the pods would get scheduled in order, each
-        seeing the ones before it, on the current records (``source='mirror'``) or on those of the last ``snapshot()``
-        (``'snapshot'``), with the node indices ``exclude`` taken as in maintenance.  With ``explain=True`` returns
-        ``(bindings, counts)``, counts being what ``explain_batch`` would return after that solve.  Nothing is placed:
-        records, snapshot, the last batch and its explanations stay as they are."""
-        src = _source(source)
-        pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
-        now = np.ascontiguousarray(now, dtype='<f8')
-        assert len(pods) == len(now)
-        ex = np.ascontiguousarray(exclude, dtype='<i4').reshape(-1)
-        if out is None:
-            out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
-        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
-        self._ck(self._L.nhd_plan_batch(self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods),
-                                        pods.ctypes.data, now.ctypes.data, out.ctypes.data,
-                                        counts.ctypes.data if explain else None))
+        """A dry run of ``solve_batch``: the bindings the pods would get scheduled in order, each seeing the ones before
+        it, on the current records (``source='mirror'``) or on those of the last ``snapshot()`` (``'snapshot'``), with
+        the node indices ``exclude`` taken as in maintenance.  With ``explain=True`` returns ``(bindings, counts)``,
+        counts being what ``explain_batch`` would return after that solve.  Nothing is placed: records, snapshot, the
+        last batch and its explanations stay as they are."""
+        out, _, counts = self._plan_batch(pods, now, source, exclude, explain, out)
         return (out, counts) if explain else out
 
     def plan_batch_rounds(self, pods, now, round_clocks, source='mirror', exclude=(), explain=False):
-        """``plan_batch`` over several pending scans (``nhd_plan_batch_rounds``): after the dry run of the batch, at each
-        clock of ``round_clocks`` (never going down, none before a pod clock) the pods not placed yet are solved again
-        in order on the records the previous scan left, the nodes ``exclude`` in maintenance throughout.  Returns
-        ``(bindings, pod_round)``: each pod's last attempt and the round that placed it, or ``len(round_clocks)`` if
-        none did; ``explain=True``: ``(bindings, pod_round, counts)``, ``counts`` the per-reason node counts of the pods
-        whose last attempt found no node, at that attempt.  The same answer as ``plan_scenarios`` with this one scenario
-        and rounds, from the batch path: meant for one large pending set.  Nothing is placed."""
-        src = _source(source)
-        pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
-        now = np.ascontiguousarray(now, dtype='<f8')
-        assert len(pods) == len(now)
-        ex = np.ascontiguousarray(exclude, dtype='<i4').reshape(-1)
-        clocks = np.ascontiguousarray(round_clocks, dtype='<f8').reshape(-1)
-        out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
-        pod_round = np.zeros(len(pods), dtype='<i4')
-        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
-        self._ck(self._L.nhd_plan_batch_rounds(self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods),
-                                               pods.ctypes.data, now.ctypes.data, len(clocks),
-                                               clocks.ctypes.data if len(clocks) else None, out.ctypes.data,
-                                               counts.ctypes.data if explain else None, pod_round.ctypes.data))
+        """``plan_batch`` over several pending scans: after the dry run of the batch, at each clock of ``round_clocks``
+        (never going down, none before a pod clock) the pods not placed yet are solved again in order on the records the
+        previous scan left, the nodes ``exclude`` in maintenance throughout.  Returns ``(bindings, pod_round)``: each
+        pod's last attempt and the round that placed it, or ``len(round_clocks)`` if none did; ``explain=True``:
+        ``(bindings, pod_round, counts)``, ``counts`` the per-reason node counts of the pods whose last attempt found no
+        node, at that attempt.  The same answer as ``plan_scenarios`` with this one scenario and rounds, from the batch
+        path: meant for one large pending set.  Nothing is placed."""
+        out, pod_round, counts = self._plan_batch(pods, now, source, exclude, explain, round_clocks=round_clocks)
         return (out, pod_round, counts) if explain else (out, pod_round)
 
     def plan_batch_releases(self, pods, now, round_clocks, tracked, pods_used, releases, source='mirror', exclude=(),
                             explain=False):
-        """``plan_batch_rounds`` with deployed pods ending between the scans (``nhd_plan_batch_releases``).
-        ``releases``: ``wire.RELEASE_DTYPE`` records, each applied before its ``round`` (1 .. ``len(round_clocks)``),
-        in array order, clocks never going down.  ``tracked``: the node indices whose signed NIC pod counters the plan
-        carries, every released node among them; ``pods_used``: ``(len(tracked), MAX_NICS)`` counters at plan start.
-        Returns what ``plan_batch_rounds`` returns.  Nothing is placed."""
+        """``plan_batch_rounds`` with deployed pods ending between the scans.  ``releases``: ``wire.RELEASE_DTYPE``
+        records, each applied before its ``round`` (1 .. ``len(round_clocks)``), in array order, clocks never going
+        down.  ``tracked``: the node indices whose signed NIC pod counters the plan carries, every released node among
+        them; ``pods_used``: ``(len(tracked), MAX_NICS)`` counters at plan start.  Returns what ``plan_batch_rounds``
+        returns.  Nothing is placed."""
+        out, pod_round, counts = self._plan_batch(pods, now, source, exclude, explain, round_clocks=round_clocks,
+                                                  tracked=tracked, pods_used=pods_used, releases=releases)
+        return (out, pod_round, counts) if explain else (out, pod_round)
+
+    def _plan_batch(self, pods, now, source, exclude, explain, out=None, round_clocks=None, tracked=(), pods_used=(),
+                    releases=None):
+        """The three ``plan_batch*`` methods as one ``nhd_plan_batch_releases`` call (no rounds, no tracked nodes and no
+        releases are what the two narrower entry points pass): ``(bindings, pod_round, counts or None)``, ``pod_round``
+        None without ``round_clocks``."""
         src = _source(source)
         pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
         now = np.ascontiguousarray(now, dtype='<f8')
         assert len(pods) == len(now)
         ex = np.ascontiguousarray(exclude, dtype='<i4').reshape(-1)
-        clocks = np.ascontiguousarray(round_clocks, dtype='<f8').reshape(-1)
+        clocks = np.ascontiguousarray(() if round_clocks is None else round_clocks, dtype='<f8').reshape(-1)
         tr = np.ascontiguousarray(tracked, dtype='<i4').reshape(-1)
         used = np.ascontiguousarray(pods_used, dtype='<i2').reshape(len(tr), wire.MAX_NICS)
-        rel = np.ascontiguousarray(releases, dtype=wire.RELEASE_DTYPE).reshape(-1)
-        out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
-        pod_round = np.zeros(len(pods), dtype='<i4')
+        rel = (np.zeros(0, dtype=wire.RELEASE_DTYPE) if releases is None else
+               np.ascontiguousarray(releases, dtype=wire.RELEASE_DTYPE).reshape(-1))
+        if out is None:
+            out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
+        pod_round = None if round_clocks is None else np.zeros(len(pods), dtype='<i4')
         counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
         self._ck(self._L.nhd_plan_batch_releases(self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods),
                                                  pods.ctypes.data, now.ctypes.data, len(clocks),
@@ -272,62 +281,52 @@ class Solver:
                                                  tr.ctypes.data if len(tr) else None,
                                                  used.ctypes.data if len(tr) else None, len(rel),
                                                  rel.ctypes.data if len(rel) else None, out.ctypes.data,
-                                                 counts.ctypes.data if explain else None, pod_round.ctypes.data))
-        return (out, pod_round, counts) if explain else (out, pod_round)
+                                                 counts.ctypes.data if explain else None,
+                                                 None if pod_round is None else pod_round.ctypes.data))
+        return out, pod_round, counts
 
     def plan_scenarios(self, scenarios, source='mirror', explain=False):
-        """Many independent dry runs in one call (``nhd_plan_scenarios_edited``).  ``scenarios``: a sequence of
-        ``(exclude, pods, now[, lift[, edits]])``.  Returns one ``(code, pod, bindings)`` per scenario: ``code`` 0 and
-        ``bindings`` what ``plan_batch(pods, now, source, exclude)`` returns, or the refusal ``plan_batch`` would raise
-        (``wire.ERR_*``), the index of the pod it names and None.  ``explain=True`` (``nhd_plan_scenarios_explained``):
-        one ``(code, pod, bindings, counts)`` per scenario, ``counts`` a ``(n_s, wire.WHY_COUNT)`` uint32 array of
-        per-reason node counts for the NO_CANDIDATE pods at the state each saw (zero rows for the others), as
-        ``plan_batch(..., explain=True)`` gives them, or None when refused.  Scenarios do not see each other.  Unlike
-        ``plan_batch`` the tuple limits are judged with the excluded nodes counted; ``plan_batch`` plans a scenario
-        refused for that.
-        ``lift`` (None: never): the excluded nodes are back in service from the scenario's pod ``lift`` on.  ``edits``
-        (None: none): ``(nodes, records)``, node indices and a ``wire.NODE_DTYPE`` array, the records those nodes have
-        for the whole scenario.  With either, the bindings are those of ``solve_batch`` on a scratch copy of the records
-        with the edits applied, the excluded nodes in maintenance for the pods before ``lift`` and back after.
-        ``adds`` (sixth element, None: none): ``(at, records)``, int positions and a ``wire.NODE_DTYPE`` array: nodes
-        added for the whole scenario, each right before source node ``at[k]`` (``n_nodes``: at the end), ``at`` never
-        going down (``nhd_plan_scenarios_grown``).  A pod placed on one gets node ``n_nodes + a``, ``a`` its index among
-        the added records of the whole call, in scenario order.
-        ``rounds`` (seventh element, None: none): the clocks of later pending scans, never going down and none before
-        the scenario's pod clocks (``nhd_plan_scenarios_rounds``).  At each, the scenario's pods not placed yet are
-        solved again in order on the records the previous scan left; ``bindings`` hold each pod's last attempt.  When
-        any scenario has rounds, each result gains a last element: the ``(n_s,)`` int32 round that placed each pod, or
+        """Many independent dry runs in one call.  ``scenarios``: a sequence of ``Scenario`` records, or plain tuples of
+        their fields in order (``(exclude, pods, now[, lift[, edits[, adds[, rounds]]]])``).  Returns one ``(code, pod,
+        bindings)`` per scenario: ``code`` 0 and ``bindings`` what ``plan_batch(pods, now, source, exclude)`` returns,
+        or the refusal ``plan_batch`` would raise (``wire.ERR_*``), the index of the pod it names and None.
+        ``explain=True``: one ``(code, pod, bindings, counts)`` per scenario, ``counts`` a ``(n_s, wire.WHY_COUNT)``
+        uint32 array of per-reason node counts for the NO_CANDIDATE pods at the state each saw (zero rows for the
+        others), as ``plan_batch(..., explain=True)`` gives them, or None when refused.  Scenarios do not see each
+        other.  Unlike ``plan_batch`` the tuple limits are judged with the excluded nodes counted; ``plan_batch`` plans
+        a scenario refused for that.  With ``lift``, ``edits`` or ``adds`` the bindings are those of ``solve_batch`` on
+        a scratch copy of the records with the edits applied and the additions inserted, the excluded nodes in
+        maintenance for the pods before ``lift`` and back after.  A pod placed on an added node gets node
+        ``n_nodes + a``, ``a`` its index among the added records of the whole call, in scenario order.  When any
+        scenario has ``rounds``, each result gains a last element: the ``(n_s,)`` int32 round that placed each pod, or
         ``len(rounds)`` if none did (None when refused)."""
         src = _source(source)
         # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
         # would cost more than the call itself)
         exs, podb, nowl, lifts, ednodes, edrecs, n_adds, adats, adrecs, rounds = [], [], [], [], [], [], [], [], [], []
         for sc in scenarios:
-            exclude, pods, now = sc[:3]
-            lift = sc[3] if len(sc) > 3 else None
-            edits = sc[4] if len(sc) > 4 else None
-            adds = sc[5] if len(sc) > 5 else None
-            rounds.append(sc[6] if len(sc) > 6 else None)
-            pods = np.asarray(pods)
+            sc = Scenario(*sc)
+            rounds.append(sc.rounds)
+            pods = np.asarray(sc.pods)
             if pods.dtype != wire.POD_DTYPE:
                 pods = pods.astype(wire.POD_DTYPE)
-            exs.append(np.asarray(exclude, dtype='<i4').reshape(-1))
+            exs.append(np.asarray(sc.exclude, dtype='<i4').reshape(-1))
             podb.append(np.ascontiguousarray(pods).tobytes())
-            nowl.append(np.asarray(now, dtype='<f8').reshape(-1))
+            nowl.append(np.asarray(sc.now, dtype='<f8').reshape(-1))
             assert pods.size == len(nowl[-1])
-            lifts.append(len(nowl[-1]) if lift is None else int(lift))
-            if edits is None:
+            lifts.append(len(nowl[-1]) if sc.lift is None else int(sc.lift))
+            if sc.edits is None:
                 ednodes.append(np.zeros(0, dtype='<i4'))
             else:
-                nodes, recs = edits
+                nodes, recs = sc.edits
                 ednodes.append(np.asarray(nodes, dtype='<i4').reshape(-1))
                 recs = np.asarray(recs, dtype=wire.NODE_DTYPE).reshape(-1)
                 assert len(recs) == len(ednodes[-1])
                 edrecs.append(recs.tobytes())
-            if adds is None:
+            if sc.adds is None:
                 n_adds.append(0)
             else:
-                at, recs = adds
+                at, recs = sc.adds
                 adats.append(np.asarray(at, dtype='<i4').reshape(-1))
                 recs = np.asarray(recs, dtype=wire.NODE_DTYPE).reshape(-1)
                 assert len(recs) == len(adats[-1])
@@ -349,12 +348,9 @@ class Solver:
         out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
         status = np.zeros(n, dtype='<i4')
         which = np.zeros(n, dtype='<i4')
-        head = (self._h, src, n, excl_start.ctypes.data, ex.ctypes.data if len(ex) else None,
-                lift.ctypes.data if n else None, edit_start.ctypes.data, ednode.ctypes.data if len(ednode) else None,
-                edrec.ctypes.data if len(edrec) else None)
-        tail = (pod_start.ctypes.data, pods.ctypes.data if len(pods) else None, now.ctypes.data if len(pods) else None,
-                out.ctypes.data if len(pods) else None, status.ctypes.data, which.ctypes.data)
-        adds = (None, None, None)
+        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
+        # NULL addition and round arrays unless some scenario has them: round_start selects the round kernel
+        adds, rnds, pod_round = (None, None, None), (None, None), None
         if any(n_adds):
             add_start = np.zeros(n + 1, dtype='<i4')
             add_start[1:] = np.cumsum(n_adds)
@@ -366,27 +362,21 @@ class Solver:
             round_start = np.zeros(n + 1, dtype='<i4')
             round_start[1:] = np.cumsum([len(c) for c in clocks])
             round_clock = np.ascontiguousarray(np.concatenate(clocks), dtype='<f8')
-            counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
+            rnds = (round_start.ctypes.data, round_clock.ctypes.data if len(round_clock) else None)
             pod_round = np.zeros(len(pods), dtype='<i4')
-            self._ck(self._L.nhd_plan_scenarios_rounds(*head, *adds, *tail[:3], round_start.ctypes.data,
-                                                       round_clock.ctypes.data if len(round_clock) else None, *tail[3:],
-                                                       counts.ctypes.data if explain and len(pods) else None,
-                                                       pod_round.ctypes.data if len(pods) else None))
-            res = self._scenario_results(status, which, pod_start, out, counts)
-            return [r + (pod_round[a:b] if r[0] == 0 else None,)
-                    for r, a, b in zip(res, pod_start[:-1].tolist(), pod_start[1:].tolist())]
-        if any(n_adds):
-            counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
-            self._ck(self._L.nhd_plan_scenarios_grown(*head, *adds, *tail,
-                                                      counts.ctypes.data if explain and len(pods) else None))
-            return self._scenario_results(status, which, pod_start, out, counts)
-        args = head + tail
-        if not explain:
-            self._ck(self._L.nhd_plan_scenarios_edited(*args))
-            return self._scenario_results(status, which, pod_start, out, None)
-        counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4')
-        self._ck(self._L.nhd_plan_scenarios_explained(*args, counts.ctypes.data if len(pods) else None))
-        return self._scenario_results(status, which, pod_start, out, counts)
+        some = len(pods) > 0
+        self._ck(self._L.nhd_plan_scenarios_rounds(
+            self._h, src, n, excl_start.ctypes.data, ex.ctypes.data if len(ex) else None,
+            lift.ctypes.data if n else None, edit_start.ctypes.data, ednode.ctypes.data if len(ednode) else None,
+            edrec.ctypes.data if len(edrec) else None, *adds, pod_start.ctypes.data, pods.ctypes.data if some else None,
+            now.ctypes.data if some else None, *rnds, out.ctypes.data if some else None, status.ctypes.data,
+            which.ctypes.data, counts.ctypes.data if explain and some else None,
+            pod_round.ctypes.data if pod_round is not None and some else None))
+        res = self._scenario_results(status, which, pod_start, out, counts)
+        if pod_round is None:
+            return res
+        return [r + (pod_round[a:b] if r[0] == 0 else None,)
+                for r, a, b in zip(res, pod_start[:-1].tolist(), pod_start[1:].tolist())]
 
     @staticmethod
     def _scenario_results(status, which, pod_start, out, counts):

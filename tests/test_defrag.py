@@ -23,47 +23,13 @@ from tests import helpers, scenarios
 from tests.golden import make_live_golden
 from tests.golden.make_defrag_golden import defrag_sessions
 from tests.golden.make_plan_golden import mirror_session
-from tests.test_drains import OracleDrainSolver
-from tests.test_plan import _emu_lib, _four_numa, _gpu_factory, excluded
+from nhd_b200.solver import Scenario
+from tests.plan_oracle import OraclePlanner, excluded, oracle_scenario
+from tests.test_plan import _emu_lib, _four_numa, _gpu_factory
 from tests.test_query import MODES, _filter_words, _gpu_cases, oracle_state, packed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
-
-
-def oracle_defrag(recs, speed, pods, now, exclude=(), lift=None, edits=None, busy=30.0, threads=1):
-    """The five steps with the C oracle on a copy of ``recs``: the edits applied, the excluded nodes in maintenance,
-    pods ``[0, lift)`` solved, the excluded nodes' flags put back, pods ``[lift, n)`` solved."""
-    from oracle import binding
-    r = np.ascontiguousarray(recs, dtype=wire.NODE_DTYPE).copy()
-    if edits is not None and len(edits[0]):
-        r[np.asarray(edits[0], dtype=np.int64)] = edits[1]
-    ex = np.unique(np.asarray(list(exclude), dtype=np.int64))
-    lift = len(pods) if lift is None else lift
-    flags = r['flags'][ex].copy()
-    r = excluded(r, ex)
-    out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
-    if lift:
-        out[:lift], r = binding.solve(r, speed, pods[:lift], now[:lift], min_busy_secs=busy, threads=threads)
-    r['flags'][ex] = flags
-    if lift < len(pods):
-        out[lift:] = binding.solve(r, speed, pods[lift:], now[lift:], min_busy_secs=busy, threads=threads)[0]
-    return out
-
-
-class OracleDefragSolver(OracleDrainSolver):
-    """The oracle stand-in with edited scenarios: the five steps per scenario.  TEST INFRASTRUCTURE."""
-
-    def plan_scenarios(self, scenarios, source='mirror'):
-        recs = self._snap if source == 'snapshot' else self._recs
-        return [(0, -1, oracle_defrag(recs, self._speed, np.asarray(sc[1]), np.asarray(sc[2], dtype='<f8'),
-                                      [int(i) for i in sc[0]], *sc[3:5], busy=self._min_busy))
-                for sc in scenarios]
-
-
-def _sc(sc):
-    """``(exclude, pods, now, lift, edits)`` of a scenario tuple of any length."""
-    return tuple(sc[:3]) + (sc[3] if len(sc) > 3 else None, sc[4] if len(sc) > 4 else None)
 
 
 def defrag_scenarios(recs0, pods, now, nodes_of, rest, busy):
@@ -111,12 +77,12 @@ def defrag_scenarios(recs0, pods, now, nodes_of, rest, busy):
 def check_against_oracle(got, scens, st, speed, busy, where=''):
     n = 0
     for j, (sc, (code, pod, b)) in enumerate(zip(scens, got)):
-        ex, p, c, lift, edits = _sc(sc)
-        assert code == 0 and pod == -1 and len(b) == len(p), (where, j, code, pod)
-        if len(p):
-            want = oracle_defrag(st, speed, p, c, [int(i) for i in ex], lift, edits, busy)
+        sc = Scenario(*sc)
+        assert code == 0 and pod == -1 and len(b) == len(sc.pods), (where, j, code, pod)
+        if len(sc.pods):
+            want = oracle_scenario(st, speed, sc, busy=busy)[0]
             assert b.tobytes() == want.tobytes(), (where, j, helpers.first_binding_diff(want, b))
-        n += len(p)
+        n += len(sc.pods)
     return n
 
 
@@ -224,7 +190,7 @@ def _defrag_against_the_reference(factory):
 def test_plan_defrag_equals_the_reference_defrag():
     """Where the reference puts a drained node's pods and then the pending pods, answered before any drain by
     ``PlanDefrag`` with the oracle standing in for the GPU."""
-    _defrag_against_the_reference(OracleDefragSolver)
+    _defrag_against_the_reference(OraclePlanner)
 
 
 # ---------------------------------------------------------------------------------------------- CPU: emulated device
@@ -284,7 +250,8 @@ def five_steps(scratch, scens):
     nodes in maintenance, the pods before the lift, the excluded nodes' flags back, the rest of the pods."""
     out = []
     for sc in scens:
-        ex, p, c, lift, edits = _sc(sc)
+        sc = Scenario(*sc)
+        ex, p, c, lift, edits = sc.exclude, sc.pods, sc.now, sc.lift, sc.edits
         scratch.restore()
         if edits is not None and len(edits[0]):
             scratch.update_nodes(np.asarray(edits[0], dtype='<i4'), edits[1])
@@ -448,9 +415,8 @@ def test_config4_full_size():
         s.close()
         scratch.close()
     for sc, (code, _, b) in zip(sample, got):
-        ex, p, c, lift, edits = _sc(sc)
-        want = oracle_defrag(after, speed, p, c, ex, lift, edits, 30.0, threads=os.cpu_count() or 1)
-        assert code == 0 and b.tobytes() == want.tobytes(), (ex, helpers.first_binding_diff(want, b))
+        want = oracle_scenario(after, speed, sc, threads=os.cpu_count() or 1)[0]
+        assert code == 0 and b.tobytes() == want.tobytes(), (sc[0], helpers.first_binding_diff(want, b))
 
 
 @pytest.mark.gpu

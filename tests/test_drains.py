@@ -21,18 +21,12 @@ from nhd_b200 import wire
 from tests import helpers, scenarios
 from tests.golden import make_live_golden
 from tests.golden.make_plan_golden import drain_sessions, mirror_session
-from tests.test_plan import OraclePlanSolver, _emu_lib, _gpu_factory, oracle_plan
+from tests.plan_oracle import OraclePlanner, oracle_scenario
+from tests.test_plan import _emu_lib, _gpu_factory
 from tests.test_query import MODES, _filter_words, _gpu_cases, oracle_state, packed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
-
-
-class OracleDrainSolver(OraclePlanSolver):
-    """The oracle stand-in with scenario plans: one oracle plan per scenario.  TEST INFRASTRUCTURE."""
-
-    def plan_scenarios(self, scenarios, source='mirror'):
-        return [(0, -1, self.plan_batch(pods, now, source=source, exclude=ex)) for ex, pods, now in scenarios]
 
 
 def drain_scenarios(recs, pods, now, nodes_of, rest=None):
@@ -81,7 +75,7 @@ def check_against_oracle(got, scens, refused, st, speed, busy, where=''):
             continue
         assert code == 0 and pod == -1 and len(b) == len(p), (where, j, code, pod)
         if len(p):
-            want = oracle_plan(st, speed, p, c, [int(i) for i in ex], busy)[0]
+            want = oracle_scenario(st, speed, (ex, p, c), busy=busy, explain=True)[0]
             assert b.tobytes() == want.tobytes(), (where, j, list(ex), helpers.first_binding_diff(want, b))
         n += len(p)
     return n
@@ -131,12 +125,12 @@ def _drains_against_the_reference(factory):
 def test_plan_drains_equals_the_reference_drains():
     """Where the reference re-schedules the pods of each drained node, answered before any drain by ``PlanDrains``
     with the oracle standing in for the GPU."""
-    _drains_against_the_reference(OracleDrainSolver)
+    _drains_against_the_reference(OraclePlanner)
 
 
 def test_plan_drains_equals_plan_drain_per_group():
     """``PlanDrains(groups)[g]`` is ``PlanDrain(g)[0]`` from the same state, for single nodes and pairs."""
-    _drains_equal_plan_drain(OracleDrainSolver, drain_sessions()[:4])
+    _drains_equal_plan_drain(OraclePlanner, drain_sessions()[:4])
 
 
 def _drains_equal_plan_drain(factory, sessions):
@@ -463,7 +457,7 @@ def test_config4_full_size():
     finally:
         s.close()
     for (ex, p, c), (code, _, b) in zip(sample, got):
-        want = oracle_plan(after, speed, p, c, ex, threads=os.cpu_count() or 1)[0]
+        want = oracle_scenario(after, speed, (ex, p, c), threads=os.cpu_count() or 1, explain=True)[0]
         assert code == 0 and b.tobytes() == want.tobytes(), (ex, helpers.first_binding_diff(want, b))
 
 

@@ -21,77 +21,14 @@ import numpy as np
 import pytest
 
 from nhd_b200 import wire
+from nhd_b200.solver import Scenario
 from tests import helpers
-from tests.test_defrag import OracleDefragSolver, oracle_defrag
+from tests.plan_oracle import OraclePlanner, grown, mapped, oracle_scenario
 from tests.test_plan import _emu_lib, _gpu_factory
-from tests.test_plan_reasons import oracle_explained
 from tests.test_query import MODES, _filter_words, _gpu_cases, oracle_state, packed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
-
-
-def _sc(sc):
-    """``(exclude, pods, now, lift, edits, adds)`` of a scenario tuple of any length."""
-    return tuple(sc[:3]) + tuple(sc[k] if len(sc) > k else None for k in (3, 4, 5))
-
-
-def grown(recs, edits=None, adds=None, base=0):
-    """The grown scratch records of a scenario: ``recs`` with the edits applied and the added records inserted, each
-    right before source node ``at`` (added nodes at one position in array order).  Returns ``(records, ids)``, ``ids``
-    the index each grown node reports: its source index, or ``len(recs) + base + k`` for the scenario's k-th
-    addition (``base``: the additions of the call before this scenario)."""
-    r = np.ascontiguousarray(recs, dtype=wire.NODE_DTYPE).copy()
-    if edits is not None and len(edits[0]):
-        r[np.asarray(edits[0], dtype=np.int64)] = edits[1]
-    at, arecs = (np.zeros(0, dtype=np.int64), r[:0]) if adds is None else adds
-    at = np.asarray(at, dtype=np.int64)
-    assert (np.diff(at) >= 0).all()
-    n = len(r)
-    ids = np.arange(n, dtype=np.int64)
-    if len(at):
-        ids = np.insert(ids, at, n + base + np.arange(len(at)))    # each in front of source node at[k]
-    out = np.zeros(len(ids), dtype=wire.NODE_DTYPE)
-    src = ids < n
-    out[src] = r
-    out[~src] = np.asarray(arecs, dtype=wire.NODE_DTYPE)[ids[~src] - n - base]
-    return out, ids
-
-
-def _mapped(b, ids):
-    b = b.copy()
-    on = b['node'] >= 0
-    b['node'][on] = ids[b['node'][on]]
-    return b
-
-
-def oracle_grown(recs, speed, pods, now, exclude=(), lift=None, edits=None, adds=None, base=0, busy=30.0, threads=1,
-                 explain=False):
-    """The five steps with the C oracle on the grown copy, node indices mapped back: the bindings, or
-    ``(bindings, counts)`` with ``explain``."""
-    g, ids = grown(recs, edits, adds, base)
-    where = np.flatnonzero(ids < len(recs))                            # grown position of each source node
-    ex = [int(where[int(i)]) for i in exclude]
-    if explain:
-        out, counts = oracle_explained(g, speed, pods, now, ex, lift, None, busy, threads)
-        return _mapped(out, ids), counts
-    return _mapped(oracle_defrag(g, speed, pods, now, ex, lift, None, busy, threads), ids)
-
-
-class OracleExpandSolver(OracleDefragSolver):
-    """The oracle stand-in with grown scenarios: the five steps on the grown records per scenario, indices mapped
-    back.  TEST INFRASTRUCTURE."""
-
-    def plan_scenarios(self, scenarios, source='mirror', explain=False):
-        recs = self._snap if source == 'snapshot' else self._recs
-        out, base = [], 0
-        for sc in scenarios:
-            ex, pods, now, lift, edits, adds = _sc(sc)
-            r = oracle_grown(recs, self._speed, np.asarray(pods), np.asarray(now, dtype='<f8'), [int(i) for i in ex],
-                             lift, edits, adds, base, self._min_busy, explain=explain)
-            out.append((0, -1) + (r if explain else (r,)))
-            base += 0 if adds is None else len(adds[0])
-        return out
 
 
 # ---------------------------------------------------------------------------------------------- scenario families
@@ -167,23 +104,21 @@ def check_against_oracle(got, scens, st, speed, busy, where='', explain=False, r
     and the pods placed on added nodes."""
     n = on_added = base = 0
     for j, (sc, g) in enumerate(zip(scens, got)):
-        ex, p, c, lift, edits, adds = _sc(sc)
+        sc = Scenario(*sc)
+        adds = sc.adds
         if j in refused:
             assert g[0] == refused[j][0] and g[1] == refused[j][1] and g[2] is None, (where, j, g[:2])
         else:
-            assert g[0] == 0 and g[1] == -1 and len(g[2]) == len(p), (where, j, g[:2])
-            if len(p):
-                want = oracle_grown(st, speed, p, c, [int(i) for i in ex], lift, edits, adds, base, busy,
-                                    explain=explain)
-                b = want[0] if explain else want
+            assert g[0] == 0 and g[1] == -1 and len(g[2]) == len(sc.pods), (where, j, g[:2])
+            if len(sc.pods):
+                b, _, rows, _ = oracle_scenario(st, speed, sc, base, busy, explain=explain)
                 assert g[2].tobytes() == b.tobytes(), (where, j, helpers.first_binding_diff(b, g[2]))
                 if explain:
-                    rows = want[1]
                     bad = (g[3] != rows).any(1)
                     assert not bad.any(), (where, j, np.flatnonzero(bad), g[3][bad][:2], rows[bad][:2])
                     none = g[2]['status'] == wire.NO_CANDIDATE
                     assert (g[3][none].sum(1) == len(st) + (0 if adds is None else len(adds[0]))).all(), (where, j)
-            n += len(p)
+            n += len(sc.pods)
             on_added += int((g[2]['node'] >= len(st)).sum())
         base += 0 if adds is None else len(adds[0])
     return n, on_added
@@ -193,24 +128,24 @@ def _raw(s, scens, add_start=True, fill=None):
     """``nhd_plan_scenarios_grown`` itself (``add_start=False``: NULL), with a per-scenario list of ``(exclude, pods,
     now, lift, edits, adds)``: ``(rc, status, which, out, counts)``."""
     n = len(scens)
-    parts = [_sc(sc) for sc in scens]
+    parts = [Scenario(*sc) for sc in scens]
     cat = lambda xs, dt: np.ascontiguousarray(np.concatenate(xs) if xs else np.zeros(0), dtype=dt)  # noqa: E731
     off = lambda ls: np.concatenate([[0], np.cumsum(ls)]).astype('<i4')                           # noqa: E731
-    ex = cat([np.asarray(p[0], dtype='<i4').reshape(-1) for p in parts], '<i4')
-    pods = cat([p[1] for p in parts], wire.POD_DTYPE)
-    now = cat([np.asarray(p[2], dtype='<f8') for p in parts], '<f8')
-    lift = np.asarray([len(p[1]) if p[3] is None else p[3] for p in parts], dtype='<i4')
-    edn = cat([np.asarray([] if p[4] is None else p[4][0], dtype='<i4') for p in parts], '<i4')
-    edr = cat([p[4][1] for p in parts if p[4] is not None], wire.NODE_DTYPE)
-    adat = cat([np.asarray([] if p[5] is None else p[5][0], dtype='<i4') for p in parts], '<i4')
-    adr = cat([p[5][1] for p in parts if p[5] is not None], wire.NODE_DTYPE)
+    ex = cat([np.asarray(p.exclude, dtype='<i4').reshape(-1) for p in parts], '<i4')
+    pods = cat([p.pods for p in parts], wire.POD_DTYPE)
+    now = cat([np.asarray(p.now, dtype='<f8') for p in parts], '<f8')
+    lift = np.asarray([len(p.pods) if p.lift is None else p.lift for p in parts], dtype='<i4')
+    edn = cat([np.asarray([] if p.edits is None else p.edits[0], dtype='<i4') for p in parts], '<i4')
+    edr = cat([p.edits[1] for p in parts if p.edits is not None], wire.NODE_DTYPE)
+    adat = cat([np.asarray([] if p.adds is None else p.adds[0], dtype='<i4') for p in parts], '<i4')
+    adr = cat([p.adds[1] for p in parts if p.adds is not None], wire.NODE_DTYPE)
     out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
     status, which = np.zeros(n, dtype='<i4'), np.zeros(n, dtype='<i4')
     counts = None if fill is None else np.full((len(pods), wire.WHY_COUNT), fill, dtype='<u4')
     ptr = lambda a: a.ctypes.data if a is not None and len(a) else None                           # noqa: E731
-    excl_start, pod_start = off([len(p[0]) for p in parts]), off([len(p[1]) for p in parts])
-    edit_start = off([0 if p[4] is None else len(p[4][0]) for p in parts])
-    astart = off([0 if p[5] is None else len(p[5][0]) for p in parts])
+    excl_start, pod_start = off([len(p.exclude) for p in parts]), off([len(p.pods) for p in parts])
+    edit_start = off([0 if p.edits is None else len(p.edits[0]) for p in parts])
+    astart = off([0 if p.adds is None else len(p.adds[0]) for p in parts])
     rc = s._L.nhd_plan_scenarios_grown(s._h, 0, n, excl_start.ctypes.data, ptr(ex), lift.ctypes.data,
                                        edit_start.ctypes.data, ptr(edn), ptr(edr),
                                        astart.ctypes.data if add_start else None, ptr(adat), ptr(adr),
@@ -332,7 +267,7 @@ def _expand_against_the_reference(factory):
 def test_plan_expansion_equals_the_reference_with_the_nodes_added():
     """Where the reference puts the pending pods with candidate nodes inserted into its node dict, and its drop
     decisions for those left without a node, answered by ``PlanExpansion`` with the oracle standing in for the GPU."""
-    _expand_against_the_reference(OracleExpandSolver)
+    _expand_against_the_reference(OraclePlanner)
 
 
 def test_grown_records_put_added_nodes_in_front_of_their_position():
@@ -406,8 +341,9 @@ def five_steps_grown(scratch, st, scens, which=None):
     node indices mapped back."""
     out, base = {}, 0
     for j, sc in enumerate(scens):
-        ex, p, c, lift, edits, adds = _sc(sc)
-        g, ids = grown(st, edits, adds, base)
+        sc = Scenario(*sc)
+        ex, p, c, lift, adds = sc.exclude, sc.pods, sc.now, sc.lift, sc.adds
+        g, ids = grown(st, sc.edits, adds, base)
         base += 0 if adds is None else len(adds[0])
         if which is not None and j not in which:
             continue
@@ -425,7 +361,7 @@ def five_steps_grown(scratch, st, scens, which=None):
             scratch.update_nodes(ex, back)
         if lift < len(p):
             b.append(scratch.solve_batch(p[lift:], c[lift:]))
-        out[j] = _mapped(np.concatenate(b), ids) if b else np.zeros(0, dtype=wire.BINDING_DTYPE)
+        out[j] = mapped(np.concatenate(b), ids) if b else np.zeros(0, dtype=wire.BINDING_DTYPE)
     return [out[j] for j in sorted(out)] if which is None else out
 
 
@@ -568,8 +504,8 @@ def test_config4_full_size():
         scratch.close()
     base = 0
     for sc, g in zip(scens, got):
-        ex, p, c, lift, edits, adds = _sc(sc)
-        w = oracle_grown(after, speed, p, c, ex, lift, edits, adds, base, 30.0, threads=os.cpu_count() or 1)
+        adds = Scenario(*sc).adds
+        w = oracle_scenario(after, speed, sc, base, threads=os.cpu_count() or 1)[0]
         assert g[0] == 0 and g[2].tobytes() == w.tobytes(), (len(adds[0]), helpers.first_binding_diff(w, g[2]))
         base += len(adds[0])
 

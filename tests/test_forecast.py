@@ -22,85 +22,15 @@ import numpy as np
 import pytest
 
 from nhd_b200 import wire
+from nhd_b200.solver import Scenario
 from tests import helpers
-from tests.test_expand import OracleExpandSolver, _mapped, _raw as _raw_grown, expand_scenarios, grown
-from tests.test_plan import _emu_lib, _gpu_factory, excluded
+from tests.plan_oracle import OraclePlanner, grown, mapped, oracle_scenario
+from tests.test_expand import _raw as _raw_grown, expand_scenarios
+from tests.test_plan import _emu_lib, _gpu_factory
 from tests.test_query import MODES, _filter_words, _gpu_cases, oracle_state, packed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
-
-
-def _sc(sc):
-    """``(exclude, pods, now, lift, edits, adds, rounds)`` of a scenario tuple of any length."""
-    return tuple(sc[:3]) + tuple(sc[k] if len(sc) > k else None for k in (3, 4, 5, 6))
-
-
-def oracle_rounds(recs, speed, pods, now, exclude=(), lift=None, edits=None, adds=None, rounds=None, base=0, busy=30.0,
-                  threads=1, explain=False):
-    """The five steps with the C oracle on the grown copy, then per round clock the pods not placed yet solved again in
-    order (exclusions held at the last pod held again): ``(bindings, pod_round, counts or None, touched)``, node
-    indices mapped back; ``touched`` the grown nodes any attempt chose."""
-    from oracle import binding
-    from tests import explain_oracle
-    g, ids = grown(recs, edits, adds, base)
-    where = np.flatnonzero(ids < len(recs))
-    ex = np.unique(where[np.asarray(list(exclude), dtype=np.int64)])
-    n = len(pods)
-    lift = n if lift is None else lift
-    rounds = [] if rounds is None else [float(c) for c in rounds]
-    kw = dict(min_busy_secs=busy, threads=threads)
-    out = np.zeros(n, dtype=wire.BINDING_DTYPE)
-    counts = np.zeros((n, wire.WHY_COUNT), dtype='<u4')
-    touched = set()
-
-    def phase(r, idx, clocks):
-        if explain:
-            _, why = explain_oracle.batch(r, speed, pods[idx], clocks, **kw)
-            counts[idx] = explain_oracle.counts(why, len(idx))
-        b, r = binding.solve(r, speed, pods[idx], clocks, **kw)
-        out[idx] = b
-        touched.update(int(x) for x in b['node'] if x >= 0)
-        return r
-    r = g.copy()
-    flags = r['flags'][ex].copy()
-    r = excluded(r, ex)
-    if lift:
-        r = phase(r, np.arange(lift), now[:lift])
-    r['flags'][ex] = flags
-    if lift < n:
-        r = phase(r, np.arange(lift, n), now[lift:])
-    pod_round = np.where(out['status'] == wire.PLACED, 0, len(rounds)).astype('<i4')
-    for k, c in enumerate(rounds, 1):
-        idx = np.flatnonzero(out['status'] != wire.PLACED)
-        if not len(idx):
-            continue
-        held = r['flags'][ex].copy()
-        if lift == n:
-            r = excluded(r, ex)
-        r = phase(r, idx, np.full(len(idx), c))
-        r['flags'][ex] = held
-        pod_round[idx[out['status'][idx] == wire.PLACED]] = k
-    return _mapped(out, ids), pod_round, (counts if explain else None), touched
-
-
-class OracleForecastSolver(OracleExpandSolver):
-    """The oracle stand-in with rounds: per scenario the five steps on the grown records and a loop of oracle solves
-    per round, indices mapped back.  TEST INFRASTRUCTURE."""
-
-    def plan_scenarios(self, scenarios, source='mirror', explain=False):
-        if not any(_sc(sc)[6] is not None for sc in scenarios):
-            return super().plan_scenarios(scenarios, source, explain)
-        recs = self._snap if source == 'snapshot' else self._recs
-        out, base = [], 0
-        for sc in scenarios:
-            ex, pods, now, lift, edits, adds, rounds = _sc(sc)
-            b, rnd, counts, _ = oracle_rounds(recs, self._speed, np.asarray(pods), np.asarray(now, dtype='<f8'),
-                                              [int(i) for i in ex], lift, edits, adds, rounds, base, self._min_busy,
-                                              explain=explain)
-            out.append((0, -1, b) + ((counts,) if explain else ()) + (rnd,))
-            base += 0 if adds is None else len(adds[0])
-        return out
 
 
 # ---------------------------------------------------------------------------------------------- scenario families
@@ -156,11 +86,11 @@ def check_against_oracle(got, scens, st, speed, busy, where='', explain=False):
     walk = 0.0
     base = 0
     for j, (sc, g) in enumerate(zip(scens, got)):
-        ex, p, c, lift, edits, adds, rounds = _sc(sc)
+        sc = Scenario(*sc)
+        p, adds = sc.pods, sc.adds
         assert g[0] == 0 and g[1] == -1 and len(g[2]) == len(p), (where, j, g[:2])
         if len(p):
-            b, rnd, rows, touched = oracle_rounds(st, speed, p, c, [int(i) for i in ex], lift, edits, adds, rounds,
-                                                  base, busy, explain=explain)
+            b, rnd, rows, touched = oracle_scenario(st, speed, sc, base, busy, explain=explain)
             assert g[2].tobytes() == b.tobytes(), (where, j, helpers.first_binding_diff(b, g[2]))
             assert (g[-1] == rnd).all(), (where, j, g[-1], rnd)
             if explain:
@@ -179,27 +109,27 @@ def _raw(s, scens, round_start=True, fill=None, pod_round=True):
     """``nhd_plan_scenarios_rounds`` itself (``round_start=False``: NULL): ``(rc, status, which, out, counts,
     pod_round)``."""
     n = len(scens)
-    parts = [_sc(sc) for sc in scens]
+    parts = [Scenario(*sc) for sc in scens]
     cat = lambda xs, dt: np.ascontiguousarray(np.concatenate(xs) if xs else np.zeros(0), dtype=dt)  # noqa: E731
     off = lambda ls: np.concatenate([[0], np.cumsum(ls)]).astype('<i4')                           # noqa: E731
-    ex = cat([np.asarray(p[0], dtype='<i4').reshape(-1) for p in parts], '<i4')
-    pods = cat([p[1] for p in parts], wire.POD_DTYPE)
-    now = cat([np.asarray(p[2], dtype='<f8') for p in parts], '<f8')
-    lift = np.asarray([len(p[1]) if p[3] is None else p[3] for p in parts], dtype='<i4')
-    edn = cat([np.asarray([] if p[4] is None else p[4][0], dtype='<i4') for p in parts], '<i4')
-    edr = cat([p[4][1] for p in parts if p[4] is not None], wire.NODE_DTYPE)
-    adat = cat([np.asarray([] if p[5] is None else p[5][0], dtype='<i4') for p in parts], '<i4')
-    adr = cat([p[5][1] for p in parts if p[5] is not None], wire.NODE_DTYPE)
-    clk = cat([np.asarray([] if p[6] is None else p[6], dtype='<f8') for p in parts], '<f8')
+    ex = cat([np.asarray(p.exclude, dtype='<i4').reshape(-1) for p in parts], '<i4')
+    pods = cat([p.pods for p in parts], wire.POD_DTYPE)
+    now = cat([np.asarray(p.now, dtype='<f8') for p in parts], '<f8')
+    lift = np.asarray([len(p.pods) if p.lift is None else p.lift for p in parts], dtype='<i4')
+    edn = cat([np.asarray([] if p.edits is None else p.edits[0], dtype='<i4') for p in parts], '<i4')
+    edr = cat([p.edits[1] for p in parts if p.edits is not None], wire.NODE_DTYPE)
+    adat = cat([np.asarray([] if p.adds is None else p.adds[0], dtype='<i4') for p in parts], '<i4')
+    adr = cat([p.adds[1] for p in parts if p.adds is not None], wire.NODE_DTYPE)
+    clk = cat([np.asarray([] if p.rounds is None else p.rounds, dtype='<f8') for p in parts], '<f8')
     out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
     status, which = np.zeros(n, dtype='<i4'), np.zeros(n, dtype='<i4')
     counts = None if fill is None else np.full((len(pods), wire.WHY_COUNT), fill, dtype='<u4')
     rnd = np.full(len(pods), -7, dtype='<i4') if pod_round else None
     ptr = lambda a: a.ctypes.data if a is not None and len(a) else None                           # noqa: E731
-    excl_start, pod_start = off([len(p[0]) for p in parts]), off([len(p[1]) for p in parts])
-    edit_start = off([0 if p[4] is None else len(p[4][0]) for p in parts])
-    astart = off([0 if p[5] is None else len(p[5][0]) for p in parts])
-    rstart = off([0 if p[6] is None else len(p[6]) for p in parts])
+    excl_start, pod_start = off([len(p.exclude) for p in parts]), off([len(p.pods) for p in parts])
+    edit_start = off([0 if p.edits is None else len(p.edits[0]) for p in parts])
+    astart = off([0 if p.adds is None else len(p.adds[0]) for p in parts])
+    rstart = off([0 if p.rounds is None else len(p.rounds) for p in parts])
     rc = s._L.nhd_plan_scenarios_rounds(s._h, 0, n, excl_start.ctypes.data, ptr(ex), lift.ctypes.data,
                                         edit_start.ctypes.data, ptr(edn), ptr(edr), astart.ctypes.data, ptr(adat),
                                         ptr(adr), pod_start.ctypes.data, ptr(pods), ptr(now),
@@ -308,7 +238,7 @@ def test_forecast_pending_equals_the_reference_over_later_scans():
     stepped by 30, 31 and 10 s and from a fractional start clock, with and without candidate nodes added, and its drop
     decisions at the last scan for the pods no scan placed, answered by ``ForecastPending`` with the oracle standing in
     for the GPU."""
-    _forecast_against_the_reference(OracleForecastSolver)
+    _forecast_against_the_reference(OraclePlanner)
 
 
 def test_forecast_golden_places_later_and_leaves_pods_unplaced():
@@ -322,7 +252,7 @@ def test_forecast_pending_checks_its_arguments():
     from tests.golden.make_forecast_golden import forecast_sessions
     from tests.golden.make_plan_golden import mirror_session
     name, script = forecast_sessions()[-1]
-    sched, _, _ = mirror_session(script, OracleForecastSolver)
+    sched, _, _ = mirror_session(script, OraclePlanner)
     try:
         with pytest.raises(ValueError):
             sched.ForecastPending(0)
@@ -413,8 +343,9 @@ def scratch_rounds(scratch, st, scens, which=None):
     the rounds; node indices mapped back.  ``{j: (bindings, pod_round)}``."""
     out, base = {}, 0
     for j, sc in enumerate(scens):
-        ex, p, c, lift, edits, adds, rounds = _sc(sc)
-        g, ids = grown(st, edits, adds, base)
+        sc = Scenario(*sc)
+        ex, p, c, lift, adds, rounds = sc.exclude, sc.pods, sc.now, sc.lift, sc.adds, sc.rounds
+        g, ids = grown(st, sc.edits, adds, base)
         base += 0 if adds is None else len(adds[0])
         if which is not None and j not in which:
             continue
@@ -449,7 +380,7 @@ def scratch_rounds(scratch, st, scens, which=None):
             if len(ex) and lift == n:
                 flag(False)
             rnd[idx[b['status'][idx] == wire.PLACED]] = k
-        out[j] = (_mapped(b, ids), rnd)
+        out[j] = (mapped(b, ids), rnd)
     return out
 
 
@@ -587,9 +518,8 @@ def test_config4_full_size():
         scratch.close()
     base = 0
     for sc, g in zip(scens, got):
-        ex, p, c, lift, edits, adds, rounds = _sc(sc)
-        b, rnd, _, _ = oracle_rounds(after, speed, p, c, ex, lift, edits, adds, rounds, base, 30.0,
-                                     threads=os.cpu_count() or 1)
+        adds = Scenario(*sc).adds
+        b, rnd, _, _ = oracle_scenario(after, speed, sc, base, threads=os.cpu_count() or 1)
         assert g[0] == 0 and g[2].tobytes() == b.tobytes() and (g[-1] == rnd).all(), helpers.first_binding_diff(b, g[2])
         base += len(adds[0])
 

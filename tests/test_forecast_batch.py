@@ -6,7 +6,7 @@ records the previous round left": byte for byte each pod's last attempt, the rou
 the pods whose last attempt found no node.  That is what ``nhd_plan_scenarios_rounds`` gives the same pods as one
 scenario, so the chain of evidence is the one of tests/test_forecast.py with one more link:
   * on the CPU emulation of the device (tests/emu), both lane orders, the call equals the oracle loop
-    (``oracle_rounds``) and the scenario call on every family, refuses every malformed argument and moves nothing of
+    (``plan_oracle.oracle_scenario``) and the scenario call on every family, refuses every malformed argument and moves nothing of
     the handle (no GPU);
   * ``ForecastPending`` through a solver with ``plan_batch_rounds`` equals the reference's own later scans frozen in
     tests/golden/live/forecast.json.gz and the route through the scenario call; ``ForecastDrain`` equals the oracle loop
@@ -21,9 +21,10 @@ import numpy as np
 import pytest
 
 from nhd_b200 import _lib, wire
+from nhd_b200.solver import Scenario
 from tests import helpers
-from tests.test_forecast import (OracleForecastSolver, _forecast_against_the_reference, _steps, oracle_rounds,
-                                 scratch_rounds, walker)
+from tests.plan_oracle import OraclePlanner, oracle_scenario
+from tests.test_forecast import _forecast_against_the_reference, _steps, scratch_rounds, walker
 from tests.test_plan import _emu_lib, _gpu_factory, exclusion_sets
 from tests.test_query import MODES, _filter_words, _gpu_cases, oracle_state, packed
 
@@ -63,7 +64,7 @@ def check_batch_cases(s, cases, st, speed, busy, source='mirror', where=''):
     n = later = gone = 0
     for j, (ex, p, c, rounds) in enumerate(cases):
         out, rnd, rows = s.plan_batch_rounds(p, c, rounds, source=source, exclude=ex, explain=True)
-        b, wrnd, wrows, _ = oracle_rounds(st, speed, p, c, [int(i) for i in ex], rounds=rounds, busy=busy, explain=True)
+        b, wrnd, wrows, _ = oracle_scenario(st, speed, Scenario(ex, p, c, rounds=rounds), busy=busy, explain=True)
         assert out.tobytes() == b.tobytes(), (where, j, helpers.first_binding_diff(b, out))
         assert (rnd == wrnd).all(), (where, j, rnd, wrnd)
         assert (rows == wrows).all(), (where, j, np.flatnonzero((rows != wrows).any(1)))
@@ -280,7 +281,7 @@ def _routes_agree(factory, limit=None):
     golden = make_live_golden.load('plan')['sessions']
     for (name, script, _), want in list(zip(drain_sessions(), golden))[:limit]:
         got = []
-        for f in (factory, OracleForecastSolver):
+        for f in (factory, OraclePlanner):
             sched, k8s, _ = mirror_session(script, f)
             try:
                 state, traffic = dict(sched.pod_state), k8s.transcript()
@@ -331,7 +332,7 @@ def test_forecast_drain_with_the_oracle_stand_in_takes_the_scenario_call():
     from tests.golden import make_live_golden
     from tests.golden.make_plan_golden import drain_sessions, mirror_session
     (name, script, _), want = drain_sessions()[0], make_live_golden.load('plan')['sessions'][0]
-    sched, _, _ = mirror_session(script, OracleForecastSolver)
+    sched, _, _ = mirror_session(script, OraclePlanner)
     try:
         placement, why = sched.PlanDrain(want['drain'])
         assert sched.ForecastDrain(want['drain'], 1, reasons=True) == \
@@ -460,8 +461,8 @@ def test_config4_full_size():
         out, rnd, rows = s.plan_batch_rounds(tail[sample], clock[sample], rounds, explain=True)
     finally:
         s.close()
-    b, wrnd, wrows, _ = oracle_rounds(after, speed, tail[sample], clock[sample], rounds=rounds, busy=30.0,
-                                      threads=os.cpu_count() or 1, explain=True)
+    b, wrnd, wrows, _ = oracle_scenario(after, speed, Scenario((), tail[sample], clock[sample], rounds=rounds),
+                                        threads=os.cpu_count() or 1, explain=True)
     assert out.tobytes() == b.tobytes() and (rnd == wrnd).all() and (rows == wrows).all(), \
         helpers.first_binding_diff(b, out)
 

@@ -22,8 +22,9 @@ import pytest
 
 from nhd_b200 import _lib, wire
 from tests import helpers
-from tests.test_forecast import OracleForecastSolver, _steps
-from tests.test_plan import _emu_lib, excluded
+from tests.plan_oracle import OraclePlanner, _nic_bits, oracle_releases
+from tests.test_forecast import _steps
+from tests.test_plan import _emu_lib
 from tests.test_query import MODES, _filter_words, _gpu_cases, emu_cases, packed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -37,74 +38,6 @@ def test_the_symbol_is_declared_and_exported():
     assert 'int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_t n_excluded' in text
     assert 'typedef struct nhd_release {' in text and wire.RELEASE_DTYPE.itemsize == 88
     assert 'nhd_plan_batch_releases' in _lib.EXPORTS and hasattr(_lib.load(), 'nhd_plan_batch_releases')
-
-
-# ---------------------------------------------------------------------------------------------- the oracle loop
-def _nic_bits(count, n_nics):
-    return int(sum(1 << i for i in range(n_nics) if count[i] > 0))
-
-
-def oracle_releases(recs, speed, pods, now, rounds, tracked, pods_used, releases, exclude=(), busy=30.0, explain=False,
-                    solve_one=None):
-    """``(bindings, pod_round, counts or None, cuts)``: every pod solved alone on the records the pods before it left,
-    the counters of the tracked nodes raised by each placement's claimed NICs and lowered by each release's pairings,
-    each tracked NIC's bit = counter > 0.  ``cuts[r]``: the placements of round r that claimed a NIC whose counter was
-    <= -1 (where the batch path cuts).  ``solve_one(records, pod, clock)`` -> ``(binding, records)``; the C oracle by
-    default."""
-    from oracle import binding
-    from tests import explain_oracle
-    if solve_one is None:
-        def solve_one(r, pod, clock):
-            b, r = binding.solve(r, speed, pod[None], np.array([clock]), min_busy_secs=busy)
-            return b[0], r
-    r = excluded(recs, exclude)
-    count = {int(n): np.asarray(pods_used[t], dtype=np.int64).copy() for t, n in enumerate(tracked)}
-    n = len(pods)
-    out = np.zeros(n, dtype=wire.BINDING_DTYPE)
-    counts = np.zeros((n, wire.WHY_COUNT), dtype='<u4')
-    cuts = [0] * (len(rounds) + 1)
-
-    def attempt(k, idx, clocks, last):
-        nonlocal r
-        for i, c in zip(idx, clocks):
-            if explain and last:
-                _, why = explain_oracle.batch(r, speed, pods[[i]], np.array([c]), min_busy_secs=busy)
-                counts[i] = explain_oracle.counts(why, 1)[0]
-            b, r = solve_one(r, pods[i], c)
-            out[i] = b
-            node = int(b['node'])
-            if b['status'] == wire.PLACED and node in count:
-                for j in range(int(b['n_claimed'])):
-                    nic = int(b['claimed_nics'][j])
-                    cuts[k] += int(count[node][nic] <= -1)
-                    count[node][nic] += 1
-                r = r.copy()
-                r['nic_inuse'][node] = _nic_bits(count[node], int(r['n_nics'][node]))
-
-    def release(rl):
-        nonlocal r
-        r = r.copy()
-        node = int(rl['node'])
-        r['used'][node] &= ~rl['cores']
-        r['gpu_used'][node] &= ~rl['gpus']
-        if rl['hugepages_gb'] > 0:
-            r['free_hugepages_gb'][node] += rl['hugepages_gb']
-        count[node] -= rl['nic_pairings'].astype(np.int64)
-        r['nic_inuse'][node] = _nic_bits(count[node], int(r['n_nics'][node]))
-        r['busy_time'][node] = rl['clock']
-
-    attempt(0, range(n), now, not len(rounds))
-    pod_round = np.where(out['status'] == wire.PLACED, 0, len(rounds)).astype('<i4')
-    for k, c in enumerate(rounds, 1):
-        idx = np.flatnonzero(out['status'] != wire.PLACED)
-        if not len(idx):
-            break
-        for rl in releases[releases['round'] == k]:
-            release(rl)
-        attempt(k, idx, np.full(len(idx), c), k == len(rounds))
-        pod_round[idx[out['status'][idx] == wire.PLACED]] = k
-    counts[out['status'] != wire.NO_CANDIDATE] = 0
-    return out, pod_round, (counts if explain else None), cuts
 
 
 # ---------------------------------------------------------------------------------------------- the cases
@@ -456,20 +389,6 @@ def test_config4_full_size():
 
 
 # ---------------------------------------------------------------------------------------------- the scheduler
-class OracleReleaseSolver(OracleForecastSolver):
-    """The oracle stand-in with releases: ``oracle_releases`` on the records.  TEST INFRASTRUCTURE."""
-
-    def plan_batch_releases(self, pods, now, round_clocks, tracked, pods_used, releases, source='mirror', exclude=(),
-                            explain=False):
-        recs = self._snap if source == 'snapshot' else self._recs
-        b, rnd, counts, _ = oracle_releases(recs, self._speed, np.asarray(pods), np.asarray(now, dtype='<f8'),
-                                            [float(c) for c in round_clocks], list(tracked),
-                                            np.asarray(pods_used).reshape(len(tracked), wire.MAX_NICS),
-                                            np.asarray(releases, dtype=wire.RELEASE_DTYPE), [int(i) for i in exclude],
-                                            self._min_busy, explain)
-        return (b, rnd, counts) if explain else (b, rnd)
-
-
 def _releases_against_the_reference(factory, limit=None):
     """``ForecastPending(departures=...)`` equals the reference's scans with the deletes played between them, frozen in
     tests/golden/live/releases.json.gz: the scan and node of every pending pod, and the reasons at the last scan of
@@ -509,14 +428,14 @@ def _releases_against_the_reference(factory, limit=None):
 def test_forecast_pending_with_departures_equals_the_reference():
     """Deletes mid-gap, exactly at a scan's clock and inside the busy window before a scan, periods of 30 and 10 s;
     pods placed only after a release, held a scan by its busy stamp, and pods sharing a NIC a release drove negative."""
-    _releases_against_the_reference(OracleReleaseSolver)
+    _releases_against_the_reference(OraclePlanner)
 
 
 def test_forecast_pending_checks_its_departures():
     from tests.golden.make_plan_golden import mirror_session
     from tests.golden.make_release_golden import release_sessions
     name, script = release_sessions()[-1]
-    sched, _, _ = mirror_session(script, OracleReleaseSolver)
+    sched, _, _ = mirror_session(script, OraclePlanner)
     try:
         pending = list(sched.ForecastPending(3))
         deployed = [(ns, pod) for n in sched.nodes.values() for (pod, ns) in n.pod_info]

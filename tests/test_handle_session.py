@@ -7,10 +7,9 @@ bookkeeping, the generations behind the explanation and snapshot rules, workspac
 pinned here: a seeded session generator and a runner that drives one ``Solver`` through the session and, after every
 call, compares it
 
-  * with the oracle (``oracle.binding.solve``, ``test_query.oracle_alone``, ``test_plan.oracle_plan``,
-    ``test_defrag.oracle_defrag``, ``tests/explain_oracle.py``; for the forecasts ``test_plan_reasons.oracle_explained``,
-    ``test_expand.oracle_grown``, ``test_forecast.oracle_rounds``, ``test_forecast_releases.oracle_releases``), byte
-    for byte;
+  * with the oracle (``oracle.binding.solve``, ``tests/explain_oracle.py`` and the what-if oracles of
+    ``tests/plan_oracle.py``: ``oracle_alone``, ``oracle_scenario`` for plans and every scenario call,
+    ``oracle_releases``), byte for byte;
   * with a fresh handle in the same sweep mode, loaded with the records the call reads (a snapshot source is asked of
     the fresh handle as its mirror), refusals included: the same code, naming the same pod;
   * with the runner's own model of the records, the snapshot, the deployed pods and the legality rules (DESIGN §8.6 -
@@ -25,7 +24,9 @@ import numpy as np
 import pytest
 
 from nhd_b200 import packing, wire
+from nhd_b200.solver import Scenario
 from tests import scenarios
+from tests.plan_oracle import excluded, oracle_alone, oracle_releases, oracle_scenario
 
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
 MODES = (dict(), dict(single_warp=True), dict(cpu_warps=1), dict(cpu_warps=2), dict(sweep_debug=1),
@@ -79,17 +80,17 @@ def pod_refusal(pods, now, k):
 def scenario_call_refusal(scs, src_ref, n_classes):
     """(code, pod, rule) refusing a whole scenario call, in the order nhd_api.cu's plan_scenarios checks: every
     scenario's first round clock against its pods' clocks (before the source is read), the source, then the added
-    records (a NIC speed class the handle lacks).  ``scs``: 7-tuples."""
-    for ex, pods, now, lift, edits, adds, rounds in scs:
-        if rounds is not None and len(rounds):
-            late = np.flatnonzero(np.asarray(now) > rounds[0])
+    records (a NIC speed class the handle lacks).  ``scs``: ``Scenario`` records."""
+    for sc in scs:
+        if sc.rounds is not None and len(sc.rounds):
+            late = np.flatnonzero(np.asarray(sc.now) > sc.rounds[0])
             if len(late):
                 return wire.ERR_INVALID, int(late[0]), 'round clock'
     if src_ref is not None:
         return src_ref + ('source',)
     for sc in scs:
-        if sc[5] is not None:
-            for r in np.asarray(sc[5][1], dtype=wire.NODE_DTYPE):
+        if sc.adds is not None:
+            for r in np.asarray(sc.adds[1], dtype=wire.NODE_DTYPE):
                 spd = int(r['nic_speed'][0]) | int(r['nic_speed'][1]) << 64
                 if any((spd >> (4 * i)) & 0xF >= n_classes for i in range(int(r['n_nics']))):
                     return wire.ERR_INVALID, None, 'speed class'
@@ -595,7 +596,6 @@ class Runner:
             self.expl = (pods.copy(), now.copy(), start, got.copy())
 
     def query_batch(self, pods, now, source):
-        from tests.test_query import oracle_alone
         recs, want_ref = self.source(source)
         want_ref = want_ref or pod_refusal(pods, now, max_numa(self.recs))
         got, ref = self.call(lambda: self.s.query_batch(pods, now, source=source))
@@ -615,7 +615,6 @@ class Runner:
                 self.same(f'query_batch ({source}) against a fresh handle', got, fgot)
 
     def plan_batch(self, pods, now, source, exclude, explain):
-        from tests.test_plan import oracle_plan
         recs, want_ref = self.source(source)
         ex = [int(i) for i in exclude]
         want_ref = want_ref or pod_refusal(pods, now, max_numa(self.recs, ex))
@@ -632,7 +631,7 @@ class Runner:
             self.expect('plan_batch on a fresh handle', fref, want_ref)
         if want_ref is not None:
             return
-        want, counts = oracle_plan(recs, self.speed, pods, now, ex, BUSY)
+        want, _, counts, _ = oracle_scenario(recs, self.speed, (ex, pods, now), busy=BUSY, explain=True)
         b = got[0] if explain else got
         self.same(f'plan_batch ({source}) against the oracle', b, want)
         if explain and got[1].tobytes() != counts.tobytes():
@@ -641,14 +640,9 @@ class Runner:
             self.same(f'plan_batch ({source}) against a fresh handle', b, fgot[0] if explain else fgot)
 
     def plan_scenarios(self, scenarios, source, explain=False, what='plan_scenarios'):
-        """Any scenario call: plain, edited, explained, grown (sixth element) and with rounds (seventh), each scenario
-        against the oracle of its entry point, added nodes numbered call-wide."""
-        from tests.test_defrag import oracle_defrag
-        from tests.test_expand import oracle_grown
-        from tests.test_forecast import _sc, oracle_rounds
-        from tests.test_plan import oracle_plan
-        from tests.test_plan_reasons import oracle_explained
-        scs = [_sc(sc) for sc in scenarios]
+        """Any scenario call: plain, edited, explained, grown and with rounds, each scenario against the oracle,
+        added nodes numbered call-wide."""
+        scs = [Scenario(*sc) for sc in scenarios]
         recs, want_ref = self.source(source)
         want_ref = scenario_call_refusal(scs, want_ref, self.n_classes())
         got, ref = self.call(lambda: self.s.plan_scenarios(scenarios, source=source, explain=explain))
@@ -665,37 +659,25 @@ class Runner:
             self.expect(f'{what} on a fresh handle', fref, want_ref)
         if want_ref is not None:
             return
-        rounds = any(sc[6] is not None for sc in scs)
-        grown_call = any(sc[5] is not None for sc in scs)
+        rounds = any(sc.rounds is not None for sc in scs)
         k = max_numa(self.recs)
         for sc in scs:
-            for change in (sc[4], sc[5]):                                  # edits and additions count, held or not
+            for change in (sc.edits, sc.adds):                             # edits and additions count, held or not
                 if change is not None and len(change[1]):
                     k = max(k, int(np.asarray(change[1])['n_numa'].max()))
         base, st = 0, self.stats
-        for j, (ex, pods, now, lift, edits, adds, clocks) in enumerate(scs):
+        for j, sc in enumerate(scs):
             res, where = got[j], f'{what} ({source}) scenario {j}'
-            n_add = 0 if adds is None else len(adds[0])
-            want_ref = pod_refusal(pods, now, k)
+            n_add = 0 if sc.adds is None else len(sc.adds[0])
+            want_ref = pod_refusal(sc.pods, sc.now, k)
             self.expect(where, None if res[0] == 0 else tuple(res[:2]), want_ref)
             if fgot is not None and _result_bytes(fgot[j]) != _result_bytes(res):
                 raise Mismatch(f'{where}: differs from a fresh handle')
-            if want_ref is not None or not len(pods):
+            if want_ref is not None or not len(sc.pods):
                 base += n_add
                 continue
-            b, exl, wrows, wrnd = res[2], [int(i) for i in ex], None, None
-            if rounds:
-                want, wrnd, wrows, _ = oracle_rounds(recs, self.speed, pods, now, exl, lift, edits, adds, clocks, base,
-                                                     BUSY, explain=explain)
-            elif grown_call:
-                want = oracle_grown(recs, self.speed, pods, now, exl, lift, edits, adds, base, BUSY, explain=explain)
-                want, wrows = want if explain else (want, None)
-            elif explain:
-                want, wrows = oracle_explained(recs, self.speed, pods, now, exl, lift, edits, BUSY)
-            elif lift is None and edits is None:
-                want = oracle_plan(recs, self.speed, pods, now, exl, BUSY)[0]
-            else:
-                want = oracle_defrag(recs, self.speed, pods, now, exl, lift, edits, busy=BUSY)
+            b = res[2]
+            want, wrnd, wrows, _ = oracle_scenario(recs, self.speed, sc, base, BUSY, explain=True)
             self.same(f'{where} against the oracle', b, want, len(recs) + base + n_add)
             if explain:
                 self.same_rows(where, res[3], wrows, b, len(recs) + n_add)
@@ -761,7 +743,6 @@ class Runner:
         tracked = sorted({int(x['node']) for x in rels})
         # free-NIC nodes the pods take when nothing ends (where a negative counter cuts), else any with NICs
         from oracle import binding
-        from tests.test_plan import excluded
         ok = np.isfinite(now)
         first = binding.solve(excluded(recs, [int(i) for i in exclude]), self.speed, pods[ok], now[ok],
                               min_busy_secs=BUSY)[0]
@@ -791,8 +772,6 @@ class Runner:
         """plan_batch_rounds (``rel`` None) or plan_batch_releases (``rel``: tracked, pods_used, releases) against the
         refusal model, a fresh handle and the oracle loop; a rounds forecast also against the scenario call of that
         one scenario on this handle."""
-        from tests.test_forecast import oracle_rounds
-        from tests.test_forecast_releases import oracle_releases
         recs, src_ref = self.source(source)
         ex = [int(i) for i in exclude]
         want_ref = batch_refusal(pods, now, rounds, rel, src_ref, recs, max_numa(self.recs, ex))
@@ -817,8 +796,8 @@ class Runner:
         if want_ref is not None:
             return
         if rel is None:
-            want, wrnd, wrows, _ = oracle_rounds(recs, self.speed, pods, now, ex, rounds=rounds, busy=BUSY,
-                                                 explain=explain)
+            want, wrnd, wrows, _ = oracle_scenario(recs, self.speed, Scenario(ex, pods, now, rounds=rounds), busy=BUSY,
+                                                   explain=explain)
         else:
             want, wrnd, wrows, cuts = oracle_releases(recs, self.speed, pods, now, rounds, *rel, exclude=ex, busy=BUSY,
                                                       explain=explain)

@@ -5,8 +5,7 @@ These calls keep the most per-handle state of all (DESIGN §8.11 - §8.15): the 
 arrays ``plan_batch`` swaps with the round buffer every round, the release area whose offsets move with the node count,
 the index buffer shared by the tracked nodes and the exclusions, the scenario scratch in two layouts, the reason
 buffers shared with the batch explanations.  The runner of tests/test_handle_session.py compares every call with the
-oracle of its entry point (``test_plan_reasons.oracle_explained``, ``test_expand.oracle_grown``,
-``test_forecast.oracle_rounds``, ``test_forecast_releases.oracle_releases``), with a fresh handle and with its refusal
+oracle (``oracle_scenario`` and ``oracle_releases`` of tests/plan_oracle.py), with a fresh handle and with its refusal
 model; the releases are pods the session itself deployed.  The named sessions each aim at one way the carried state
 could go wrong; the random ones assert that they reached what they are meant to test."""
 import numpy as np

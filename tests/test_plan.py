@@ -19,51 +19,20 @@ import numpy as np
 import pytest
 
 from nhd_b200 import wire
-from tests import explain_oracle, helpers, scenarios
+from tests import helpers, scenarios
 from tests.golden import make_live_golden
 from tests.golden.make_plan_golden import drain_sessions, mirror_session
-from tests.test_query import MODES, OracleQuerySolver, _filter_words, _gpu_cases, emu_cases, oracle_state, packed
+from tests.plan_oracle import OraclePlanner, excluded, oracle_scenario
+from tests.test_query import MODES, _filter_words, _gpu_cases, emu_cases, oracle_state, packed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
-
-
-def excluded(recs, exclude):
-    """A copy of ``recs`` with the nodes ``exclude`` in maintenance (the reference's NODE_MAINT_START)."""
-    out = np.ascontiguousarray(recs, dtype=wire.NODE_DTYPE).copy()
-    idx = np.asarray(list(exclude), dtype=np.int64)
-    out['flags'][idx] |= wire.NODE_MAINTENANCE
-    return out
-
-
-def oracle_plan(recs, speed, pods, now, exclude=(), busy=30.0, threads=1):
-    """The oracle's bindings and explanation counts of the batch on ``recs`` with ``exclude`` in maintenance."""
-    out, reasons = explain_oracle.batch(excluded(recs, exclude), speed, pods, now, min_busy_secs=busy, threads=threads)
-    return out, explain_oracle.counts(reasons, len(pods))
 
 
 def exclusion_sets(recs):
     """No exclusion, every third node, and every node with GPUs."""
     n = len(recs)
     return [(), tuple(range(0, n, 3)), tuple(int(i) for i in np.flatnonzero(recs['n_gpus'] > 0))]
-
-
-class OraclePlanSolver(OracleQuerySolver):
-    """The oracle stand-in with plans: the oracle's solve and explanation on a copy of the records with the excluded
-    nodes in maintenance.  TEST INFRASTRUCTURE."""
-
-    def solve_batch(self, pods, now):
-        self._last = (np.asarray(pods).copy(), np.asarray(now, dtype='<f8').copy())
-        return super().solve_batch(pods, now)
-
-    def explain_batch(self):
-        return oracle_plan(self._snap, self._speed, *self._last, busy=self._min_busy)[1]
-
-    def plan_batch(self, pods, now, source='mirror', exclude=(), explain=False):
-        recs = self._snap if source == 'snapshot' else self._recs
-        out, counts = oracle_plan(recs, self._speed, np.asarray(pods), np.asarray(now, dtype='<f8'),
-                                  [int(i) for i in exclude], self._min_busy)
-        return (out, counts) if explain else out
 
 
 # ---------------------------------------------------------------------------------------------- CPU: the reference
@@ -101,11 +70,11 @@ def _drain_against_the_reference(factory):
 def test_plan_drain_equals_the_reference_drain():
     """Where the reference re-schedules the pods of drained nodes, answered before the drain by ``PlanDrain`` with
     the oracle standing in for the GPU."""
-    _drain_against_the_reference(OraclePlanSolver)
+    _drain_against_the_reference(OraclePlanner)
 
 
 def test_plan_pods_equals_the_batch_with_the_oracle_stand_in():
-    _plan_pods_equals_the_batch(OraclePlanSolver, _plain_scripts()[:3])
+    _plan_pods_equals_the_batch(OraclePlanner, _plain_scripts()[:3])
 
 
 # ---------------------------------------------------------------------------------------------- CPU: emulated device
@@ -115,7 +84,8 @@ sys.path.insert(0, %(root)r)
 import numpy as np
 from nhd_b200.solver import Solver
 from tests import helpers
-from tests.test_plan import exclusion_sets, oracle_plan
+from tests.plan_oracle import oracle_scenario
+from tests.test_plan import exclusion_sets
 from tests.test_query import emu_cases, oracle_state, packed
 n = 0
 for j, scn in enumerate(emu_cases()):
@@ -134,7 +104,7 @@ for j, scn in enumerate(emu_cases()):
         clock = now[k:] if j %% 3 else np.full(len(now) - k, now[k])
         for ex in exclusion_sets(recs):
             got, counts = s.plan_batch(pods[k:], clock, source=source, exclude=ex, explain=True)
-            want, wcounts = oracle_plan(st, speed, pods[k:], clock, ex, busy)
+            want, _, wcounts, _ = oracle_scenario(st, speed, (ex, pods[k:], clock), busy=busy, explain=True)
             assert got.tobytes() == want.tobytes(), (j, ex, helpers.first_binding_diff(want, got))
             assert counts.tobytes() == wcounts.tobytes(), (j, ex)
             n += len(got)
@@ -247,7 +217,7 @@ def test_plan_equals_the_oracle_in_every_sweep_mode():
                 for ex in sets:
                     for clock in (now[k:], np.full(len(pods) - k, now[k])):
                         got, counts = s.plan_batch(pods[k:], clock, exclude=ex, explain=True)
-                        want, wcounts = oracle_plan(st, speed, pods[k:], clock, ex, busy)
+                        want, _, wcounts, _ = oracle_scenario(st, speed, (ex, pods[k:], clock), busy=busy, explain=True)
                         assert got.tobytes() == want.tobytes(), (j, mode, ex, helpers.first_binding_diff(want, got))
                         assert counts.tobytes() == wcounts.tobytes(), (j, mode, ex)
                         statuses += np.bincount(got['status'], minlength=5)[:5]
@@ -452,7 +422,7 @@ def test_config4_full_size():
         head = s.plan_batch(pods[:256], now[:256], exclude=ex)
     finally:
         s.close()
-    want, _ = oracle_plan(recs, speed, pods[:256], now[:256], ex, threads=os.cpu_count() or 1)
+    want = oracle_scenario(recs, speed, (ex, pods[:256], now[:256]), threads=os.cpu_count() or 1, explain=True)[0]
     assert head.tobytes() == want.tobytes(), helpers.first_binding_diff(want, head)
     assert head.tobytes() == got[:256].tobytes()
 

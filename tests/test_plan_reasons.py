@@ -18,55 +18,19 @@ import numpy as np
 import pytest
 
 from nhd_b200 import wire
-from tests import explain_oracle, helpers
+from nhd_b200.solver import Scenario
+from tests import helpers
 from tests.golden import make_live_golden
 from tests.golden.make_defrag_golden import defrag_sessions
 from tests.golden.make_plan_golden import drain_sessions, mirror_session
-from tests.test_defrag import OracleDefragSolver, _sc, defrag_scenarios
+from tests.plan_oracle import OraclePlanner, excluded, oracle_scenario
+from tests.test_defrag import defrag_scenarios
 from tests.test_drains import _each_plan, drain_scenarios
-from tests.test_plan import _emu_lib, _gpu_factory, excluded, oracle_plan
+from tests.test_plan import _emu_lib, _gpu_factory
 from tests.test_query import MODES, _filter_words, _gpu_cases, oracle_state, packed
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
-
-
-def oracle_explained(recs, speed, pods, now, exclude=(), lift=None, edits=None, busy=30.0, threads=1):
-    """The five steps with the C oracle on a copy of ``recs`` and the explanation of every NO_CANDIDATE pod on the
-    records at the start of its phase with the phase's earlier pods solved: ``(bindings, counts)``."""
-    from oracle import binding
-    r = np.ascontiguousarray(recs, dtype=wire.NODE_DTYPE).copy()
-    if edits is not None and len(edits[0]):
-        r[np.asarray(edits[0], dtype=np.int64)] = edits[1]
-    ex = np.unique(np.asarray(list(exclude), dtype=np.int64))
-    lift = len(pods) if lift is None else lift
-    flags = r['flags'][ex].copy()
-    r = excluded(r, ex)
-    out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
-    counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4')
-    kw = dict(min_busy_secs=busy, threads=threads)
-    if lift:
-        out[:lift], why = explain_oracle.batch(r, speed, pods[:lift], now[:lift], **kw)
-        counts[:lift] = explain_oracle.counts(why, lift)
-        r = binding.solve(r, speed, pods[:lift], now[:lift], **kw)[1]
-    r['flags'][ex] = flags
-    if lift < len(pods):
-        out[lift:], why = explain_oracle.batch(r, speed, pods[lift:], now[lift:], **kw)
-        counts[lift:] = explain_oracle.counts(why, len(pods) - lift)
-    return out, counts
-
-
-class OracleReasonSolver(OracleDefragSolver):
-    """The oracle stand-in with explained scenarios: the five steps and their explanations per scenario.  TEST
-    INFRASTRUCTURE."""
-
-    def plan_scenarios(self, scenarios, source='mirror', explain=False):
-        if not explain:
-            return super().plan_scenarios(scenarios, source=source)
-        recs = self._snap if source == 'snapshot' else self._recs
-        return [(0, -1) + oracle_explained(recs, self._speed, np.asarray(sc[1]), np.asarray(sc[2], dtype='<f8'),
-                                           [int(i) for i in sc[0]], *sc[3:5], busy=self._min_busy)
-                for sc in scenarios]
 
 
 def check_explained(got, plain, scens, refused, st, speed, busy, where=''):
@@ -74,13 +38,13 @@ def check_explained(got, plain, scens, refused, st, speed, busy, where=''):
     ones name the pod and have neither.  Returns the number of NO_CANDIDATE rows compared."""
     n = 0
     for j, (sc, g, p) in enumerate(zip(scens, got, plain)):
-        ex, pods, c, lift, edits = _sc(sc)
+        sc = Scenario(*sc)
         if j in refused:
             assert g == refused[j] + (None, None) and p[:2] == refused[j], (where, j, g[:2])
             continue
         assert g[:2] == (0, -1) and g[2].tobytes() == p[2].tobytes(), (where, j, g[:2])
-        if len(pods):
-            want, wc = oracle_explained(st, speed, pods, c, [int(i) for i in ex], lift, edits, busy)
+        if len(sc.pods):
+            want, _, wc, _ = oracle_scenario(st, speed, sc, busy=busy, explain=True)
             assert g[2].tobytes() == want.tobytes(), (where, j, helpers.first_binding_diff(want, g[2]))
             assert (g[3] == wc).all(), (where, j, np.flatnonzero((g[3] != wc).any(1)), g[3][(g[3] != wc).any(1)][:2],
                                         wc[(g[3] != wc).any(1)][:2])
@@ -159,7 +123,7 @@ def _counted(rows, names):
 def test_plan_drains_and_defrag_reasons_equal_the_reference():
     """The reference's own drop decisions for every re-created or pending pod it leaves without a node, answered
     before any drain by ``PlanDrains`` / ``PlanDefrag`` with ``reasons=True`` and the oracle standing in for the GPU."""
-    _reasons_against_the_reference(OracleReasonSolver)
+    _reasons_against_the_reference(OraclePlanner)
 
 
 def _drains_reasons_equal_plan_drain(factory, sessions):
@@ -182,7 +146,7 @@ def _drains_reasons_equal_plan_drain(factory, sessions):
 
 def test_plan_drains_reasons_equal_plan_drain_per_group():
     """``PlanDrains(groups, reasons=True)[g]`` is ``PlanDrain(g)`` from the same state, for single nodes and pairs."""
-    _drains_reasons_equal_plan_drain(OracleReasonSolver, drain_sessions()[:6])
+    _drains_reasons_equal_plan_drain(OraclePlanner, drain_sessions()[:6])
 
 
 # ---------------------------------------------------------------------------------------------- CPU: emulated device
@@ -312,7 +276,8 @@ def commit_path(scratch, base, scens):
     rest, ``explain_batch``.  ``[(bindings, counts)]``."""
     out = []
     for sc in scens:
-        ex, p, c, lift, edits = _sc(sc)
+        sc = Scenario(*sc)
+        ex, p, c, lift, edits = sc.exclude, sc.pods, sc.now, sc.lift, sc.edits
         scratch.load_nodes(base)
         if edits is not None and len(edits[0]):
             scratch.update_nodes(np.asarray(edits[0], dtype='<i4'), edits[1])
@@ -450,7 +415,7 @@ def test_config4_full_size():
     finally:
         s.close()
     for (ex, p, c), (code, _, b, counts) in zip(sample, got):
-        want, wc = oracle_plan(after, speed, p, c, ex, threads=os.cpu_count() or 1)
+        want, _, wc, _ = oracle_scenario(after, speed, (ex, p, c), threads=os.cpu_count() or 1, explain=True)
         assert code == 0 and b.tobytes() == want.tobytes() and (counts == wc).all(), ex
 
 

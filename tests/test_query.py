@@ -20,6 +20,7 @@ from oracle import binding
 from tests import helpers, ref_compare, scenarios
 from tests.golden import make_live_golden
 from tests.golden.make_query_golden import query_states, query_streams
+from tests.plan_oracle import OraclePlanner, oracle_alone
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 EMULATED = os.environ.get('NHD_B200_ALLOW_EMULATED') == '1'
@@ -32,25 +33,9 @@ def packed(scn):
     return scenarios.apply_preuse(recs, scn), pods, now, layout.speed_table(), float(scn.get('min_busy_secs', 30.0))
 
 
-def oracle_alone(recs, speed, pods, now, busy=30.0, threads=1):
-    """Pod i solved alone on a fresh copy of ``recs``, for every i."""
-    out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
-    for i in range(len(pods)):
-        out[i] = binding.solve(recs, speed, pods[i:i + 1], now[i:i + 1], min_busy_secs=busy, threads=threads)[0][0]
-    return out
-
-
 def oracle_state(recs, speed, pods, now, busy, k):
     """The records after pods 0..k-1 of the stream were scheduled one after the other."""
     return binding.solve(recs, speed, pods[:k], now[:k], min_busy_secs=busy)[1] if k else recs
-
-
-class OracleQuerySolver(helpers.OracleSolver):
-    """The oracle stand-in with queries: a batch of one per pod on a copy of the records.  TEST INFRASTRUCTURE."""
-
-    def query_batch(self, pods, now, source='mirror'):
-        recs = self._snap if source == 'snapshot' else self._recs
-        return oracle_alone(recs, self._speed, np.asarray(pods), np.asarray(now, dtype='<f8'), self._min_busy)
 
 
 # ---------------------------------------------------------------------------------------------- CPU: the oracle
@@ -76,7 +61,8 @@ sys.path.insert(0, %(root)r)
 import numpy as np
 from nhd_b200.solver import Solver
 from tests import helpers
-from tests.test_query import emu_cases, oracle_alone, oracle_state, packed
+from tests.plan_oracle import oracle_alone
+from tests.test_query import emu_cases, oracle_state, packed
 n = 0
 for scn in emu_cases():
     recs, pods, now, speed, busy = packed(scn)
@@ -122,7 +108,7 @@ def test_query_kernels_on_the_emulated_device_equal_the_oracle(lane_order):
 
 def test_scheduler_contention_with_the_oracle_stand_in(monkeypatch):
     """The scheduler side of ``diagnose_contention`` without a GPU: the oracle answers the queries."""
-    _contention_session(monkeypatch, OracleQuerySolver, [H_script(10, 'wild'), H_script(101, 'mixed')])
+    _contention_session(monkeypatch, OraclePlanner, [H_script(10, 'wild'), H_script(101, 'mixed')])
 
 
 # ---------------------------------------------------------------------------------------------- GPU
