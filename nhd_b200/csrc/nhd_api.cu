@@ -895,7 +895,7 @@ static int32_t launch_solve(nhd_handle* h, Workspace& w, const uint8_t* nodes, b
         uint4* const dyn = w.dyn;
         uint64_t* const bitmaps = w.bitmaps;
         unpack_slots_kernel<<<(unsigned)((n16 + 255) / 256), 256, 0, h->stream>>>(reinterpret_cast<const uint4*>(h->d_xchg.p), ws, S, h->n_super,
-                                                                              rows, W, dyn, bitmaps);
+                                                                              rows, W, h->n_nodes, h->d_class, dyn, bitmaps);
         CK(cudaGetLastError());
         launches += 2;
     }

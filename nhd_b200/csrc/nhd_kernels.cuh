@@ -594,8 +594,14 @@ filter_kernel(const FilterArgs a)
  * Node-sharded ranks: after the one collective of the batch (an all-gather of every rank's slot: the NodeDyn
  * summaries and the bitmap columns of its nodes) the slots are laid back out as the arrays the sweep reads.
  * Slot q covers super-tiles [q*S, (q+1)*S): S*256 summaries, then rows x S*4 bitmap words.
+ *
+ * A summary's hw_class is the owning rank's id: class ids are the slots the classes won in that rank's claim table,
+ * so they depend on the order its claims arrived in and on its earlier loads.  The sweep reads them against this
+ * rank's tables (ClsFast, the NIC cache, the memo keys), so every summary gets this rank's id of its node on the way
+ * in.  The bitmaps are plain facts about the nodes and are copied as they are.
  */
 __global__ void unpack_slots_kernel(const uint4* __restrict__ xchg, int ws, int S, int n_super, int rows, int W,
+                                    int n_nodes, const uint16_t* __restrict__ class_id,
                                     uint4* __restrict__ dyn, uint64_t* __restrict__ bitmaps)
 {
     const size_t slot16 = (size_t)S * 2 * (SUPER_NODES + rows);           /* 16-byte units per slot */
@@ -607,7 +613,13 @@ __global__ void unpack_slots_kernel(const uint4* __restrict__ xchg, int ws, int 
     if (lo >= hi) return;
     const size_t dyn16 = (size_t)S * SUPER_NODES * 2;
     if (r < dyn16) {
-        if (r < (size_t)(hi - lo) * SUPER_NODES * 2) dyn[(size_t)lo * SUPER_NODES * 2 + r] = xchg[i];
+        if (r < (size_t)(hi - lo) * SUPER_NODES * 2) {
+            const size_t e = (size_t)lo * SUPER_NODES * 2 + r;               /* node e / 2, half e % 2 */
+            uint4 v = xchg[i];
+            /* hw_class: bytes 20-21 of NodeDyn, the low half of the second chunk's .y (padding nodes stay zero) */
+            if ((e & 1) && e / 2 < (size_t)n_nodes) v.y = (v.y & 0xFFFF0000u) | class_id[e / 2];
+            dyn[e] = v;
+        }
     } else {
         const size_t b = r - dyn16;                                          /* 16 bytes = two words of one row */
         const int row = (int)(b / ((size_t)S * 2)), k2 = (int)(b % ((size_t)S * 2));

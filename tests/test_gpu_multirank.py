@@ -31,4 +31,5 @@ def test_sharded_ranks_equal_the_oracle(oracle_lib, world):
                           os.path.join(ROOT, 'tests', 'multirank_worker.py')],
                          cwd=ROOT, capture_output=True, text=True, timeout=1200)
     assert res.returncode == 0, (res.stdout + res.stderr)[-3000:]
-    assert res.stdout.count('equal to the oracle') == 3, res.stdout[-2000:]
+    # six two-batch legs (tests/multirank_worker.py) and three staged re-solves
+    assert res.stdout.count('equal to the oracle') == 9, res.stdout[-2000:]
