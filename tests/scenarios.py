@@ -549,6 +549,61 @@ def limit_scenarios():
     return _free_core_cases() + _nic_count_cases() + _signature_cases() + _class_cases() + nic_bandwidth_scenarios()
 
 
+# ----------------------------------------------------------------------------------
+# full-size streams (tests/test_gpu_full_size.py, tools/emu_full_size.py)
+# ----------------------------------------------------------------------------------
+def jumping_clocks(n, seed=31, t0=1000.0, step=0.001, p_forward=0.01, p_back=0.004):
+    """Per-pod clocks for a 30 s busy window that make nodes leave it inside one batch: steps of ``step`` seconds,
+    with some of +31 s (every stamp so far leaves the window) and some of -40 s (the busy set is rebuilt; the stamps
+    are then in the future and stay busy until the clock passes them by 30 s, while stamps made after the step expire
+    at the next +31 s).  Each clock is the previous one plus its step, in fp64."""
+    rng = np.random.default_rng(seed)
+    r = rng.random(n)
+    steps = np.where(r < p_back, -40.0, np.where(r < p_back + p_forward, 31.0, step))
+    steps[0] = 0.0
+    out = np.empty(n, dtype='<f8')
+    t = t0
+    for i in range(n):
+        t += steps[i]
+        out[i] = t
+    return out
+
+
+def steady_state_update(start, bindings, seed=60, n=1024, moved_every=4):
+    """The update a long-lived handle takes between two batches: ``n`` of the nodes the batch bound pods to get
+    their start records back (the pods finished), and every ``moved_every``-th of them another node's start record
+    instead (the node came back with other hardware, so its hardware class changes).  Returns (idx, new records)."""
+    rng = np.random.default_rng(seed)
+    bound = np.unique(bindings['node'][bindings['status'] == 0])
+    assert len(bound) >= n, len(bound)
+    idx = np.sort(rng.choice(bound, size=n, replace=False)).astype(np.int32)
+    src = idx.copy()
+    src[::moved_every] = rng.integers(0, len(start), size=len(src[::moved_every]))
+    return idx, start[src].copy()
+
+
+def nic_signatures(recs):
+    """The distinct per-NUMA NIC signatures of 2-NUMA records (a signature: the NIC count of one NUMA node and the
+    speed classes of its NICs in list order), as cls_fast_kernel numbers them."""
+    out = set()
+    for r in recs:
+        if int(r['n_numa']) != 2:
+            continue
+        spd = int(r['nic_speed'][0]) | int(r['nic_speed'][1]) << 64
+        for k in range(2):
+            m = int(r['nic_numa_mask'][k])
+            out.add(tuple((spd >> (4 * j)) & 0xF for j in range(32) if m >> j & 1))
+    return out
+
+
+def repeated_gpu_nodes(pods, bindings):
+    """Nodes that took two or more GPU pods of one batch: with a constant clock the busy window allows one."""
+    gpu = pods['groups']['n_gpus'].sum(axis=1) > 0
+    placed = bindings['node'][(bindings['status'] == 0) & gpu]
+    nodes, counts = np.unique(placed, return_counts=True)
+    return nodes[counts >= 2]
+
+
 def apply_preuse(recs, case):
     """The packed records of a limit case with its pre-used cores and NICs applied."""
     recs = recs.copy()
