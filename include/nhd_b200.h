@@ -538,6 +538,50 @@ int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_t n_exclude
                                 int32_t n_releases, const nhd_release* releases,
                                 nhd_binding* out, uint32_t* why_counts, int32_t* pod_round);
 
+/*
+ * nhd_plan_scenarios_rounds with running pods finishing between the scans, per scenario: "jobs A and B end in about 20
+ * minutes: does the queue clear then, or do I also need one more node like this one?", and several departure schedules
+ * side by side.  Every argument of nhd_plan_scenarios_rounds keeps its meaning; scenario s also has
+ *   - tracked nodes tracked[track_start[s] .. track_start[s+1]) with their signed NIC pod counters at plan start,
+ *     pods_used[t * NHD_MAX_NICS + i] for NIC i of tracked[t] (t call-wide), as for nhd_plan_batch_releases;
+ *   - releases releases[rel_start[s] .. rel_start[s+1]), round 1 .. R_s.
+ * Before round r >= 1, if a pod of s is still unplaced, s's releases with round == r are applied in array order to s's
+ * own records and counters: core and GPU bits cleared, hugepages_gb added when > 0, the counters lowered by
+ * nic_pairings, busy_time = clock.  On a tracked node a NIC's in-use bit is count > 0 after every release and after
+ * every placement, and each placement raises the count of every NIC in its claimed_nics by 1 when that pod commits.
+ * Scenarios commit one pod at a time, so unlike nhd_plan_batch_releases nothing is cut or solved again.
+ *   out, pod_round  as for nhd_plan_scenarios_rounds, on those records;
+ *   why_counts     (may be NULL) as for nhd_plan_scenarios_rounds: the row nhd_explain_batch would give at the start of
+ *                  the pod's last attempt.
+ * Identities: with track_start and rel_start both NULL (tracked, pods_used and releases are not read) the call is
+ * nhd_plan_scenarios_rounds.  One scenario with no edits, no additions and lift_at NULL gives the out and pod_round of
+ * nhd_plan_batch_releases with the same pods, round clocks, exclusions, tracked counters and releases, byte for byte;
+ * the only difference is the tuple-limit judgement, as between nhd_plan_scenarios and nhd_plan_batch.
+ * Releases on a node the scenario edits are out of scope: such a release refuses the call (an edited record replaces
+ * the node's whole state, so a caller releasing on it edits the record instead).
+ * Besides nhd_plan_scenarios_rounds' malformed arguments, the whole call is NHD_ERR_INVALID, before anything runs, for
+ * track or release offsets that do not start at 0 or go down; tracked or pods_used NULL with tracked nodes, releases
+ * NULL with releases; a tracked node outside [0, n_nodes) or tracked twice in one scenario; releases in a scenario
+ * without rounds, or a release round outside [1, R_s]; release clocks that go down inside a scenario, are not finite,
+ * lie before the clock of the round before theirs (for round 1: before a now[] of the scenario) or after their own
+ * round's clock; a release on a node its scenario does not track, or edits; and, checked on the device against the
+ * source records (one word read back), a tracked count whose sign disagrees with the NIC's in-use bit (> 0 exactly
+ * when set), a non-zero count on a NIC at or beyond n_nics, or a release's core, GPU or pairing bit beyond its node's
+ * logical cores, n_gpus or n_nics.  Tuple limits, refusals per scenario, side effects (none observable), collectives
+ * (none) and waiting as for nhd_plan_scenarios_rounds.  Each scenario's slot bound grows by its distinct released
+ * nodes, and the device holds its tracked nodes' counts: n_tracked_s * NHD_MAX_NICS int32.
+ */
+int32_t nhd_plan_scenarios_releases(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                    const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                    const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                                    const int32_t* add_start, const int32_t* add_at, const nhd_node_rec* add_rec,
+                                    const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                    const int32_t* round_start, const double* round_clock,
+                                    const int32_t* track_start, const int32_t* tracked, const int16_t* pods_used,
+                                    const int32_t* rel_start, const nhd_release* releases,
+                                    nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                    uint32_t* why_counts, int32_t* pod_round);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

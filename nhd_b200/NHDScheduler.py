@@ -87,7 +87,9 @@ class ClusterScenario(NamedTuple):
     objects for records and the pods as ``plan`` takes them (``now`` one clock or one per pod).  ``edits`` (None: none):
     ``{node name: Node-like object}``, packed as ``sync`` packs nodes.  ``adds`` (None: none): ``[(before, node)]``,
     each joining the node order right before the node named ``before`` (None: after the last node), packed by
-    ``pack_candidates`` before any pod (a pod may request a group name only a candidate carries)."""
+    ``pack_candidates`` before any pod (a pod may request a group name only a candidate carries).  ``releases`` (None:
+    none): ``[(node name, topology, clock)]`` of deployed pods that end between the scenario's ``rounds``, as
+    ``forecast(releases=...)`` takes them, on nodes the scenario does not edit."""
     exclude: Iterable[str]
     tops: Sequence
     pod_groups: Sequence[Iterable[str]]
@@ -97,6 +99,7 @@ class ClusterScenario(NamedTuple):
     edits: Optional[Dict[str, object]] = None
     adds: Optional[Sequence[tuple]] = None
     rounds: Optional[Sequence[float]] = None
+    releases: Optional[Sequence[tuple]] = None
 
 
 def _type_name(t) -> str:
@@ -344,7 +347,8 @@ class DeviceCluster:
     def plan_scenarios(self, scenarios: Sequence, source: str = 'mirror', explain: bool = False):
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
         of ``ClusterScenario`` records, or plain tuples of their fields in order.  When any scenario has ``rounds``,
-        each result gains the per-pod round that placed the pod (``Solver.plan_scenarios``).
+        each result gains the per-pod round that placed the pod (``Solver.plan_scenarios``).  A scenario's ``releases``
+        are packed as ``forecast`` packs them, with that scenario's clocks and rounds.
         Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
         when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods; ``explain=True``: one
         ``(code, pod, bindings, counts)``, ``counts`` the per-reason node counts of the NO_CANDIDATE pods.  A pod
@@ -373,8 +377,11 @@ class DeviceCluster:
                 perm.extend((len(perm) + order).tolist())
             # a solver stand-in need take no more fields than the call uses, nor ``explain`` unless it is asked for
             pods = (idx, self._pods(sc.tops, sc.pod_groups, sc.packed), self._clocks(len(sc.tops), sc.now))
-            args.append(Scenario(*pods, sc.lift, edits, adds, sc.rounds)
-                        if sc.lift is not None or edits or adds or sc.rounds is not None else pods)
+            rel = None
+            if sc.releases is not None:
+                rel = self._releases(sc.releases, float(np.max(pods[2], initial=-np.inf)), sc.rounds or ())
+            args.append(Scenario(*pods, sc.lift, edits, adds, sc.rounds, rel)
+                        if sc.lift is not None or edits or adds or sc.rounds is not None or rel is not None else pods)
         res = fn(args, source=source, explain=True) if explain else fn(args, source=source)
         if perm and sorted(perm) != perm:
             n, back = len(self._names), np.asarray(perm, dtype=np.int64)
@@ -1010,31 +1017,69 @@ class NHDScheduler:
         busy from the delete) before the first scan at or after it; a pod that would give nothing back is left out, as
         the delete leaves it, and one after the last scan changes nothing.  A pod never annotated (its delete re-scans
         every node), a departure that is also among ``keys``, an offset <= 0, and ``departures`` together with
-        ``additions`` are ValueErrors.  Releases need the batch path (``Solver.plan_batch_releases``)."""
+        ``additions`` are ValueErrors.  Departures here run on the batch path (``Solver.plan_batch_releases``);
+        ``ForecastDepartures`` plans several departure schedules, with or without added nodes, in one call."""
         rel = None
         if departures is not None:
             if additions is not None:
                 raise ValueError('departures are planned on the cluster as it is, not with additions')
             if keys is None:
-                phase = self._service_pods()
-                keys = [k for k in phase if self._wanted(phase)(k)]
-            pending = {(k[0], k[1]) for k in keys}
-            rel = []
-            for (ns, name), offset in departures.items():
-                offset = float(offset)
-                if (ns, name) in pending:
-                    raise ValueError(f'pod {ns}.{name} is pending and cannot depart')
-                if not offset > 0.0:
-                    raise ValueError(f'departure of {ns}.{name} at {offset} s is not after the first scan')
-                target = self._release_target(name, ns)
-                if target is None:
-                    raise ValueError(f'pod {ns}.{name} was never annotated: its delete re-scans every node')
-                if target[0] is not None:
-                    rel.append((target[0], target[1], offset))
+                keys = self._pending_keys()
+            rel = self._departures(departures, keys)
         result = self._grown_plans([[]] if additions is None else additions, keys, reasons,
                                    self._scan_periods(scans, period), departures=rel)
         out = [(p, why) if reasons else p for p, why in result]
         return out[0] if additions is None else out
+
+    def ForecastDepartures(self, schedules: Sequence[Dict], scans: int, keys: Sequence = None, period: float = None,
+                           additions: Sequence = None, reasons: bool = False) -> List:
+        """``ForecastPending`` under several departure schedules side by side: "jobs A and B end in about 20 minutes:
+        does the queue clear then, or do I also need one more node like this one?".  ``schedules``: a sequence of
+        departure dicts, each as ``ForecastPending(departures=...)`` takes them (``{(ns, name): seconds after the first
+        scan}``).  ``additions`` None: every schedule on the cluster as it is; else one addition list per schedule, as
+        ``PlanExpansion`` takes them.  ``scans``, ``keys``, ``period`` and ``reasons`` as for ``ForecastPending``.
+        Returns one ``{(ns, name): (scan, node name) or None}`` per schedule, an added node named by its own name
+        (``reasons=True``: ``(placement, reasons)``).  All schedules are planned in one GPU call, one warp each
+        (``Solver.plan_scenarios`` with ``releases``); a pod beyond the solver's tuple limits maps to None.  The
+        departures are checked as ``ForecastPending`` checks them: a pod never annotated, a departure that is also
+        pending and an offset <= 0 are ValueErrors, as is an ``additions`` list of another length.
+        ``ForecastDepartures([d], n)`` is ``ForecastPending(n, departures=d)``.  Every schedule, an empty one too,
+        carries the signed NIC counters of the nodes that have a negative one, so ``ForecastDepartures([{}], n,
+        additions=[a])`` is ``ForecastPending(n, additions=[a])`` (which reads the NIC bits only) while no counter is
+        negative.  Only reads happen, as ``ForecastPending``."""
+        schedules = list(schedules)
+        if additions is not None and len(additions) != len(schedules):
+            raise ValueError(f'{len(additions)} addition lists for {len(schedules)} schedules')
+        if keys is None:
+            keys = self._pending_keys()
+        deps = [self._departures(d, keys) for d in schedules]
+        result = self._grown_plans([[] for _ in schedules] if additions is None else additions, keys, reasons,
+                                   self._scan_periods(scans, period), schedules=deps)
+        return [(p, why) if reasons else p for p, why in result]
+
+    def _pending_keys(self) -> List:
+        """The pods the next ``CheckPendingPods`` would attempt, in its order."""
+        phase = self._service_pods()
+        return [k for k in phase if self._wanted(phase)(k)]
+
+    def _departures(self, departures: Dict, keys: Sequence) -> List[tuple]:
+        """``(node name, topology, seconds after the first scan)`` of the departures that give something back, as
+        their deletes would (``_release_target``); a pending pod among ``keys``, an offset <= 0 and a pod never
+        annotated are ValueErrors."""
+        pending = {(k[0], k[1]) for k in keys}
+        rel = []
+        for (ns, name), offset in departures.items():
+            offset = float(offset)
+            if (ns, name) in pending:
+                raise ValueError(f'pod {ns}.{name} is pending and cannot depart')
+            if not offset > 0.0:
+                raise ValueError(f'departure of {ns}.{name} at {offset} s is not after the first scan')
+            target = self._release_target(name, ns)
+            if target is None:
+                raise ValueError(f'pod {ns}.{name} was never annotated: its delete re-scans every node')
+            if target[0] is not None:
+                rel.append((target[0], target[1], offset))
+        return rel
 
     def ForecastDrain(self, node_names: Sequence[str], scans: int, period: float = None, reasons: bool = False):
         """When do the pods of drained nodes get back in?  ``PlanDrain``'s pods (the pods now on ``node_names``, nodes in
@@ -1062,11 +1107,12 @@ class NHDScheduler:
         return [float(60 * 0.5 if period is None else period)] * (scans - 1)
 
     def _grown_plans(self, additions: Sequence[Sequence], keys: Sequence, reasons: bool, periods: Sequence[float],
-                     exclude: Sequence[str] = (), departures: Sequence = None):
+                     exclude: Sequence[str] = (), departures: Sequence = None, schedules: Sequence = None):
         """``PlanExpansion``'s plans, with a later scan after each of ``periods`` seconds: per scenario ``(placement,
         reasons)``, a placed pod mapped to its node name, or with ``periods`` (even an empty list) to ``(scan, node
         name)``.  ``periods`` None: one scan, through the call without rounds.  ``exclude``: nodes in maintenance
-        throughout, in every scenario."""
+        throughout, in every scenario.  ``departures`` (``_departures``' list): releases on the batch path, for one
+        scenario without additions; ``schedules``: one such list per scenario, planned on the scenario path."""
         scens = [[(node, before) for node, before in sc] for sc in additions]
         for sc in scens:
             names = [node.name for node, _ in sc]
@@ -1092,18 +1138,22 @@ class NHDScheduler:
                 for p in periods:
                     clocks.append(clocks[-1] + float(p))
                 clocks = clocks[1:]
-            releases = None
-            if departures is not None:              # seconds after the first scan -> clocks (a scan's own when equal)
-                offs, releases = [], []
-                for p in periods:
-                    offs.append((offs[-1] if offs else 0.0) + float(p))
-                for node, top, off in departures:
+            offs = []
+            for p in periods or ():
+                offs.append((offs[-1] if offs else 0.0) + float(p))
+
+            def release_clocks(deps):               # seconds after the first scan -> clocks (a scan's own when equal)
+                releases = []
+                for node, top, off in deps:
                     if offs and off <= offs[-1]:
                         k = next(k for k, o in enumerate(offs) if off <= o)
                         at = clocks[k] if off == offs[k] else max(now + off, clocks[k - 1] if k else now)
                         releases.append((node, top, min(at, clocks[k])))
+                return releases
+            releases = None if departures is None else release_clocks(departures)
+            scheduled = None if schedules is None else [release_clocks(d) for d in schedules]
             todo = [(j, entries) for j in range(len(scens))]
-            if clocks is not None and scens == [[]]:
+            if clocks is not None and scens == [[]] and schedules is None:
                 # one scenario on the cluster as it is: one batch per scan (a pod beyond the tuple limits is dropped
                 # and the rest planned again, as _plan_prepared does)
                 res, ok, _ = self._without_refused(
@@ -1125,7 +1175,8 @@ class NHDScheduler:
             planned = self._plan_refused(
                 todo, lambda item: ClusterScenario(exclude, [e.top for e in item[1]], [e.groups for e in item[1]], now,
                                                    [e.rec for e in item[1]], rounds=clocks,
-                                                   adds=[(before, node) for node, before in scens[item[0]]]),
+                                                   adds=[(before, node) for node, before in scens[item[0]]],
+                                                   releases=None if scheduled is None else scheduled[item[0]]),
                 lambda item, pod: (item[0], item[1][:pod] + item[1][pod + 1:]) if len(item[1]) > 1 else None, reasons,
                 lambda item, code, pod: f'nhd_plan_scenarios_grown refused scenario {item[0]}: code {code}, pod {pod}')
             n_nodes = len(self.nodes)

@@ -1582,7 +1582,12 @@ extern "C" int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_
  * one names it n_nodes + its call-wide index.  With rounds (nhd_plan_scenarios_rounds) the same warp walks the
  * scenario's unplaced pods again at each round clock (scenario_plan_kernel<., true>); scenario s's slots then start at
  * slot_start[s] and hold n_edits + n_adds + min(n_s * (1 + R_s), n_nodes) records, and the reasons' base pass reads
- * each pod's clock of its last attempt instead of the staged clocks.
+ * each pod's clock of its last attempt instead of the staged clocks.  With releases (nhd_plan_scenarios_releases,
+ * scenario_plan_kernel<., true, true>, the rounds layout even without round clocks) the accepted scenarios' tracked
+ * nodes, counts (int32, seeded from pods_used, after the pod rounds in d_sidx) and releases are compacted like the
+ * rest, each release carrying its node's compacted count row; a scenario's slots grow by its distinct released nodes,
+ * min(n_s * (1 + R_s) + D_s, n_nodes).  release_check_kernel first checks the call's releases and tracked counts
+ * against the source records, one word read back.
  */
 /*
  * why_counts of the scenario call just run on w (its bindings b, its pods and clocks run_pods / run_now, its correction
@@ -1640,24 +1645,29 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
                               const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
                               const int32_t* add_start, const int32_t* add_at, const nhd_node_rec* add_rec,
                               const int32_t* pod_start, const nhd_pod* pods, const double* now,
-                              const int32_t* round_start, const double* round_clock, nhd_binding* out,
-                              int32_t* scenario_status, int32_t* scenario_pod, uint32_t* why_counts, int32_t* pod_round)
+                              const int32_t* round_start, const double* round_clock, const int32_t* track_start,
+                              const int32_t* tracked, const int16_t* pods_used, const int32_t* rel_start,
+                              const nhd_release* releases, nhd_binding* out, int32_t* scenario_status,
+                              int32_t* scenario_pod, uint32_t* why_counts, int32_t* pod_round)
 {
     if (!h || n_scenarios < 0 || !excl_start || !pod_start || (n_scenarios > 0 && (!scenario_status || !scenario_pod)))
         return NHD_ERR_INVALID;
     if (excl_start[0] != 0 || pod_start[0] != 0 || (edit_start && edit_start[0] != 0) || (add_start && add_start[0] != 0) ||
-        (round_start && round_start[0] != 0))
+        (round_start && round_start[0] != 0) || (track_start && track_start[0] != 0) || (rel_start && rel_start[0] != 0))
         return fail(h, NHD_ERR_INVALID, "scenario offsets must start at 0");
     for (int s = 0; s < n_scenarios; s++)
         if (excl_start[s + 1] < excl_start[s] || pod_start[s + 1] < pod_start[s] ||
             (edit_start && edit_start[s + 1] < edit_start[s]) || (add_start && add_start[s + 1] < add_start[s]) ||
-            (round_start && round_start[s + 1] < round_start[s]))
+            (round_start && round_start[s + 1] < round_start[s]) || (track_start && track_start[s + 1] < track_start[s]) ||
+            (rel_start && rel_start[s + 1] < rel_start[s]))
             return fail(h, NHD_ERR_INVALID, "scenario %d: offsets go down", s);
     const int n_excl = excl_start[n_scenarios], n_pods = pod_start[n_scenarios];
     const int n_edit = edit_start ? edit_start[n_scenarios] : 0, n_add = add_start ? add_start[n_scenarios] : 0;
     const int n_round = round_start ? round_start[n_scenarios] : 0;
+    const int n_trk = track_start ? track_start[n_scenarios] : 0, n_rel = rel_start ? rel_start[n_scenarios] : 0;
     if ((n_excl > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)) || (n_edit > 0 && (!edit_node || !edit_rec)) ||
-        (n_add > 0 && (!add_at || !add_rec)) || (n_round > 0 && !round_clock))
+        (n_add > 0 && (!add_at || !add_rec)) || (n_round > 0 && !round_clock) ||
+        (n_trk > 0 && (!tracked || !pods_used)) || (n_rel > 0 && !releases))
         return NHD_ERR_INVALID;
     for (int s = 0; s < n_scenarios && n_round > 0; s++)
         for (int r = round_start[s]; r < round_start[s + 1]; r++) {
@@ -1711,14 +1721,88 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
                                 k, nic_speed_class(add_rec[e], k), h->params.n_speed_classes);
             max_numa = std::max(max_numa, (int)add_rec[e].n_numa);
         }
+    /* releases (nhd_plan_scenarios_releases): per release its node's call-wide tracked row, per scenario its distinct
+     * released nodes (the slot bound grows by them) */
+    const bool with_releases = track_start || rel_start;
+    std::vector<int32_t> rel_row((size_t)n_rel), rel_nodes(with_releases ? n_scenarios : 0, 0);
+    for (int s = 0; s < n_scenarios && with_releases; s++) {
+        const int t0 = track_start ? track_start[s] : 0, t1 = track_start ? track_start[s + 1] : 0;
+        std::vector<std::pair<int32_t, int32_t>> trk;                   /* (node, call-wide row), sorted by node */
+        for (int t = t0; t < t1; t++) {
+            if (tracked[t] < 0 || tracked[t] >= h->n_nodes)
+                return fail(h, NHD_ERR_INVALID, "tracked node %d outside the %d loaded nodes", tracked[t], h->n_nodes);
+            trk.emplace_back(tracked[t], t);
+        }
+        std::sort(trk.begin(), trk.end());
+        for (size_t k = 1; k < trk.size(); k++)
+            if (trk[k].first == trk[k - 1].first)
+                return fail(h, NHD_ERR_INVALID, "scenario %d: node %d tracked twice", s, trk[k].first);
+        const int l0 = rel_start ? rel_start[s] : 0, l1 = rel_start ? rel_start[s + 1] : 0;
+        const int R_s = round_start ? round_start[s + 1] - round_start[s] : 0;
+        const double* clk = round_start ? round_clock + round_start[s] : nullptr;
+        if (l1 > l0 && R_s == 0) return fail(h, NHD_ERR_INVALID, "scenario %d: releases without rounds", s);
+        double t_first = -INFINITY;
+        for (int i = pod_start[s]; i < pod_start[s + 1]; i++) t_first = std::max(t_first, now[i]);
+        std::vector<int32_t> seen;
+        for (int k = l0; k < l1; k++) {
+            const nhd_release& rl = releases[k];
+            if (rl.round < 1 || rl.round > R_s)
+                return fail(h, NHD_ERR_INVALID, "scenario %d: release %d: round %d outside [1, %d]", s, k - l0, rl.round, R_s);
+            if (!std::isfinite(rl.clock))
+                return fail(h, NHD_ERR_INVALID, "scenario %d: release %d: clock is not finite", s, k - l0);
+            if (k > l0 && rl.clock < releases[k - 1].clock)
+                return fail(h, NHD_ERR_INVALID, "scenario %d: release clocks go down at %d", s, k - l0);
+            if (rl.clock < (rl.round > 1 ? clk[rl.round - 2] : t_first) || rl.clock > clk[rl.round - 1])
+                return fail(h, NHD_ERR_INVALID, "scenario %d: release %d: clock outside the gap before round %d", s,
+                            k - l0, rl.round);
+            const auto it = std::lower_bound(trk.begin(), trk.end(), std::make_pair(rl.node, (int32_t)INT32_MIN));
+            if (it == trk.end() || it->first != rl.node)
+                return fail(h, NHD_ERR_INVALID, "scenario %d: release %d: node %d is not tracked", s, k - l0, rl.node);
+            for (int e = edit_start ? edit_start[s] : 0; e < (edit_start ? edit_start[s + 1] : 0); e++)
+                if (edit_node[e] == rl.node)
+                    return fail(h, NHD_ERR_INVALID, "scenario %d: release %d: node %d is one the scenario edits", s,
+                                k - l0, rl.node);
+            rel_row[k] = it->second;
+            seen.push_back(rl.node);
+        }
+        std::sort(seen.begin(), seen.end());
+        rel_nodes[s] = (int32_t)(std::unique(seen.begin(), seen.end()) - seen.begin());
+    }
+    if (n_rel + n_trk > 0) {           /* the checks that need the records (release_check_kernel), one word read back */
+        const int32_t none = 0x7FFFFFFF;
+        CK(cudaSetDevice(h->params.device));
+        CK(h->d_rel.grow(4));
+        CK(h->d_rels.grow((size_t)std::max(n_rel, 1) * sizeof(nhd_release)));
+        CK(h->d_pidx.grow((size_t)std::max(n_trk, 1) * (4 + NHD_MAX_NICS * 2)));
+        CK(cudaMemcpyAsync(h->d_rel, &none, 4, cudaMemcpyHostToDevice, h->stream));
+        if (n_rel) CK(cudaMemcpyAsync(h->d_rels, releases, (size_t)n_rel * sizeof(nhd_release), cudaMemcpyHostToDevice, h->stream));
+        if (n_trk) {
+            CK(cudaMemcpyAsync(h->d_pidx, tracked, (size_t)n_trk * 4, cudaMemcpyHostToDevice, h->stream));
+            CK(cudaMemcpyAsync(h->d_pidx + n_trk, pods_used, (size_t)n_trk * NHD_MAX_NICS * 2, cudaMemcpyHostToDevice, h->stream));
+        }
+        release_check_kernel<<<(n_rel + n_trk + 255) / 256, 256, 0, h->stream>>>(
+            records, h->d_rels, n_rel, h->d_pidx, reinterpret_cast<const int16_t*>(h->d_pidx + n_trk), n_trk, h->d_rel);
+        CK(cudaGetLastError());
+        int32_t bad = 0;
+        CK(cudaMemcpyAsync(&bad, h->d_rel, 4, cudaMemcpyDeviceToHost, h->stream));
+        CK(cudaStreamSynchronize(h->stream));
+        if (bad < n_rel)
+            return fail(h, NHD_ERR_INVALID, "release %d: a core, GPU or NIC beyond node %d's own", bad, releases[bad].node);
+        if (bad != none)
+            return fail(h, NHD_ERR_INVALID, "tracked node %d: pods_used disagrees with its NIC bits", tracked[bad - n_rel]);
+    }
+    const bool rounds = round_start != nullptr || with_releases;
 
     /* per scenario: its refusal, or its place among the accepted ones (pods, exclusions and edits compacted, the
      * exclusions sorted and each once).  idx = pod offsets | exclusion offsets | exclusions | edit offsets | edited
      * nodes | lift indices | add offsets | add positions of the accepted scenarios, and with rounds | round offsets |
-     * first working slots. */
+     * first working slots, and with releases | track offsets | tracked nodes | release offsets | release rows. */
     std::vector<int32_t> acc, pod_off{0}, ex_off{0}, ex, ed_off{0}, ed_node, lift, ad_off{0}, ad_at, rd_off{0}, sl_start;
+    std::vector<int32_t> tr_off, tr_node, tr_count, rl_off, rl_row;
     std::vector<nhd_node_rec> ed_rec, ad_rec;
+    std::vector<nhd_release> rl_rec;
     std::vector<double> rd_clock;
+    if (with_releases) { tr_off.push_back(0); rl_off.push_back(0); }
     size_t n_slots = 0;
     for (int s = 0; s < n_scenarios; s++) {
         scenario_status[s] = NHD_OK;
@@ -1748,11 +1832,26 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         ad_off.push_back((int32_t)ad_at.size());
         const int64_t n_s = pod_start[s + 1] - pod_start[s];
         int64_t touches = n_s;                 /* without rounds: one slot per pod, as scenario_plan_kernel<., false> */
-        if (round_start) {
-            rd_clock.insert(rd_clock.end(), round_clock + round_start[s], round_clock + round_start[s + 1]);
+        if (rounds) {
+            const int64_t R_s = round_start ? round_start[s + 1] - round_start[s] : 0;
+            if (round_start) rd_clock.insert(rd_clock.end(), round_clock + round_start[s], round_clock + round_start[s + 1]);
             rd_off.push_back((int32_t)rd_clock.size());
             sl_start.push_back((int32_t)n_slots);
-            touches = std::min(n_s * (1 + (int64_t)(round_start[s + 1] - round_start[s])), (int64_t)h->n_nodes);
+            touches = std::min(n_s * (1 + R_s) + (with_releases ? rel_nodes[s] : 0), (int64_t)h->n_nodes);
+        }
+        if (with_releases) {
+            const int t0 = track_start ? track_start[s] : 0, t1 = track_start ? track_start[s + 1] : 0;
+            const int row0 = (int)tr_node.size() - t0;                /* call-wide row -> compacted row */
+            for (int t = t0; t < t1; t++) {
+                tr_node.push_back(tracked[t]);
+                for (int i = 0; i < NHD_MAX_NICS; i++) tr_count.push_back(pods_used[(size_t)t * NHD_MAX_NICS + i]);
+            }
+            tr_off.push_back((int32_t)tr_node.size());
+            for (int k = rel_start ? rel_start[s] : 0; k < (rel_start ? rel_start[s + 1] : 0); k++) {
+                rl_rec.push_back(releases[k]);
+                rl_row.push_back(row0 + rel_row[k]);
+            }
+            rl_off.push_back((int32_t)rl_rec.size());
         }
         n_slots += (size_t)(touches + (edit_start ? edit_start[s + 1] - edit_start[s] : 0) +
                             (add_start ? add_start[s + 1] - add_start[s] : 0));
@@ -1777,19 +1876,23 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
 
     std::vector<int32_t> idx;
     idx.reserve(pod_off.size() + ex_off.size() + ex.size() + ed_off.size() + ed_node.size() + lift.size() +
-                ad_off.size() + ad_at.size() + rd_off.size() + sl_start.size());
-    for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift, &ad_off, &ad_at, &rd_off, &sl_start})
+                ad_off.size() + ad_at.size() + rd_off.size() + sl_start.size() + tr_off.size() + tr_node.size() +
+                rl_off.size() + rl_row.size());
+    for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift, &ad_off, &ad_at, &rd_off, &sl_start, &tr_off,
+                          &tr_node, &rl_off, &rl_row})
         idx.insert(idx.end(), v->begin(), v->end());
     const size_t off_ex_off = pod_off.size(), off_ex = off_ex_off + ex_off.size(), off_ed_off = off_ex + ex.size();
     const size_t off_ed_node = off_ed_off + ed_off.size(), off_lift = off_ed_node + ed_node.size();
     const size_t off_ad_off = off_lift + lift.size(), off_ad_at = off_ad_off + ad_off.size();
     const size_t off_rd_off = off_ad_at + ad_at.size(), off_sl = off_rd_off + rd_off.size();
+    const size_t off_tr_off = off_sl + sl_start.size(), off_tr_node = off_tr_off + tr_off.size();
+    const size_t off_rl_off = off_tr_node + tr_node.size(), off_rl_row = off_rl_off + rl_off.size();
     const size_t off_nodes = idx.size(), off_bad = off_nodes + n_slots, off_round = off_bad + 1;
-    const bool rounds = round_start != nullptr;
+    const size_t off_count = off_round + (rounds ? n_run : 0);     /* with releases: the tracked counts */
     /* d_swork: the working slots, then the edit records and the added records the kernel seeds them from, then (with
      * rounds) the round clocks and the clocks of each pod's last attempt (reasons' base pass), 16-byte chunks */
     const size_t rd_chunks = rounds ? (rd_clock.size() + 1) / 2 : 0, last_chunks = rounds && why_counts ? ((size_t)n_run + 1) / 2 : 0;
-    CK(h->d_sidx.grow((off_round + (rounds ? n_run : 0)) * 4));
+    CK(h->d_sidx.grow((off_count + tr_count.size()) * 4));
     CK(h->d_swork.grow((n_slots + n_ed + n_ad) * sizeof(nhd_node_rec) + (rd_chunks + last_chunks) * 16));
     CK(cudaMemcpyAsync(h->d_sidx, idx.data(), idx.size() * 4, cudaMemcpyHostToDevice, h->stream));
     CK(cudaMemsetAsync(h->d_sidx + off_bad, 0, 4, h->stream));
@@ -1803,6 +1906,12 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         CK(cudaMemcpyAsync(d_add_rec, ad_rec.data(), (size_t)n_ad * sizeof(nhd_node_rec), cudaMemcpyHostToDevice, h->stream));
     if (!rd_clock.empty())
         CK(cudaMemcpyAsync(d_round_clock, rd_clock.data(), rd_clock.size() * 8, cudaMemcpyHostToDevice, h->stream));
+    if (!tr_count.empty())
+        CK(cudaMemcpyAsync(h->d_sidx + off_count, tr_count.data(), tr_count.size() * 4, cudaMemcpyHostToDevice, h->stream));
+    if (!rl_rec.empty()) {  /* the accepted scenarios' releases, in place of the call's that the check read */
+        CK(h->d_rels.grow(rl_rec.size() * sizeof(nhd_release)));
+        CK(cudaMemcpyAsync(h->d_rels, rl_rec.data(), rl_rec.size() * sizeof(nhd_release), cudaMemcpyHostToDevice, h->stream));
+    }
     if (why_counts) {       /* scenario_reasons' buffers: base rows | rows, base_row | keys | corrections, node lists */
         CK(h->d_xcounts.grow((size_t)2 * n_run * NHD_WHY_COUNT * 4));
         CK(h->d_xpod.grow((size_t)n_run * (NHD_WHY_COUNT + 3) * 4));
@@ -1827,12 +1936,16 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     sa.why_delta = why_counts ? h->d_xpod + 2 * (size_t)n_run : nullptr;
     sa.round_start = h->d_sidx + off_rd_off; sa.round_clock = d_round_clock; sa.slot_start = h->d_sidx + off_sl;
     sa.pod_round = h->d_sidx + off_round;
+    sa.track_start = h->d_sidx + off_tr_off; sa.tracked = h->d_sidx + off_tr_node; sa.count = h->d_sidx + off_count;
+    sa.rel_start = h->d_sidx + off_rl_off; sa.rel = h->d_rels; sa.rel_track = h->d_sidx + off_rl_row;
     const int warps_per_cta = SCENARIO_THREADS / 32;
     const int grid = std::min((n_acc + warps_per_cta - 1) / warps_per_cta, h->sm_count * 16);
     /* through a pointer: the CPU emulation (tests/emu) rewrites a launch into a macro call, whose argument list would
      * split a kernel name with two template arguments */
-    void (*const kernel)(ScenarioArgs) = rounds ? (why_counts ? scenario_plan_kernel<true, true> : scenario_plan_kernel<false, true>)
-                                                : (why_counts ? scenario_plan_kernel<true, false> : scenario_plan_kernel<false, false>);
+    void (*const kernel)(ScenarioArgs) =
+        with_releases ? (why_counts ? scenario_plan_kernel<true, true, true> : scenario_plan_kernel<false, true, true>)
+        : rounds      ? (why_counts ? scenario_plan_kernel<true, true> : scenario_plan_kernel<false, true>)
+                      : (why_counts ? scenario_plan_kernel<true, false> : scenario_plan_kernel<false, false>);
     kernel<<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
     CK(cudaGetLastError());
     uint32_t bad = 0;
@@ -1887,8 +2000,8 @@ extern "C" int32_t nhd_plan_scenarios(nhd_handle* h, int32_t source, int32_t n_s
                                       int32_t* scenario_pod)
 {
     return plan_scenarios(h, "nhd_plan_scenarios", source, n_scenarios, excl_start, excluded, nullptr, nullptr, nullptr,
-                          nullptr, nullptr, nullptr, nullptr, pod_start, pods, now, nullptr, nullptr, out,
-                          scenario_status, scenario_pod, nullptr, nullptr);
+                          nullptr, nullptr, nullptr, nullptr, pod_start, pods, now, nullptr, nullptr, nullptr,
+                          nullptr, nullptr, nullptr, nullptr, out, scenario_status, scenario_pod, nullptr, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1900,7 +2013,8 @@ extern "C" int32_t nhd_plan_scenarios_edited(nhd_handle* h, int32_t source, int3
 {
     return plan_scenarios(h, "nhd_plan_scenarios_edited", source, n_scenarios, excl_start, excluded, lift_at,
                           edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, nullptr,
-                          nullptr, out, scenario_status, scenario_pod, nullptr, nullptr);
+                          nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out, scenario_status, scenario_pod, nullptr,
+                          nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1913,7 +2027,8 @@ extern "C" int32_t nhd_plan_scenarios_explained(nhd_handle* h, int32_t source, i
 {
     return plan_scenarios(h, "nhd_plan_scenarios_explained", source, n_scenarios, excl_start, excluded, lift_at,
                           edit_start, edit_node, edit_rec, nullptr, nullptr, nullptr, pod_start, pods, now, nullptr,
-                          nullptr, out, scenario_status, scenario_pod, why_counts, nullptr);
+                          nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out, scenario_status, scenario_pod,
+                          why_counts, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_grown(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1927,7 +2042,8 @@ extern "C" int32_t nhd_plan_scenarios_grown(nhd_handle* h, int32_t source, int32
 {
     return plan_scenarios(h, "nhd_plan_scenarios_grown", source, n_scenarios, excl_start, excluded, lift_at,
                           edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now, nullptr,
-                          nullptr, out, scenario_status, scenario_pod, why_counts, nullptr);
+                          nullptr, nullptr, nullptr, nullptr, nullptr, nullptr, out, scenario_status, scenario_pod,
+                          why_counts, nullptr);
 }
 
 extern "C" int32_t nhd_plan_scenarios_rounds(nhd_handle* h, int32_t source, int32_t n_scenarios,
@@ -1942,7 +2058,26 @@ extern "C" int32_t nhd_plan_scenarios_rounds(nhd_handle* h, int32_t source, int3
 {
     return plan_scenarios(h, "nhd_plan_scenarios_rounds", source, n_scenarios, excl_start, excluded, lift_at,
                           edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now,
-                          round_start, round_clock, out, scenario_status, scenario_pod, why_counts, pod_round);
+                          round_start, round_clock, nullptr, nullptr, nullptr, nullptr, nullptr, out, scenario_status,
+                          scenario_pod, why_counts, pod_round);
+}
+
+extern "C" int32_t nhd_plan_scenarios_releases(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                               const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                               const int32_t* edit_start, const int32_t* edit_node,
+                                               const nhd_node_rec* edit_rec, const int32_t* add_start,
+                                               const int32_t* add_at, const nhd_node_rec* add_rec,
+                                               const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                               const int32_t* round_start, const double* round_clock,
+                                               const int32_t* track_start, const int32_t* tracked,
+                                               const int16_t* pods_used, const int32_t* rel_start,
+                                               const nhd_release* releases, nhd_binding* out, int32_t* scenario_status,
+                                               int32_t* scenario_pod, uint32_t* why_counts, int32_t* pod_round)
+{
+    return plan_scenarios(h, "nhd_plan_scenarios_releases", source, n_scenarios, excl_start, excluded, lift_at,
+                          edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now,
+                          round_start, round_clock, track_start, tracked, pods_used, rel_start, releases, out,
+                          scenario_status, scenario_pod, why_counts, pod_round);
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

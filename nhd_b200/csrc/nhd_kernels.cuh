@@ -3037,6 +3037,13 @@ struct ScenarioArgs {
     const double* round_clock;     /* each scenario's later rounds' clocks */
     const int32_t* slot_start;     /* [n_scenarios]: scenario s's first working slot (replaces the fixed layout) */
     int32_t* pod_round;            /* [n_pods]: the round that placed the pod, or the scenario's round count */
+    /* scenario_plan_kernel<., true, true> only (nhd_plan_scenarios_releases) */
+    const int32_t* track_start;    /* [n_scenarios + 1] into tracked / count */
+    const int32_t* tracked;        /* each scenario's tracked nodes, each once */
+    int32_t* count;                /* [tracked][NHD_MAX_NICS]: the signed NIC pod counts, seeded with pods_used */
+    const int32_t* rel_start;      /* [n_scenarios + 1] into rel / rel_track */
+    const nhd_release* rel;        /* each scenario's releases, in array order */
+    const int32_t* rel_track;      /* [release]: its node's row of count */
 };
 
 constexpr int SCENARIO_THREADS = 128;
@@ -3098,6 +3105,54 @@ __device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const Pod
     }
 }
 
+/* scenario_plan_kernel<., true, true> at the start of round r >= 1, the whole warp: when a pod of the scenario is still
+ * unplaced, its releases with round == r in array order, each on its node's working record (AddResourcesFromTopology
+ * + SetBusy, as release_kernel): core and GPU bits cleared, hugepages added when > 0, the node's counts lowered by the
+ * pairings and its NIC bits rewritten as count > 0, busy_time = the release clock.  A released node not yet touched
+ * gets the next slot, seeded from its source record, and is touched from then on.  Returns the new touched count. */
+__device__ __noinline__ int scenario_releases(const ScenarioArgs& a, int r, int p0, int p1, int l0, int l1, uint4* work,
+                                              int32_t* work_node, int n_touched)
+{
+    const int lane = threadIdx.x & 31;
+    int pending = 0;
+    for (int i = p0 + lane; i < p1; i += 32) pending |= a.out[i].status != NHD_PLACED;
+    if (!__ballot_sync(0xFFFFFFFFu, pending)) return n_touched;
+    for (int j = l0; j < l1; j++) {
+        const nhd_release& rl = a.rel[j];
+        if (rl.round != r) continue;                                   /* warp-uniform */
+        const int node = rl.node;
+        int slot = n_touched;
+        for (int base = 0; base < n_touched; base += 32) {
+            const unsigned m = __ballot_sync(0xFFFFFFFFu, base + lane < n_touched && work_node[base + lane] == node);
+            if (m) { slot = base + ctz32(m); break; }
+        }
+        if (lane == 0) {
+            RecU u;
+            if (slot < n_touched) {
+                for (int c = 0; c < REC_CHUNKS; c++) u.q[c] = work[(size_t)slot * REC_CHUNKS + c];
+            } else {
+                load_rec(a.nodes, node, u);
+            }
+            for (int w = 0; w < 4; w++) u.r.used[w] &= ~rl.cores[w];
+            u.r.gpu_used &= (uint16_t)~rl.gpus;
+            if (rl.hugepages_gb > 0) u.r.free_hugepages_gb += rl.hugepages_gb;
+            int32_t* cnt = a.count + (size_t)a.rel_track[j] * NHD_MAX_NICS;
+            uint32_t inuse = 0;
+            for (int i = 0; i < u.r.n_nics; i++) {
+                cnt[i] -= rl.nic_pairings[i];
+                inuse |= (cnt[i] > 0 ? 1u : 0u) << i;
+            }
+            u.r.nic_inuse = inuse;
+            u.r.busy_time = rl.clock;
+            for (int c = 0; c < REC_CHUNKS; c++) work[(size_t)slot * REC_CHUNKS + c] = u.q[c];
+            work_node[slot] = node;
+        }
+        if (slot == n_touched) n_touched++;
+        __syncwarp();                                                  /* the slot is read by every lane from here on */
+    }
+    return n_touched;
+}
+
 /* One warp per scenario (grid-stride).  The working set starts with the scenario's edited records, then its added
  * ones.  For each pod: the first touched node, not excluded, that passes every stage on its working record
  * (explain_node, lanes over the touched set, warp minimum of the order key) and the first untouched candidate (query_select_kernel's ballot scan, skipping excluded and touched
@@ -3110,8 +3165,14 @@ __device__ __noinline__ void scenario_why_delta(const ScenarioArgs& a, const Pod
  * last pod stay held.  The touched set stays exact across rounds (a round only adds the nodes its own attempts reach),
  * but an attempt that fails its assignment can reach a new node in every round, so the scenario's slots start at
  * slot_start[s], sized by the host for n_edits + n_adds + min(n_pods * (1 + rounds), n_nodes) touched nodes: at most
- * one new node per attempt, and each source node at most once. */
-template <bool WHY, bool ROUNDS>
+ * one new node per attempt, and each source node at most once.
+ * RELEASES (nhd_plan_scenarios_releases, always with ROUNDS): each later round first plays the scenario's releases of
+ * that round (scenario_releases), which can touch each released node once more, so the host sizes the slots for
+ * n_edits + n_adds + min(n_pods * (1 + rounds) + distinct released nodes, n_nodes).  After a placement on a tracked
+ * node lane 0 raises the node's count of every claimed NIC and clears the bit where the count is still <= 0
+ * (ClaimPodNICResources, Node.py:644-646).  The warp commits one pod at a time, so this is the reference's counter
+ * rule exactly: two pods can share a NIC a release drove to -1 without any cut. */
+template <bool WHY, bool ROUNDS, bool RELEASES = false>
 __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const __grid_constant__ ScenarioArgs a)
 {
     const int lane = threadIdx.x & 31, W = a.words;
@@ -3142,6 +3203,10 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
         __syncwarp();                                    /* the edited nodes are the first touched ones, then the added */
         int n_touched = n_edits + n_adds;
         for (int r = 0; r <= n_rounds; r++) {
+            if constexpr (RELEASES) {
+                if (r > 0 && a.rel_start[s + 1] > a.rel_start[s])
+                    n_touched = scenario_releases(a, r, p0, p1, a.rel_start[s], a.rel_start[s + 1], work, work_node, n_touched);
+            }
             for (int i = p0; i < p1; i++) {
                 if constexpr (ROUNDS) {                                    /* lane 0 wrote the pod's last binding */
                     if (r > 0 && __shfl_sync(0xFFFFFFFFu, lane == 0 ? a.out[i].status : 0, 0) == NHD_PLACED) continue;
@@ -3223,6 +3288,14 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
                         slot = best_k;
                     }
                 }
+                int trk = -1;                                              /* the chosen node's row of count, if tracked */
+                if constexpr (RELEASES) {
+                    const int t0 = a.track_start[s], n_tr = a.track_start[s + 1] - t0;
+                    for (int base = 0; chosen >= 0 && chosen < a.n_nodes && base < n_tr; base += 32) {
+                        const unsigned m = __ballot_sync(0xFFFFFFFFu, base + lane < n_tr && a.tracked[t0 + base + lane] == chosen);
+                        if (m) { trk = t0 + base + ctz32(m); break; }
+                    }
+                }
                 if (lane == 0) {
                     union { nhd_binding b; uint4 q[8]; } bu;
                     for (int c = 0; c < 8; c++) bu.q[c] = make_uint4(0, 0, 0, 0);
@@ -3239,6 +3312,15 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
                         if (evaluate_mapping(u.r, t, a.cap, &m)) {
                             bu.b.node = chosen;
                             assign_pod(u.r, t, m, now, &bu.b);             /* the reference's unwind on a failed assignment */
+                            if constexpr (RELEASES) {
+                                if (trk >= 0 && bu.b.status == NHD_PLACED) {
+                                    int32_t* cnt = a.count + (size_t)trk * NHD_MAX_NICS;
+                                    for (int j = 0; j < (int)bu.b.n_claimed; j++) {
+                                        const int nic = bu.b.claimed_nics[j];
+                                        if (++cnt[nic] <= 0) u.r.nic_inuse &= ~(1u << nic);
+                                    }
+                                }
+                            }
                         } else {
                             atomicAdd(a.bad, 1u);                          /* the candidate test said feasible */
                             bu.q[0] = make_uint4(NHD_NO_CANDIDATE, 0xFFFFFFFFu, t.G, 0);

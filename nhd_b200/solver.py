@@ -71,7 +71,9 @@ class Scenario(NamedTuple):
     ``wire.NODE_DTYPE`` array: nodes added for the whole scenario, each right before source node ``at[k]``
     (``n_nodes``: at the end), ``at`` never going down.  ``rounds`` (None: none): the clocks of later pending scans,
     never going down and none before the scenario's pod clocks; at each, the scenario's pods not placed yet are solved
-    again in order on the records the previous scan left, and the bindings hold each pod's last attempt."""
+    again in order on the records the previous scan left, and the bindings hold each pod's last attempt.  ``releases``
+    (None: none): ``(tracked, pods_used, releases)`` as ``plan_batch_releases`` takes them, node indices of source
+    nodes the scenario does not edit, each release applied before its ``round`` (1 .. ``len(rounds)``)."""
     exclude: Sequence[int]
     pods: np.ndarray
     now: Sequence[float]
@@ -79,6 +81,7 @@ class Scenario(NamedTuple):
     edits: Optional[tuple] = None
     adds: Optional[tuple] = None
     rounds: Optional[Sequence[float]] = None
+    releases: Optional[tuple] = None
 
 
 class Solver:
@@ -299,14 +302,18 @@ class Solver:
         maintenance for the pods before ``lift`` and back after.  A pod placed on an added node gets node
         ``n_nodes + a``, ``a`` its index among the added records of the whole call, in scenario order.  When any
         scenario has ``rounds``, each result gains a last element: the ``(n_s,)`` int32 round that placed each pod, or
-        ``len(rounds)`` if none did (None when refused)."""
+        ``len(rounds)`` if none did (None when refused).  When any scenario has ``releases`` the call is
+        ``nhd_plan_scenarios_releases``: that scenario's deployed pods end between its rounds, each scenario on its own
+        records and NIC counters."""
         src = _source(source)
         # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
         # would cost more than the call itself)
         exs, podb, nowl, lifts, ednodes, edrecs, n_adds, adats, adrecs, rounds = [], [], [], [], [], [], [], [], [], []
+        rels = []
         for sc in scenarios:
             sc = Scenario(*sc)
             rounds.append(sc.rounds)
+            rels.append(sc.releases)
             pods = np.asarray(sc.pods)
             if pods.dtype != wire.POD_DTYPE:
                 pods = pods.astype(wire.POD_DTYPE)
@@ -365,13 +372,35 @@ class Solver:
             rnds = (round_start.ctypes.data, round_clock.ctypes.data if len(round_clock) else None)
             pod_round = np.zeros(len(pods), dtype='<i4')
         some = len(pods) > 0
-        self._ck(self._L.nhd_plan_scenarios_rounds(
-            self._h, src, n, excl_start.ctypes.data, ex.ctypes.data if len(ex) else None,
-            lift.ctypes.data if n else None, edit_start.ctypes.data, ednode.ctypes.data if len(ednode) else None,
-            edrec.ctypes.data if len(edrec) else None, *adds, pod_start.ctypes.data, pods.ctypes.data if some else None,
-            now.ctypes.data if some else None, *rnds, out.ctypes.data if some else None, status.ctypes.data,
-            which.ctypes.data, counts.ctypes.data if explain and some else None,
-            pod_round.ctypes.data if pod_round is not None and some else None))
+        args = [self._h, src, n, excl_start.ctypes.data, ex.ctypes.data if len(ex) else None,
+                lift.ctypes.data if n else None, edit_start.ctypes.data, ednode.ctypes.data if len(ednode) else None,
+                edrec.ctypes.data if len(edrec) else None, *adds, pod_start.ctypes.data,
+                pods.ctypes.data if some else None, now.ctypes.data if some else None, *rnds]
+        tail = [out.ctypes.data if some else None, status.ctypes.data, which.ctypes.data,
+                counts.ctypes.data if explain and some else None,
+                pod_round.ctypes.data if pod_round is not None and some else None]
+        if any(r is not None for r in rels):
+            # NULL release arrays unless some scenario has that field: existing calls go out as before
+            trs, useds, rls = [], [], []
+            for r in rels:
+                tr, used, rl = ((), (), None) if r is None else r
+                trs.append(np.asarray(tr, dtype='<i4').reshape(-1))
+                useds.append(np.asarray(used, dtype='<i2').reshape(len(trs[-1]), wire.MAX_NICS))
+                rls.append(np.zeros(0, dtype=wire.RELEASE_DTYPE) if rl is None else
+                           np.asarray(rl, dtype=wire.RELEASE_DTYPE).reshape(-1))
+            track_start = np.zeros(n + 1, dtype='<i4')
+            track_start[1:] = np.cumsum([len(t) for t in trs])
+            rel_start = np.zeros(n + 1, dtype='<i4')
+            rel_start[1:] = np.cumsum([len(x) for x in rls])
+            tracked = np.ascontiguousarray(np.concatenate(trs), dtype='<i4')
+            used = np.ascontiguousarray(np.concatenate(useds), dtype='<i2')
+            rel = np.ascontiguousarray(np.concatenate(rls), dtype=wire.RELEASE_DTYPE)
+            self._ck(self._L.nhd_plan_scenarios_releases(
+                *args, track_start.ctypes.data, tracked.ctypes.data if len(tracked) else None,
+                used.ctypes.data if len(tracked) else None, rel_start.ctypes.data, rel.ctypes.data if len(rel) else None,
+                *tail))
+        else:
+            self._ck(self._L.nhd_plan_scenarios_rounds(*args, *tail))
         res = self._scenario_results(status, which, pod_start, out, counts)
         if pod_round is None:
             return res
