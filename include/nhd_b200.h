@@ -582,6 +582,50 @@ int32_t nhd_plan_scenarios_releases(nhd_handle* h, int32_t source, int32_t n_sce
                                     nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
                                     uint32_t* why_counts, int32_t* pod_round);
 
+/*
+ * nhd_plan_scenarios_releases with pods created between the scans, per scenario: "we submit these 200 jobs at 10:05 and
+ * jobs A and B end at 10:10: when does each one start, and on which node?".  Every argument of
+ * nhd_plan_scenarios_releases keeps its meaning; pod i also has
+ *   arrive_round[i]  0: pending at plan start; r in [1, R_s]: created in the gap before round r, at clock now[i].  The
+ *                    round-0 pods come first in the scenario's pod order, and (arrive_round, now) never goes down in
+ *                    pod order.
+ * Per scenario: round 0 solves the round-0 pods in order, each at its now[].  Each gap r >= 1 then plays, merged by
+ * clock, the scenario's releases of round r and the first attempt of each pod arriving in it, solved alone at its
+ * now[] (the reference attempts a new pod on its create event); a release goes before an arrival at the same clock,
+ * and arrivals keep pod order.  Round r's scan then retries, in pod order at the round's clock, every arrived pod
+ * (arrive_round <= r) not placed yet, the gap's failed arrivals included.  A gap's releases are played while a pod of
+ * the scenario is unplaced or has not arrived yet.
+ *   out            the binding of each pod's placing attempt, or else of its last one;
+ *   pod_round      the round r whose arrival or scan placed the pod, or R_s if none did;
+ *   pod_clock      (may be NULL) the clock of the attempt whose binding is in out: now[i] or a round's clock;
+ *   why_counts     (may be NULL) as for nhd_plan_scenarios_releases: the row at the start of the pod's last attempt,
+ *                  always a scan (every gap is followed by its scan).
+ * Exclusions: lift_at[s] must be <= n0_s, the number of round-0 pods (the maintenance ends after round 0 from that
+ * pod on), or == n_s (held throughout).
+ * Identities: with arrive_round NULL the call is nhd_plan_scenarios_releases byte for byte, pod_clock then now[i] or
+ * the clock of the round that made the pod's last attempt.  A scenario whose pods all arrive in gap 1 and which has
+ * no release of round 1 gives the out, why_counts and pod_clock of nhd_plan_scenarios_releases on the same pods as
+ * round-0 pods at the same now[], and its pod_round with 0 read as 1.
+ * Besides nhd_plan_scenarios_releases' malformed arguments, the whole call is NHD_ERR_INVALID, before anything runs,
+ * for an arrive_round outside [0, R_s] or going down in pod order, an arrival in a scenario without rounds, arrival
+ * clocks going down among the arrivals of one gap, an arrival clock before the clock of the round before its gap (for
+ * gap 1: before a now[] of a round-0 pod) or after its own round's clock, and a lift_at other than the two above.
+ * The rule that no round clock is earlier than a now[] of its scenario reads the round-0 pods only, as does the lower
+ * bound of a round-1 release's clock.  Each pod is attempted at most 1 + R_s times, so the slot bound of
+ * nhd_plan_scenarios_releases holds.  Tuple limits, refusals per scenario, side effects (none observable), collectives
+ * (none) and waiting as for nhd_plan_scenarios_releases.
+ */
+int32_t nhd_plan_scenarios_arrivals(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                    const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                    const int32_t* edit_start, const int32_t* edit_node, const nhd_node_rec* edit_rec,
+                                    const int32_t* add_start, const int32_t* add_at, const nhd_node_rec* add_rec,
+                                    const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                    const int32_t* round_start, const double* round_clock,
+                                    const int32_t* track_start, const int32_t* tracked, const int16_t* pods_used,
+                                    const int32_t* rel_start, const nhd_release* releases, const int32_t* arrive_round,
+                                    nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                    uint32_t* why_counts, int32_t* pod_round, double* pod_clock);
+
 /* Per-pod-type feasibility bitmaps of the last solve's snapshot filter
  * (debug / tests): words[t * words_per_type + w], bit b of word w = node 64*w+b. */
 int32_t nhd_read_filter(nhd_handle* h, int32_t* n_types, int32_t* words_per_type,

@@ -89,7 +89,9 @@ class ClusterScenario(NamedTuple):
     each joining the node order right before the node named ``before`` (None: after the last node), packed by
     ``pack_candidates`` before any pod (a pod may request a group name only a candidate carries).  ``releases`` (None:
     none): ``[(node name, topology, clock)]`` of deployed pods that end between the scenario's ``rounds``, as
-    ``forecast(releases=...)`` takes them, on nodes the scenario does not edit."""
+    ``forecast(releases=...)`` takes them, on nodes the scenario does not edit.  ``arrive`` (None: every pod pending at
+    the start): per pod the round in the gap before which it is created at its own ``now`` (0: pending at the start),
+    as ``solver.Scenario.arrive``."""
     exclude: Iterable[str]
     tops: Sequence
     pod_groups: Sequence[Iterable[str]]
@@ -100,6 +102,18 @@ class ClusterScenario(NamedTuple):
     adds: Optional[Sequence[tuple]] = None
     rounds: Optional[Sequence[float]] = None
     releases: Optional[Sequence[tuple]] = None
+    arrive: Optional[Sequence[int]] = None
+
+
+class Arrival(NamedTuple):
+    """A pod ``ForecastArrivals`` expects to be created: ``key`` ``(ns, name)``, its config as the pod's config map
+    holds it (``cfgtype``, ``cfgstr``, read through ``GetCfgParser(cfgtype, cfgstr).CfgToTopology(False)``), its node
+    groups, and ``at``, the seconds after the first scan at which it is created."""
+    key: tuple
+    cfgtype: str
+    cfgstr: str
+    groups: Sequence[str]
+    at: float
 
 
 def _type_name(t) -> str:
@@ -348,7 +362,9 @@ class DeviceCluster:
         """Many independent dry runs in one GPU call, each as ``plan`` would answer it alone.  ``scenarios``: a sequence
         of ``ClusterScenario`` records, or plain tuples of their fields in order.  When any scenario has ``rounds``,
         each result gains the per-pod round that placed the pod (``Solver.plan_scenarios``).  A scenario's ``releases``
-        are packed as ``forecast`` packs them, with that scenario's clocks and rounds.
+        are packed as ``forecast`` packs them, with that scenario's clocks and rounds.  When any scenario has
+        ``arrive``, each result also gains the clock of each pod's attempt in its bindings; a release's round is then
+        judged from the clocks of the round-0 pods.
         Returns one ``(code, pod, bindings)`` per scenario (``Solver.plan_scenarios``): ``bindings`` None
         when the scenario is refused, ``code`` and ``pod`` saying why and for which of its pods; ``explain=True``: one
         ``(code, pod, bindings, counts)``, ``counts`` the per-reason node counts of the NO_CANDIDATE pods.  A pod
@@ -379,9 +395,13 @@ class DeviceCluster:
             pods = (idx, self._pods(sc.tops, sc.pod_groups, sc.packed), self._clocks(len(sc.tops), sc.now))
             rel = None
             if sc.releases is not None:
-                rel = self._releases(sc.releases, float(np.max(pods[2], initial=-np.inf)), sc.rounds or ())
-            args.append(Scenario(*pods, sc.lift, edits, adds, sc.rounds, rel)
-                        if sc.lift is not None or edits or adds or sc.rounds is not None or rel is not None else pods)
+                start = pods[2] if sc.arrive is None else pods[2][np.asarray(sc.arrive, dtype=np.int64) == 0]
+                rel = self._releases(sc.releases, float(np.max(start, initial=-np.inf)), sc.rounds or ())
+            if sc.arrive is not None:
+                args.append(Scenario(*pods, sc.lift, edits, adds, sc.rounds, rel, sc.arrive))
+            else:
+                args.append(Scenario(*pods, sc.lift, edits, adds, sc.rounds, rel)
+                            if sc.lift is not None or edits or adds or sc.rounds is not None or rel is not None else pods)
         res = fn(args, source=source, explain=True) if explain else fn(args, source=source)
         if perm and sorted(perm) != perm:
             n, back = len(self._names), np.asarray(perm, dtype=np.int64)
@@ -1057,6 +1077,70 @@ class NHDScheduler:
                                    self._scan_periods(scans, period), schedules=deps)
         return [(p, why) if reasons else p for p, why in result]
 
+    def ForecastArrivals(self, arrivals: Sequence[Sequence[Arrival]], scans: int, keys: Sequence = None,
+                         period: float = None, departures: Sequence[Dict] = None, additions: Sequence = None,
+                         reasons: bool = False) -> List:
+        """``ForecastDepartures`` with pods created between the scans: "we submit these 200 jobs at 10:05 and jobs A
+        and B end at 10:10: when does each one start, and on which node?  Do we also need one more node like this
+        one?".  ``arrivals``: one list of ``Arrival`` per scenario.  ``run()`` attempts a new pod as soon as its create
+        event arrives, at that moment's clock; a pod that fails there is pending and retried at every later scan, after
+        the older pending pods (``ServicePods`` is in creation order).  So the retry order is ``keys`` (default: the
+        pods the next ``CheckPendingPods`` would attempt), then the arrivals by ``(at, given order)``.  Each gap plays
+        its departures and its arrivals by clock, a departure before an arrival at the same offset; an arrival exactly
+        at a scan's offset is created right before that scan.  ``departures`` None or one dict per scenario, as
+        ``ForecastDepartures`` takes them; ``additions`` None or one addition list per scenario, as ``PlanExpansion``
+        takes them; ``scans`` and ``period`` as for ``ForecastPending``.
+        Returns one ``{(ns, name): (seconds after the first scan of the placing attempt, node name) or None}`` per
+        scenario, for the pending and the arriving pods (``reasons=True``: ``(placement, reasons)``, the reasons of the
+        pods no attempt placed, at the last scan).  An arrival whose config does not parse, or whose request is beyond
+        the packed limits, maps to None, as a pending pod does.  ValueErrors: an arrival key that names an existing pod
+        or repeats within a scenario, ``at`` <= 0 or after the last scan, list lengths that differ from
+        ``len(arrivals)``, and the departure checks of ``ForecastDepartures``.  All scenarios are planned in one GPU
+        call, one warp each (``Solver.plan_scenarios`` with ``arrive``).  Only reads happen, as ``ForecastPending``."""
+        arrivals = [list(a) for a in arrivals]
+        for what, v in (('departure dicts', departures), ('addition lists', additions)):
+            if v is not None and len(v) != len(arrivals):
+                raise ValueError(f'{len(v)} {what} for {len(arrivals)} arrival lists')
+        periods = self._scan_periods(scans, period)
+        last = float(sum(periods))
+        if keys is None:
+            keys = self._pending_keys()
+        existing = {(k[0], k[1]) for k in keys} | {(k[0], k[1]) for k in self._service_pods()} | \
+            {(ns, pod) for n in self.nodes.values() for (pod, ns) in n.pod_info}
+        for arr in arrivals:
+            seen = set()
+            for a in arr:
+                key = (a.key[0], a.key[1])
+                if key in existing:
+                    raise ValueError(f'arrival {key[0]}.{key[1]} names an existing pod')
+                if key in seen:
+                    raise ValueError(f'arrival {key[0]}.{key[1]} is given twice')
+                seen.add(key)
+                if not 0.0 < float(a.at) <= last:
+                    raise ValueError(f'arrival {key[0]}.{key[1]} at {a.at} s is not inside the {last} s of the scans')
+        deps = [self._departures({} if departures is None else d, keys) for d in (departures or [{}] * len(arrivals))]
+        result = self._grown_plans([[] for _ in arrivals] if additions is None else additions, keys, reasons, periods,
+                                   schedules=deps, arrivals=arrivals)
+        return [(p, why) if reasons else p for p, why in result]
+
+    def _arrival_entries(self, arrivals: Sequence[Arrival]) -> List[tuple]:
+        """``(entry, at)`` of each arrival in ``(at, given order)``: the pod read from its config as ``_prepare`` reads a
+        pending pod."""
+        out = []
+        for i, a in sorted(enumerate(arrivals), key=lambda x: (float(x[1].at), x[0])):
+            e = _Pending(i, (a.key[0], a.key[1]))
+            e.ready = True
+            e.tcfg = self.GetCfgParser(a.cfgtype, a.cfgstr)
+            e.top = e.tcfg.CfgToTopology(False)
+            if e.top is not None:
+                e.groups = list(a.groups)
+                try:
+                    e.rec = packing.pack_pod(e.top, e.groups, self.cluster.layout)
+                except packing.UnsupportedError as err:
+                    e.unsupported = str(err)
+            out.append((e, float(a.at)))
+        return out
+
     def _pending_keys(self) -> List:
         """The pods the next ``CheckPendingPods`` would attempt, in its order."""
         phase = self._service_pods()
@@ -1107,12 +1191,15 @@ class NHDScheduler:
         return [float(60 * 0.5 if period is None else period)] * (scans - 1)
 
     def _grown_plans(self, additions: Sequence[Sequence], keys: Sequence, reasons: bool, periods: Sequence[float],
-                     exclude: Sequence[str] = (), departures: Sequence = None, schedules: Sequence = None):
+                     exclude: Sequence[str] = (), departures: Sequence = None, schedules: Sequence = None,
+                     arrivals: Sequence = None):
         """``PlanExpansion``'s plans, with a later scan after each of ``periods`` seconds: per scenario ``(placement,
         reasons)``, a placed pod mapped to its node name, or with ``periods`` (even an empty list) to ``(scan, node
         name)``.  ``periods`` None: one scan, through the call without rounds.  ``exclude``: nodes in maintenance
         throughout, in every scenario.  ``departures`` (``_departures``' list): releases on the batch path, for one
-        scenario without additions; ``schedules``: one such list per scenario, planned on the scenario path."""
+        scenario without additions; ``schedules``: one such list per scenario, planned on the scenario path.
+        ``arrivals`` (with ``schedules``): one ``Arrival`` list per scenario, created between the scans; a placed pod
+        then maps to ``(seconds after the first scan, node name)``."""
         scens = [[(node, before) for node, before in sc] for sc in additions]
         for sc in scens:
             names = [node.name for node, _ in sc]
@@ -1127,7 +1214,12 @@ class NHDScheduler:
             keys = [k for k in phase if self._wanted(phase)(k)]
         entries = [e for e in self._read([(k[0], k[1]) for k in keys], {}) if e.solvable]
         result = [({(k[0], k[1]): None for k in keys}, {}) for _ in scens]
-        if self.nodes and entries:
+        arrived = None
+        if arrivals is not None:
+            arrived = [self._arrival_entries(a) for a in arrivals]
+            for (placement, _), arr in zip(result, arrivals):
+                placement.update({(a.key[0], a.key[1]): None for a in arr})
+        if self.nodes and (entries or (arrived and any(e.solvable for arr in arrived for e, _ in arr))):
             for sc in scens:                        # a candidate's new NIC speed: the sync below reloads the solver
                 self.cluster.pack_candidates([node for node, _ in sc])
             self._sync()
@@ -1153,7 +1245,15 @@ class NHDScheduler:
             releases = None if departures is None else release_clocks(departures)
             scheduled = None if schedules is None else [release_clocks(d) for d in schedules]
             todo = [(j, entries) for j in range(len(scens))]
-            if clocks is not None and scens == [[]] and schedules is None:
+            arrive_at = {}                          # per arriving entry: (round, clock, seconds after the first scan)
+            if arrived is not None:
+                for arr in arrived:
+                    for e, at in arr:
+                        k = next(k for k, o in enumerate(offs) if at <= o)
+                        clock = clocks[k] if at == offs[k] else max(now + at, clocks[k - 1] if k else now)
+                        arrive_at[id(e)] = (k + 1, min(clock, clocks[k]), at)
+                todo = [(j, entries + [e for e, _ in arrived[j] if e.solvable]) for j in range(len(scens))]
+            if clocks is not None and scens == [[]] and schedules is None and arrivals is None:
                 # one scenario on the cluster as it is: one batch per scan (a pod beyond the tuple limits is dropped
                 # and the rest planned again, as _plan_prepared does)
                 res, ok, _ = self._without_refused(
@@ -1172,11 +1272,18 @@ class NHDScheduler:
                             placement[(e.key[0], e.key[1])] = (int(r), self.cluster.name_of(int(b['node'])))
                     if reasons:
                         why.update(self._reasons(ok, res[0], res[2]))
+            def scenario(item):
+                es, arrive = item[1], None
+                if arrived is not None:
+                    arrive = [arrive_at[id(e)][0] if id(e) in arrive_at else 0 for e in es]
+                return ClusterScenario(exclude, [e.top for e in es], [e.groups for e in es],
+                                       now if arrive is None else [arrive_at[id(e)][1] if id(e) in arrive_at else now
+                                                                   for e in es],
+                                       [e.rec for e in es], rounds=clocks,
+                                       adds=[(before, node) for node, before in scens[item[0]]],
+                                       releases=None if scheduled is None else scheduled[item[0]], arrive=arrive)
             planned = self._plan_refused(
-                todo, lambda item: ClusterScenario(exclude, [e.top for e in item[1]], [e.groups for e in item[1]], now,
-                                                   [e.rec for e in item[1]], rounds=clocks,
-                                                   adds=[(before, node) for node, before in scens[item[0]]],
-                                                   releases=None if scheduled is None else scheduled[item[0]]),
+                todo, scenario,
                 lambda item, pod: (item[0], item[1][:pod] + item[1][pod + 1:]) if len(item[1]) > 1 else None, reasons,
                 lambda item, code, pod: f'nhd_plan_scenarios_grown refused scenario {item[0]}: code {code}, pod {pod}')
             n_nodes = len(self.nodes)
@@ -1189,7 +1296,13 @@ class NHDScheduler:
                         if int(b['status']) == wire.PLACED:
                             n = int(b['node'])
                             name = self.cluster.name_of(n) if n < n_nodes else added[n - n_nodes]
-                            placement[(e.key[0], e.key[1])] = name if clocks is None else (int(r[-1][k]), name)
+                            if arrived is not None:     # on its creation, or at a scan
+                                a = arrive_at.get(id(e))
+                                at = a[2] if a is not None and float(r[-1][k]) == a[1] and int(r[-2][k]) == a[0] \
+                                    else ([0.0] + offs)[int(r[-2][k])]
+                                placement[(e.key[0], e.key[1])] = (at, name)
+                            else:
+                                placement[(e.key[0], e.key[1])] = name if clocks is None else (int(r[-1][k]), name)
                     if reasons:
                         why.update(self._reasons(ok, out, r[3]))
         return result

@@ -1587,7 +1587,11 @@ extern "C" int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_
  * nodes, counts (int32, seeded from pods_used, after the pod rounds in d_sidx) and releases are compacted like the
  * rest, each release carrying its node's compacted count row; a scenario's slots grow by its distinct released nodes,
  * min(n_s * (1 + R_s) + D_s, n_nodes).  release_check_kernel first checks the call's releases and tracked counts
- * against the source records, one word read back.
+ * against the source records, one word read back.  With arrivals (nhd_plan_scenarios_arrivals,
+ * scenario_plan_kernel<., true, true, true>, the releases' layout even without releases) each timeline is expanded
+ * into the kernel's rounds, each over its own pod range (round 0, one round per arrival at its clock, one per scan
+ * over the pods arrived so far), each release attached to the round it precedes; pod_round is mapped back to the
+ * call's rounds, and pod_clock is the clock of each pod's last kernel round.
  */
 /*
  * why_counts of the scenario call just run on w (its bindings b, its pods and clocks run_pods / run_now, its correction
@@ -1648,7 +1652,8 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
                               const int32_t* round_start, const double* round_clock, const int32_t* track_start,
                               const int32_t* tracked, const int16_t* pods_used, const int32_t* rel_start,
                               const nhd_release* releases, nhd_binding* out, int32_t* scenario_status,
-                              int32_t* scenario_pod, uint32_t* why_counts, int32_t* pod_round)
+                              int32_t* scenario_pod, uint32_t* why_counts, int32_t* pod_round,
+                              const int32_t* arrive_round = nullptr, double* pod_clock = nullptr)
 {
     if (!h || n_scenarios < 0 || !excl_start || !pod_start || (n_scenarios > 0 && (!scenario_status || !scenario_pod)))
         return NHD_ERR_INVALID;
@@ -1677,10 +1682,31 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
                 return fail(h, NHD_ERR_INVALID, "scenario %d: round clocks go down at %d", s, r);
             if (r == round_start[s])                     /* a monotonic clock never goes back */
                 for (int i = pod_start[s]; i < pod_start[s + 1]; i++)
-                    if (round_clock[r] < now[i])
+                    if ((!arrive_round || arrive_round[i] == 0) && round_clock[r] < now[i])
                         return fail(h, NHD_ERR_INVALID, "scenario %d: round clock %d is earlier than the clock of pod %d",
                                     s, r, i - pod_start[s]);
         }
+    /* arrivals (nhd_plan_scenarios_arrivals): rounds in [0, R_s] never going down in pod order, and each arrival's
+     * clock inside its gap, not before the arrival before it in that gap */
+    for (int s = 0; s < n_scenarios && arrive_round; s++) {
+        const int R_s = round_start ? round_start[s + 1] - round_start[s] : 0;
+        const double* clk = round_start ? round_clock + round_start[s] : nullptr;
+        double t0 = -INFINITY;                                         /* the latest clock of the round-0 pods */
+        for (int i = pod_start[s]; i < pod_start[s + 1]; i++) {
+            const int g = arrive_round[i], k = i - pod_start[s];
+            if (g != 0 && R_s == 0) return fail(h, NHD_ERR_INVALID, "scenario %d: pod %d arrives without rounds", s, k);
+            if (g < 0 || g > R_s)
+                return fail(h, NHD_ERR_INVALID, "scenario %d: pod %d: arrival round %d outside [0, %d]", s, k, g, R_s);
+            if (i > pod_start[s] && g < arrive_round[i - 1])
+                return fail(h, NHD_ERR_INVALID, "scenario %d: arrival rounds go down at pod %d", s, k);
+            if (g == 0) { t0 = std::max(t0, now[i]); continue; }
+            if (i > pod_start[s] && g == arrive_round[i - 1] && now[i] < now[i - 1])
+                return fail(h, NHD_ERR_INVALID, "scenario %d: arrival clocks go down at pod %d", s, k);
+            if (now[i] < (g > 1 ? clk[g - 2] : t0) || now[i] > clk[g - 1])
+                return fail(h, NHD_ERR_INVALID, "scenario %d: pod %d: arrival clock outside the gap before round %d", s,
+                            k, g);
+        }
+    }
     if (pod_round && !round_start && n_pods > 0) memset(pod_round, 0, (size_t)n_pods * 4);
     const uint8_t* records = nullptr;
     int32_t rc = source_records(h, source, "plan", &records);
@@ -1706,6 +1732,13 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         if (lift_at[s] < 0 || lift_at[s] > pod_start[s + 1] - pod_start[s])
             return fail(h, NHD_ERR_INVALID, "scenario %d: lift index %d outside [0, %d]", s, lift_at[s],
                         pod_start[s + 1] - pod_start[s]);
+    for (int s = 0; s < n_scenarios && lift_at && arrive_round; s++) {    /* lifted after round 0, or held throughout */
+        int n0 = 0;
+        while (pod_start[s] + n0 < pod_start[s + 1] && arrive_round[pod_start[s] + n0] == 0) n0++;
+        if (lift_at[s] > n0 && lift_at[s] != pod_start[s + 1] - pod_start[s])
+            return fail(h, NHD_ERR_INVALID, "scenario %d: lift index %d neither at most the %d pods of round 0 nor %d",
+                        s, lift_at[s], n0, pod_start[s + 1] - pod_start[s]);
+    }
     for (int s = 0; s < n_scenarios && n_add > 0; s++)
         for (int e = add_start[s]; e < add_start[s + 1]; e++) {
             if (add_at[e] < 0 || add_at[e] > h->n_nodes)
@@ -1723,7 +1756,8 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         }
     /* releases (nhd_plan_scenarios_releases): per release its node's call-wide tracked row, per scenario its distinct
      * released nodes (the slot bound grows by them) */
-    const bool with_releases = track_start || rel_start;
+    const bool arrivals = arrive_round != nullptr;                     /* always with the releases' layout */
+    const bool with_releases = track_start || rel_start || arrivals;
     std::vector<int32_t> rel_row((size_t)n_rel), rel_nodes(with_releases ? n_scenarios : 0, 0);
     for (int s = 0; s < n_scenarios && with_releases; s++) {
         const int t0 = track_start ? track_start[s] : 0, t1 = track_start ? track_start[s + 1] : 0;
@@ -1742,7 +1776,8 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         const double* clk = round_start ? round_clock + round_start[s] : nullptr;
         if (l1 > l0 && R_s == 0) return fail(h, NHD_ERR_INVALID, "scenario %d: releases without rounds", s);
         double t_first = -INFINITY;
-        for (int i = pod_start[s]; i < pod_start[s + 1]; i++) t_first = std::max(t_first, now[i]);
+        for (int i = pod_start[s]; i < pod_start[s + 1]; i++)
+            if (!arrive_round || arrive_round[i] == 0) t_first = std::max(t_first, now[i]);
         std::vector<int32_t> seen;
         for (int k = l0; k < l1; k++) {
             const nhd_release& rl = releases[k];
@@ -1802,6 +1837,9 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     std::vector<nhd_node_rec> ed_rec, ad_rec;
     std::vector<nhd_release> rl_rec;
     std::vector<double> rd_clock;
+    /* with arrivals: per kernel round (n_rounds + 1 per accepted scenario) its pods [q0, q1) and the round r of the
+     * call it belongs to; per release the kernel round it precedes */
+    std::vector<int32_t> rd_pods, rd_ext, rel_iround(arrivals ? n_rel : 0);
     if (with_releases) { tr_off.push_back(0); rl_off.push_back(0); }
     size_t n_slots = 0;
     for (int s = 0; s < n_scenarios; s++) {
@@ -1834,7 +1872,38 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
         int64_t touches = n_s;                 /* without rounds: one slot per pod, as scenario_plan_kernel<., false> */
         if (rounds) {
             const int64_t R_s = round_start ? round_start[s + 1] - round_start[s] : 0;
-            if (round_start) rd_clock.insert(rd_clock.end(), round_clock + round_start[s], round_clock + round_start[s + 1]);
+            if (arrivals) {
+                /* the timeline as the kernel's rounds: round 0 over the pods pending at the start; then per gap g, in
+                 * clock order, each arrival alone at its own clock (the gap's releases at or before that clock go
+                 * first), and the scan over the pods arrived so far, after the gap's remaining releases */
+                const int c0 = pod_off[pod_off.size() - 2], p0 = pod_start[s], p1 = pod_start[s + 1];
+                const int l0 = rel_start ? rel_start[s] : 0, l1 = rel_start ? rel_start[s + 1] : 0;
+                const int32_t e0 = (int32_t)rd_ext.size();                /* this scenario's round 0 */
+                int i = p0;
+                while (i < p1 && arrive_round[i] == 0) i++;
+                rd_pods.insert(rd_pods.end(), {c0, c0 + i - p0});
+                rd_ext.push_back(0);
+                for (int g = 1; g <= R_s; g++) {
+                    int k = l0;
+                    for (; i < p1 && arrive_round[i] == g; i++) {
+                        for (; k < l1; k++)
+                            if (releases[k].round == g) {
+                                if (releases[k].clock > now[i]) break;
+                                rel_iround[k] = (int32_t)rd_ext.size() - e0;
+                            }
+                        rd_clock.push_back(now[i]);
+                        rd_pods.insert(rd_pods.end(), {c0 + i - p0, c0 + i - p0 + 1});
+                        rd_ext.push_back(g);
+                    }
+                    for (; k < l1; k++)
+                        if (releases[k].round == g) rel_iround[k] = (int32_t)rd_ext.size() - e0;
+                    rd_clock.push_back(round_clock[round_start[s] + g - 1]);
+                    rd_pods.insert(rd_pods.end(), {c0, c0 + i - p0});
+                    rd_ext.push_back(g);
+                }
+            } else if (round_start) {
+                rd_clock.insert(rd_clock.end(), round_clock + round_start[s], round_clock + round_start[s + 1]);
+            }
             rd_off.push_back((int32_t)rd_clock.size());
             sl_start.push_back((int32_t)n_slots);
             touches = std::min(n_s * (1 + R_s) + (with_releases ? rel_nodes[s] : 0), (int64_t)h->n_nodes);
@@ -1849,6 +1918,7 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
             tr_off.push_back((int32_t)tr_node.size());
             for (int k = rel_start ? rel_start[s] : 0; k < (rel_start ? rel_start[s + 1] : 0); k++) {
                 rl_rec.push_back(releases[k]);
+                if (arrivals) rl_rec.back().round = rel_iround[k];      /* the kernel's round it precedes */
                 rl_row.push_back(row0 + rel_row[k]);
             }
             rl_off.push_back((int32_t)rl_rec.size());
@@ -1877,9 +1947,9 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     std::vector<int32_t> idx;
     idx.reserve(pod_off.size() + ex_off.size() + ex.size() + ed_off.size() + ed_node.size() + lift.size() +
                 ad_off.size() + ad_at.size() + rd_off.size() + sl_start.size() + tr_off.size() + tr_node.size() +
-                rl_off.size() + rl_row.size());
+                rl_off.size() + rl_row.size() + rd_pods.size());
     for (const auto* v : {&pod_off, &ex_off, &ex, &ed_off, &ed_node, &lift, &ad_off, &ad_at, &rd_off, &sl_start, &tr_off,
-                          &tr_node, &rl_off, &rl_row})
+                          &tr_node, &rl_off, &rl_row, &rd_pods})
         idx.insert(idx.end(), v->begin(), v->end());
     const size_t off_ex_off = pod_off.size(), off_ex = off_ex_off + ex_off.size(), off_ed_off = off_ex + ex.size();
     const size_t off_ed_node = off_ed_off + ed_off.size(), off_lift = off_ed_node + ed_node.size();
@@ -1887,6 +1957,7 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     const size_t off_rd_off = off_ad_at + ad_at.size(), off_sl = off_rd_off + rd_off.size();
     const size_t off_tr_off = off_sl + sl_start.size(), off_tr_node = off_tr_off + tr_off.size();
     const size_t off_rl_off = off_tr_node + tr_node.size(), off_rl_row = off_rl_off + rl_off.size();
+    const size_t off_rd_pods = off_rl_row + rl_row.size();
     const size_t off_nodes = idx.size(), off_bad = off_nodes + n_slots, off_round = off_bad + 1;
     const size_t off_count = off_round + (rounds ? n_run : 0);     /* with releases: the tracked counts */
     /* d_swork: the working slots, then the edit records and the added records the kernel seeds them from, then (with
@@ -1938,12 +2009,16 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     sa.pod_round = h->d_sidx + off_round;
     sa.track_start = h->d_sidx + off_tr_off; sa.tracked = h->d_sidx + off_tr_node; sa.count = h->d_sidx + off_count;
     sa.rel_start = h->d_sidx + off_rl_off; sa.rel = h->d_rels; sa.rel_track = h->d_sidx + off_rl_row;
+    sa.round_pods = h->d_sidx + off_rd_pods;
+    if (arrivals)           /* not NHD_PLACED until attempted: an arrival's first round walks it, releases see it */
+        CK(cudaMemsetAsync(w.out, 0xFF, (size_t)n_run * sizeof(nhd_binding), h->stream));
     const int warps_per_cta = SCENARIO_THREADS / 32;
     const int grid = std::min((n_acc + warps_per_cta - 1) / warps_per_cta, h->sm_count * 16);
     /* through a pointer: the CPU emulation (tests/emu) rewrites a launch into a macro call, whose argument list would
      * split a kernel name with two template arguments */
     void (*const kernel)(ScenarioArgs) =
-        with_releases ? (why_counts ? scenario_plan_kernel<true, true, true> : scenario_plan_kernel<false, true, true>)
+        arrivals      ? (why_counts ? scenario_plan_kernel<true, true, true, true> : scenario_plan_kernel<false, true, true, true>)
+        : with_releases ? (why_counts ? scenario_plan_kernel<true, true, true> : scenario_plan_kernel<false, true, true>)
         : rounds      ? (why_counts ? scenario_plan_kernel<true, true> : scenario_plan_kernel<false, true>)
                       : (why_counts ? scenario_plan_kernel<true, false> : scenario_plan_kernel<false, false>);
     kernel<<<grid, SCENARIO_THREADS, 0, h->stream>>>(sa);
@@ -1960,15 +2035,17 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
     if ((rc = fetch_bindings(h, w, n_run, compact ? run.data() : out)) != NHD_OK) return rc;
     if (bad) return fail(h, NHD_ERR_STATE, "%s: %u chosen nodes without a mapping", what, bad);
     std::vector<uint32_t> run_rows;
+    const double* run_now = compact ? cnow.data() : now;
+    std::vector<double> last_now;
+    if (rounds && (why_counts || pod_clock)) {  /* the clock of each pod's last attempt (its kernel round's) */
+        last_now.resize(n_run);
+        for (int k = 0; k < n_acc; k++)
+            for (int i = pod_off[k]; i < pod_off[k + 1]; i++)
+                last_now[i] = run_round[i] == 0 ? run_now[i] : rd_clock[rd_off[k] + run_round[i] - 1];
+    }
     if (why_counts) {
         if (compact) run_rows.resize((size_t)n_run * NHD_WHY_COUNT);
-        const double* run_now = compact ? cnow.data() : now;
-        std::vector<double> last_now;
         if (rounds) {            /* the base pass evaluates each pod at the clock of its last attempt */
-            last_now.resize(n_run);
-            for (int k = 0; k < n_acc; k++)
-                for (int i = pod_off[k]; i < pod_off[k + 1]; i++)
-                    last_now[i] = run_round[i] == 0 ? run_now[i] : rd_clock[rd_off[k] + run_round[i] - 1];
             CK(cudaMemcpyAsync(d_last_now, last_now.data(), (size_t)n_run * 8, cudaMemcpyHostToDevice, h->stream));
             run_now = last_now.data();
         }
@@ -1977,7 +2054,14 @@ static int32_t plan_scenarios(nhd_handle* h, const char* what, int32_t source, i
                                    compact ? run_rows.data() : why_counts, what)) != NHD_OK)
             return rc;
     }
+    if (arrivals)                /* kernel rounds -> the call's rounds: an arrival or a scan of gap g reads g */
+        for (int k = 0; k < n_acc; k++)
+            for (int i = pod_off[k]; i < pod_off[k + 1]; i++) run_round[i] = rd_ext[rd_off[k] + k + run_round[i]];
     if (rounds && !compact && pod_round) memcpy(pod_round, run_round.data(), (size_t)n_run * 4);
+    if (pod_clock)
+        for (int k = 0; k < n_acc; k++)
+            for (int i = pod_off[k]; i < pod_off[k + 1]; i++)
+                pod_clock[pod_start[acc[k]] + i - pod_off[k]] = rounds ? last_now[i] : run_now[i];
     if (compact)
         for (int k = 0; k < n_acc; k++) {
             const size_t n_k = (size_t)(pod_off[k + 1] - pod_off[k]);
@@ -2078,6 +2162,25 @@ extern "C" int32_t nhd_plan_scenarios_releases(nhd_handle* h, int32_t source, in
                           edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now,
                           round_start, round_clock, track_start, tracked, pods_used, rel_start, releases, out,
                           scenario_status, scenario_pod, why_counts, pod_round);
+}
+
+extern "C" int32_t nhd_plan_scenarios_arrivals(nhd_handle* h, int32_t source, int32_t n_scenarios,
+                                               const int32_t* excl_start, const int32_t* excluded, const int32_t* lift_at,
+                                               const int32_t* edit_start, const int32_t* edit_node,
+                                               const nhd_node_rec* edit_rec, const int32_t* add_start,
+                                               const int32_t* add_at, const nhd_node_rec* add_rec,
+                                               const int32_t* pod_start, const nhd_pod* pods, const double* now,
+                                               const int32_t* round_start, const double* round_clock,
+                                               const int32_t* track_start, const int32_t* tracked,
+                                               const int16_t* pods_used, const int32_t* rel_start,
+                                               const nhd_release* releases, const int32_t* arrive_round,
+                                               nhd_binding* out, int32_t* scenario_status, int32_t* scenario_pod,
+                                               uint32_t* why_counts, int32_t* pod_round, double* pod_clock)
+{
+    return plan_scenarios(h, "nhd_plan_scenarios_arrivals", source, n_scenarios, excl_start, excluded, lift_at,
+                          edit_start, edit_node, edit_rec, add_start, add_at, add_rec, pod_start, pods, now,
+                          round_start, round_clock, track_start, tracked, pods_used, rel_start, releases, out,
+                          scenario_status, scenario_pod, why_counts, pod_round, arrive_round, pod_clock);
 }
 
 /* debug: 16 cycle accumulators + 16 counters of the last sweep (only filled by NHD_PROFILE builds) */

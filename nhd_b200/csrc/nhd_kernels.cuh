@@ -3044,6 +3044,8 @@ struct ScenarioArgs {
     const int32_t* rel_start;      /* [n_scenarios + 1] into rel / rel_track */
     const nhd_release* rel;        /* each scenario's releases, in array order */
     const int32_t* rel_track;      /* [release]: its node's row of count */
+    /* scenario_plan_kernel<., true, true, true> only (nhd_plan_scenarios_arrivals) */
+    const int32_t* round_pods;     /* [round_start[s] + s + r][2]: the pods [q0, q1) that round r of scenario s walks */
 };
 
 constexpr int SCENARIO_THREADS = 128;
@@ -3171,8 +3173,16 @@ __device__ __noinline__ int scenario_releases(const ScenarioArgs& a, int r, int 
  * n_edits + n_adds + min(n_pods * (1 + rounds) + distinct released nodes, n_nodes).  After a placement on a tracked
  * node lane 0 raises the node's count of every claimed NIC and clears the bit where the count is still <= 0
  * (ClaimPodNICResources, Node.py:644-646).  The warp commits one pod at a time, so this is the reference's counter
- * rule exactly: two pods can share a NIC a release drove to -1 without any cut. */
-template <bool WHY, bool ROUNDS, bool RELEASES = false>
+ * rule exactly: two pods can share a NIC a release drove to -1 without any cut.
+ * ARRIVALS (nhd_plan_scenarios_arrivals, always with ROUNDS and RELEASES): round r walks the pods
+ * round_pods[r0 + s + r] instead of the whole scenario.  The host expands each scenario's timeline into these rounds:
+ * round 0 over the pods pending at plan start, an arrival as a round over that pod alone at its own clock, a scan as a
+ * round over the pods arrived so far at the scan's clock, each release on the round it precedes.  The host seeds the
+ * bindings of the pods not yet attempted with a status other than NHD_PLACED, so that the placed-pod skip lets an
+ * arrival's first attempt through and scenario_releases plays a gap's releases while a pod has not arrived yet.  Each
+ * pod is still attempted at most 1 + R_s times (its arrival, then at most every scan from its gap on), so the slot
+ * bound stays n_edits + n_adds + min(n_pods * (1 + R_s) + distinct released nodes, n_nodes). */
+template <bool WHY, bool ROUNDS, bool RELEASES = false, bool ARRIVALS = false>
 __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const __grid_constant__ ScenarioArgs a)
 {
     const int lane = threadIdx.x & 31, W = a.words;
@@ -3207,7 +3217,12 @@ __global__ void __launch_bounds__(SCENARIO_THREADS) scenario_plan_kernel(const _
                 if (r > 0 && a.rel_start[s + 1] > a.rel_start[s])
                     n_touched = scenario_releases(a, r, p0, p1, a.rel_start[s], a.rel_start[s + 1], work, work_node, n_touched);
             }
-            for (int i = p0; i < p1; i++) {
+            int q0 = p0, q1 = p1;
+            if constexpr (ARRIVALS) {
+                q0 = a.round_pods[2 * (r0 + s + r)];
+                q1 = a.round_pods[2 * (r0 + s + r) + 1];
+            }
+            for (int i = q0; i < q1; i++) {
                 if constexpr (ROUNDS) {                                    /* lane 0 wrote the pod's last binding */
                     if (r > 0 && __shfl_sync(0xFFFFFFFFu, lane == 0 ? a.out[i].status : 0, 0) == NHD_PLACED) continue;
                 }

@@ -73,7 +73,10 @@ class Scenario(NamedTuple):
     never going down and none before the scenario's pod clocks; at each, the scenario's pods not placed yet are solved
     again in order on the records the previous scan left, and the bindings hold each pod's last attempt.  ``releases``
     (None: none): ``(tracked, pods_used, releases)`` as ``plan_batch_releases`` takes them, node indices of source
-    nodes the scenario does not edit, each release applied before its ``round`` (1 .. ``len(rounds)``)."""
+    nodes the scenario does not edit, each release applied before its ``round`` (1 .. ``len(rounds)``).  ``arrive``
+    (None: every pod pending at the start): per pod the round ``r`` in the gap before which it is created, at its own
+    clock, and first attempted then (0: pending at the start); the round-0 pods come first and ``(arrive, now)`` never
+    goes down in pod order."""
     exclude: Sequence[int]
     pods: np.ndarray
     now: Sequence[float]
@@ -82,6 +85,7 @@ class Scenario(NamedTuple):
     adds: Optional[tuple] = None
     rounds: Optional[Sequence[float]] = None
     releases: Optional[tuple] = None
+    arrive: Optional[Sequence[int]] = None
 
 
 class Solver:
@@ -304,16 +308,20 @@ class Solver:
         scenario has ``rounds``, each result gains a last element: the ``(n_s,)`` int32 round that placed each pod, or
         ``len(rounds)`` if none did (None when refused).  When any scenario has ``releases`` the call is
         ``nhd_plan_scenarios_releases``: that scenario's deployed pods end between its rounds, each scenario on its own
-        records and NIC counters."""
+        records and NIC counters.  When any scenario has ``arrive`` the call is ``nhd_plan_scenarios_arrivals``: each
+        later pod is first attempted alone at its clock, merged with its gap's releases, and retried at every scan from
+        then on; each accepted result then also gains a last element, the ``(n_s,)`` float64 clock of the attempt whose
+        binding it holds."""
         src = _source(source)
         # (thousands of small scenarios: gathered as bytes, since numpy's per-array checks of the structured pod dtype
         # would cost more than the call itself)
         exs, podb, nowl, lifts, ednodes, edrecs, n_adds, adats, adrecs, rounds = [], [], [], [], [], [], [], [], [], []
-        rels = []
+        rels, arrs = [], []
         for sc in scenarios:
             sc = Scenario(*sc)
             rounds.append(sc.rounds)
             rels.append(sc.releases)
+            arrs.append(sc.arrive)
             pods = np.asarray(sc.pods)
             if pods.dtype != wire.POD_DTYPE:
                 pods = pods.astype(wire.POD_DTYPE)
@@ -379,7 +387,12 @@ class Solver:
         tail = [out.ctypes.data if some else None, status.ctypes.data, which.ctypes.data,
                 counts.ctypes.data if explain and some else None,
                 pod_round.ctypes.data if pod_round is not None and some else None]
-        if any(r is not None for r in rels):
+        arrivals = any(a is not None for a in arrs)
+        pod_clock = np.zeros(len(pods), dtype='<f8') if arrivals else None
+        if arrivals and pod_round is None:
+            pod_round = np.zeros(len(pods), dtype='<i4')
+            tail[-1] = pod_round.ctypes.data if some else None
+        if any(r is not None for r in rels) or arrivals:
             # NULL release arrays unless some scenario has that field: existing calls go out as before
             trs, useds, rls = [], [], []
             for r in rels:
@@ -395,16 +408,28 @@ class Solver:
             tracked = np.ascontiguousarray(np.concatenate(trs), dtype='<i4')
             used = np.ascontiguousarray(np.concatenate(useds), dtype='<i2')
             rel = np.ascontiguousarray(np.concatenate(rls), dtype=wire.RELEASE_DTYPE)
-            self._ck(self._L.nhd_plan_scenarios_releases(
-                *args, track_start.ctypes.data, tracked.ctypes.data if len(tracked) else None,
-                used.ctypes.data if len(tracked) else None, rel_start.ctypes.data, rel.ctypes.data if len(rel) else None,
-                *tail))
+            rel_args = (track_start.ctypes.data, tracked.ctypes.data if len(tracked) else None,
+                        used.ctypes.data if len(tracked) else None, rel_start.ctypes.data,
+                        rel.ctypes.data if len(rel) else None)
+            if arrivals:
+                arrive = np.ascontiguousarray(np.concatenate(
+                    [np.zeros(len(t), dtype='<i4') if a is None else np.asarray(a, dtype='<i4').reshape(-1)
+                     for a, t in zip(arrs, nowl)]) if n else np.zeros(0), dtype='<i4')
+                assert len(arrive) == len(pods)
+                self._ck(self._L.nhd_plan_scenarios_arrivals(
+                    *args, *rel_args, arrive.ctypes.data if some else None, *tail,
+                    pod_clock.ctypes.data if some else None))
+            else:
+                self._ck(self._L.nhd_plan_scenarios_releases(*args, *rel_args, *tail))
         else:
             self._ck(self._L.nhd_plan_scenarios_rounds(*args, *tail))
         res = self._scenario_results(status, which, pod_start, out, counts)
         if pod_round is None:
             return res
-        return [r + (pod_round[a:b] if r[0] == 0 else None,)
+        if pod_clock is None:
+            return [r + (pod_round[a:b] if r[0] == 0 else None,)
+                    for r, a, b in zip(res, pod_start[:-1].tolist(), pod_start[1:].tolist())]
+        return [r + ((pod_round[a:b], pod_clock[a:b]) if r[0] == 0 else (None, None))
                 for r, a, b in zip(res, pod_start[:-1].tolist(), pod_start[1:].tolist())]
 
     @staticmethod
