@@ -539,6 +539,46 @@ int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_t n_exclude
                                 nhd_binding* out, uint32_t* why_counts, int32_t* pod_round);
 
 /*
+ * nhd_plan_batch_releases with pods created between the scans, on the batch path: "we submit these 4 000 jobs at 10:05
+ * and jobs A and B end at 10:10: when does each one start, and on which node?", one timeline of many pods.  Every
+ * argument of nhd_plan_batch_releases keeps its meaning; pod i also has
+ *   arrive_round[i]  0: pending at plan start; r in [1, n_rounds]: created in the gap before round r, at clock now[i].
+ *                    The round-0 pods come first, and (arrive_round, now) never goes down in pod order.
+ * Round 0 solves the round-0 pods as nhd_plan_batch_releases does.  Each gap r >= 1 then plays, merged by clock, the
+ * releases of round r and the first attempt of each pod arriving in it, at its now[] (the reference attempts a new pod
+ * on its create event); a release goes before an arrival at the same clock, and arrivals keep pod order.  Round r's
+ * scan then retries, in pod order at round_clock[r-1], every arrived pod not placed yet, the gap's failed arrivals after
+ * the older pods.  A gap's releases are played while a pod is unplaced or has not arrived yet.  The excluded nodes stay
+ * in maintenance throughout.
+ *   out            the binding of each pod's placing attempt, or else of its last one;
+ *   pod_round      (may be NULL) the round r whose arrival or scan placed the pod, or n_rounds if none did;
+ *   pod_clock      (may be NULL) the clock of the attempt whose binding is in out: now[i] or a round's clock;
+ *   why_counts     (may be NULL) the row at the start of the pod's last attempt, always a scan, as for
+ *                  nhd_plan_batch_releases.
+ * Identities: with arrive_round NULL the call is nhd_plan_batch_releases byte for byte on out, pod_round and
+ * why_counts, pod_clock then now[i] or the clock of the round that made the pod's last attempt.  The call gives the
+ * out, pod_round, pod_clock and why_counts of nhd_plan_scenarios_arrivals called with this one timeline as one scenario,
+ * its exclusions held throughout (lift_at = n_pods), no edits and no additions; the one difference is the tuple-limit
+ * judgement, as between nhd_plan_scenarios and nhd_plan_batch.
+ * Each run of a gap's arrivals between two of its releases is solved as one batch at per-pod clocks, with its commit,
+ * and cut where a claim meets a negative NIC count exactly as a round is; arrivals add no negative count, so the bound
+ * on cuts of nhd_plan_batch_releases holds.
+ * Refused as nhd_plan_batch_releases refuses, and, before anything is placed, NHD_ERR_INVALID for an arrive_round
+ * outside [0, n_rounds] or going down in pod order, an arrival with n_rounds == 0, arrival clocks going down among the
+ * arrivals of one gap, and an arrival clock before the clock of the round before its gap (for gap 1: before a now[] of a
+ * round-0 pod) or after its own round's clock.  The rule that no round clock is earlier than a now[] reads the round-0
+ * pods only, as does the lower bound of a round-1 release's clock.  Tuple limits are judged as by nhd_plan_batch.
+ * Nothing is written that a caller can observe (the list of nhd_plan_batch), no collective is entered, and the call
+ * waits for the device before returning.
+ */
+int32_t nhd_plan_batch_arrivals(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                                int32_t n_pods, const nhd_pod* pods, const double* now,
+                                int32_t n_rounds, const double* round_clock,
+                                int32_t n_tracked, const int32_t* tracked, const int16_t* pods_used,
+                                int32_t n_releases, const nhd_release* releases, const int32_t* arrive_round,
+                                nhd_binding* out, uint32_t* why_counts, int32_t* pod_round, double* pod_clock);
+
+/*
  * nhd_plan_scenarios_rounds with running pods finishing between the scans, per scenario: "jobs A and B end in about 20
  * minutes: does the queue clear then, or do I also need one more node like this one?", and several departure schedules
  * side by side.  Every argument of nhd_plan_scenarios_rounds keeps its meaning; scenario s also has

@@ -297,7 +297,7 @@ class DeviceCluster:
 
     def forecast(self, tops: Sequence, pod_groups: Sequence[Iterable[str]], now, round_clocks: Sequence[float],
                  source: str = 'mirror', exclude: Iterable[str] = (), explain: bool = False, packed: Sequence = None,
-                 releases: Sequence = None):
+                 releases: Sequence = None, arrive: Sequence[int] = None):
         """``plan`` over several pending scans (``Solver.plan_batch_rounds``): after the dry run at ``now``, at each
         clock of ``round_clocks`` the pods no earlier scan placed are retried in order on the cluster the earlier scans
         left, the nodes named in ``exclude`` in maintenance throughout.  Returns ``(bindings, pod_round)``: each pod's
@@ -309,13 +309,25 @@ class DeviceCluster:
         busy from ``clock``) right before the first scan whose clock is not earlier than ``clock``; one after the last
         scan changes nothing and is left out, one at or before ``now`` is a ValueError.  The nodes' signed NIC pod
         counters are those of the synced ``Node`` objects; every node with a release or a negative counter is tracked.
-        None when the solver in use cannot (a stand-in without ``plan_batch_releases``)."""
-        fn = getattr(self._solver, 'plan_batch_rounds' if releases is None else 'plan_batch_releases', None)
+        None when the solver in use cannot (a stand-in without ``plan_batch_releases``).
+        ``arrive`` (``Solver.plan_batch_arrivals``): per pod 0 when pending at ``now``, else the round in whose gap it is
+        created, at its own clock in ``now``; the nodes with a negative counter are tracked even without ``releases``,
+        and a release's round is judged from the clocks of the round-0 pods.  Returns ``(bindings, pod_round,
+        pod_clock)`` (``explain=True``: and the counts).  None when the solver in use cannot (a stand-in without
+        ``plan_batch_arrivals``)."""
+        fn = getattr(self._solver, 'plan_batch_rounds' if releases is None and arrive is None else
+                     'plan_batch_releases' if arrive is None else 'plan_batch_arrivals', None)
         if fn is None:
             return None
         idx = self._indices(exclude, 'exclude')
+        clocks = self._clocks(len(tops), now)
+        if arrive is not None:
+            start = clocks[np.asarray(arrive, dtype=np.int64) == 0]
+            rel = self._releases(releases or (), float(np.max(start, initial=-np.inf)), round_clocks)
+            return fn(self._pods(tops, pod_groups, packed), clocks, round_clocks, *rel, arrive, source=source,
+                      exclude=idx, explain=explain)
         rel = () if releases is None else self._releases(releases, float(np.max(now)), round_clocks)
-        return fn(self._pods(tops, pod_groups, packed), self._clocks(len(tops), now), round_clocks, *rel, source=source,
+        return fn(self._pods(tops, pod_groups, packed), clocks, round_clocks, *rel, source=source,
                   exclude=idx, explain=explain)
 
     def _releases(self, releases: Sequence, now: float, round_clocks: Sequence[float]):
@@ -1015,7 +1027,7 @@ class NHDScheduler:
         return result if reasons else [p for p, _ in result]
 
     def ForecastPending(self, scans: int, keys: Sequence = None, period: float = None, additions: Sequence = None,
-                        reasons: bool = False, departures: Dict = None):
+                        reasons: bool = False, departures: Dict = None, arrivals: Sequence = None):
         """Which pending pods get in at a later scan, and which never do?  ``run()`` retries every pod still pending
         each ``idle_thresh x block_secs`` seconds, and a GPU node that took a pod less than ``MIN_BUSY_SECS`` earlier
         takes no GPU pod, so one scan places at most one GPU pod per node.  This plans ``scans`` pending scans in a row
@@ -1038,16 +1050,28 @@ class NHDScheduler:
         the delete leaves it, and one after the last scan changes nothing.  A pod never annotated (its delete re-scans
         every node), a departure that is also among ``keys``, an offset <= 0, and ``departures`` together with
         ``additions`` are ValueErrors.  Departures here run on the batch path (``Solver.plan_batch_releases``);
-        ``ForecastDepartures`` plans several departure schedules, with or without added nodes, in one call."""
-        rel = None
-        if departures is not None:
+        ``ForecastDepartures`` plans several departure schedules, with or without added nodes, in one call.
+        ``arrivals``: a list of ``Arrival``, pods created between the scans, on the cluster as it is: one timeline of
+        many pods, solved on the batch path (``Solver.plan_batch_arrivals``).  Retry order, clock mapping, argument
+        checks and the placement ``(seconds after the first scan of the placing attempt, node name)`` are those of
+        ``ForecastArrivals``, and ``ForecastPending(n, keys, period, reasons=r, departures=d, arrivals=a)`` is
+        ``ForecastArrivals([a], n, keys, period, departures=[d], reasons=r)[0]``; ``arrivals`` together with
+        ``additions`` is a ValueError.  ``ForecastArrivals`` plans several timelines, or added nodes, one warp each."""
+        rel = arrived = None
+        if arrivals is not None and additions is not None:
+            raise ValueError('arrivals are planned on the batch path on the cluster as it is, not with additions')
+        periods = self._scan_periods(scans, period)
+        if departures is not None or arrivals is not None:
             if additions is not None:
                 raise ValueError('departures are planned on the cluster as it is, not with additions')
             if keys is None:
                 keys = self._pending_keys()
-            rel = self._departures(departures, keys)
-        result = self._grown_plans([[]] if additions is None else additions, keys, reasons,
-                                   self._scan_periods(scans, period), departures=rel)
+            if arrivals is not None:
+                arrived = [list(arrivals)]
+                self._check_arrivals(arrived, keys, float(sum(periods)))
+            rel = self._departures({} if departures is None else departures, keys)
+        result = self._grown_plans([[]] if additions is None else additions, keys, reasons, periods, departures=rel,
+                                   arrivals=arrived)
         out = [(p, why) if reasons else p for p, why in result]
         return out[0] if additions is None else out
 
@@ -1102,9 +1126,17 @@ class NHDScheduler:
             if v is not None and len(v) != len(arrivals):
                 raise ValueError(f'{len(v)} {what} for {len(arrivals)} arrival lists')
         periods = self._scan_periods(scans, period)
-        last = float(sum(periods))
         if keys is None:
             keys = self._pending_keys()
+        self._check_arrivals(arrivals, keys, float(sum(periods)))
+        deps = [self._departures({} if departures is None else d, keys) for d in (departures or [{}] * len(arrivals))]
+        result = self._grown_plans([[] for _ in arrivals] if additions is None else additions, keys, reasons, periods,
+                                   schedules=deps, arrivals=arrivals)
+        return [(p, why) if reasons else p for p, why in result]
+
+    def _check_arrivals(self, arrivals: Sequence[Sequence[Arrival]], keys: Sequence, last: float):
+        """ValueErrors of ``ForecastArrivals`` and ``ForecastPending(arrivals=...)``: an arrival key that names an
+        existing pod or repeats within its list, and ``at`` <= 0 or after the last scan (``last`` seconds)."""
         existing = {(k[0], k[1]) for k in keys} | {(k[0], k[1]) for k in self._service_pods()} | \
             {(ns, pod) for n in self.nodes.values() for (pod, ns) in n.pod_info}
         for arr in arrivals:
@@ -1118,10 +1150,6 @@ class NHDScheduler:
                 seen.add(key)
                 if not 0.0 < float(a.at) <= last:
                     raise ValueError(f'arrival {key[0]}.{key[1]} at {a.at} s is not inside the {last} s of the scans')
-        deps = [self._departures({} if departures is None else d, keys) for d in (departures or [{}] * len(arrivals))]
-        result = self._grown_plans([[] for _ in arrivals] if additions is None else additions, keys, reasons, periods,
-                                   schedules=deps, arrivals=arrivals)
-        return [(p, why) if reasons else p for p, why in result]
 
     def _arrival_entries(self, arrivals: Sequence[Arrival]) -> List[tuple]:
         """``(entry, at)`` of each arrival in ``(at, given order)``: the pod read from its config as ``_prepare`` reads a
@@ -1198,8 +1226,9 @@ class NHDScheduler:
         name)``.  ``periods`` None: one scan, through the call without rounds.  ``exclude``: nodes in maintenance
         throughout, in every scenario.  ``departures`` (``_departures``' list): releases on the batch path, for one
         scenario without additions; ``schedules``: one such list per scenario, planned on the scenario path.
-        ``arrivals`` (with ``schedules``): one ``Arrival`` list per scenario, created between the scans; a placed pod
-        then maps to ``(seconds after the first scan, node name)``."""
+        ``arrivals``: one ``Arrival`` list per scenario, created between the scans, on the scenario path with
+        ``schedules`` and on the batch path with ``departures`` (one list); a placed pod then maps to ``(seconds after
+        the first scan, node name)``."""
         scens = [[(node, before) for node, before in sc] for sc in additions]
         for sc in scens:
             names = [node.name for node, _ in sc]
@@ -1253,25 +1282,36 @@ class NHDScheduler:
                         clock = clocks[k] if at == offs[k] else max(now + at, clocks[k - 1] if k else now)
                         arrive_at[id(e)] = (k + 1, min(clock, clocks[k]), at)
                 todo = [(j, entries + [e for e, _ in arrived[j] if e.solvable]) for j in range(len(scens))]
-            if clocks is not None and scens == [[]] and schedules is None and arrivals is None:
+
+            def placed_at(e, rnd, clk):             # an arrival's own offset when its creation placed it, else a scan's
+                a = arrive_at.get(id(e))
+                return a[2] if a is not None and float(clk) == a[1] and int(rnd) == a[0] else ([0.0] + offs)[int(rnd)]
+            if clocks is not None and scens == [[]] and schedules is None:
                 # one scenario on the cluster as it is: one batch per scan (a pod beyond the tuple limits is dropped
                 # and the rest planned again, as _plan_prepared does)
                 res, ok, _ = self._without_refused(
-                    lambda es: self.cluster.forecast([e.top for e in es], [e.groups for e in es], now, clocks,
-                                                     exclude=exclude, explain=reasons, packed=[e.rec for e in es],
-                                                     releases=releases),
-                    entries)
+                    lambda es: self.cluster.forecast(
+                        [e.top for e in es], [e.groups for e in es],
+                        now if arrived is None else [arrive_at[id(e)][1] if id(e) in arrive_at else now for e in es],
+                        clocks, exclude=exclude, explain=reasons, packed=[e.rec for e in es], releases=releases,
+                        arrive=None if arrived is None else [arrive_at[id(e)][0] if id(e) in arrive_at else 0
+                                                             for e in es]),
+                    todo[0][1])
+                if arrived is not None and res is None and ok:
+                    self._supported(None, 'forecast arrivals (no plan_batch_arrivals)')
                 if releases is not None and res is None and ok:
                     self._supported(None, 'forecast releases (no plan_batch_releases)')
                 if res is not None or not ok:
                     todo = []
                 if res is not None:
                     placement, why = result[0]
-                    for e, b, r in zip(ok, res[0], res[1]):
+                    for k, (e, b, r) in enumerate(zip(ok, res[0], res[1])):
                         if int(b['status']) == wire.PLACED:
-                            placement[(e.key[0], e.key[1])] = (int(r), self.cluster.name_of(int(b['node'])))
+                            name = self.cluster.name_of(int(b['node']))
+                            placement[(e.key[0], e.key[1])] = \
+                                (int(r), name) if arrived is None else (placed_at(e, r, res[2][k]), name)
                     if reasons:
-                        why.update(self._reasons(ok, res[0], res[2]))
+                        why.update(self._reasons(ok, res[0], res[-1]))
             def scenario(item):
                 es, arrive = item[1], None
                 if arrived is not None:
@@ -1297,10 +1337,7 @@ class NHDScheduler:
                             n = int(b['node'])
                             name = self.cluster.name_of(n) if n < n_nodes else added[n - n_nodes]
                             if arrived is not None:     # on its creation, or at a scan
-                                a = arrive_at.get(id(e))
-                                at = a[2] if a is not None and float(r[-1][k]) == a[1] and int(r[-2][k]) == a[0] \
-                                    else ([0.0] + offs)[int(r[-2][k])]
-                                placement[(e.key[0], e.key[1])] = (at, name)
+                                placement[(e.key[0], e.key[1])] = (placed_at(e, r[-2][k], r[-1][k]), name)
                             else:
                                 placement[(e.key[0], e.key[1])] = name if clocks is None else (int(r[-1][k]), name)
                     if reasons:

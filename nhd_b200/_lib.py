@@ -16,8 +16,8 @@ EXPORTS = ('nhd_default_params', 'nhd_nccl_unique_id', 'nhd_shard_min_pairs', 'n
            'nhd_debug_counters', 'nhd_explain_batch', 'nhd_explain_pod', 'nhd_query_batch', 'nhd_plan_batch',
            'nhd_plan_scenarios', 'nhd_plan_scenarios_edited', 'nhd_plan_scenarios_explained',
            'nhd_plan_scenarios_grown', 'nhd_plan_scenarios_rounds', 'nhd_plan_batch_rounds', 'nhd_plan_batch_releases',
-           'nhd_plan_scenarios_releases', 'nhd_plan_scenarios_arrivals', 'nhd_alloc_pinned', 'nhd_free_pinned',
-           'nhd_ingest_create', 'nhd_ingest_destroy', 'nhd_ingest_node', 'nhd_ingest_group_mask',
+           'nhd_plan_scenarios_releases', 'nhd_plan_scenarios_arrivals', 'nhd_plan_batch_arrivals', 'nhd_alloc_pinned',
+           'nhd_free_pinned', 'nhd_ingest_create', 'nhd_ingest_destroy', 'nhd_ingest_node', 'nhd_ingest_group_mask',
            'nhd_ingest_speed_table', 'nhd_node_stats_from_records')
 
 
@@ -87,6 +87,8 @@ def load():
         'nhd_plan_scenarios_arrivals': (i32, [vp, i32, i32] + [vp] * 26),
         'nhd_plan_batch_rounds': (i32, [vp, i32, i32, vp, i32, vp, vp, i32, vp, vp, vp, vp]),
         'nhd_plan_batch_releases': (i32, [vp, i32, i32, vp, i32, vp, vp, i32, vp, i32, vp, vp, i32, vp, vp, vp, vp]),
+        'nhd_plan_batch_arrivals': (i32, [vp, i32, i32, vp, i32, vp, vp, i32, vp, i32, vp, vp, i32, vp, vp, vp, vp, vp,
+                                          vp]),
         'nhd_alloc_pinned': (i32, [ctypes.c_uint64, ctypes.POINTER(vp)]),
         'nhd_free_pinned': (i32, [vp]),
         'nhd_ingest_create': (i32, [ctypes.POINTER(vp)]),

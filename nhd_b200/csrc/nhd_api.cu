@@ -210,6 +210,10 @@ struct nhd_handle {
     DevBuf<nhd_binding> d_rout;
     DevBuf<uint32_t> d_rwhy;
     PinnedBuf<int32_t> h_rcount;
+    /* a plan's arrivals (nhd_plan_batch_arrivals): the staged pods, apart from the scans' double buffers | the clock of
+     * each pod's last attempt */
+    DevBuf<uint8_t> d_apods;
+    DevBuf<double> d_rclock;
     /* a plan's releases (nhd_plan_batch_releases): the records a segment started from, the releases, and counts |
      * node -> tracked slot | release -> slot | releases by round and node | node starts | the check word */
     DevBuf<uint8_t> d_pseg;
@@ -1267,12 +1271,19 @@ extern "C" int32_t nhd_query_batch(nhd_handle* h, int32_t source, int32_t n_pods
  * rest of the round is the next segment, at the same clock (Workspace::seg).  claim_count_kernel then adds the
  * segment's claims to the counts and clears the bits the counts leave at <= 0.  A last-round segment is explained on
  * the records it started from.
+ * With arrivals (nhd_plan_batch_arrivals) every pod is staged once, arrivals included, and the staged arrays move to
+ * d_apods, which no scan writes: round 0 and each run of a gap's arrivals (the arrivals between two release blocks, a
+ * block being the gap's releases at or before the next arrival's clock) are solved from there as segments with their
+ * commit, at their own clocks, cut as a round is.  arrival_advance_kernel then hands the gap's arrivals to its scan:
+ * the failed ones behind the pods the previous scan left (whose count round_advance_kernel left in a device word, so
+ * the host reads one word per gap).  With pod_clock every pod's clock starts as its own and round_clock_kernel writes
+ * each scan's over the pods of the scan.
  */
 static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32_t n_excluded, const int32_t* excluded,
                           int32_t n_pods, const nhd_pod* pods, const double* now, int32_t n_rounds,
                           const double* round_clock, int32_t n_tracked, const int32_t* tracked, const int16_t* pods_used,
                           int32_t n_releases, const nhd_release* releases, nhd_binding* out, uint32_t* why_counts,
-                          int32_t* pod_round)
+                          int32_t* pod_round, const int32_t* arrive_round = nullptr, double* pod_clock = nullptr)
 {
     if (!h || n_pods < 0 || n_excluded < 0 || (n_excluded > 0 && !excluded) || (n_pods > 0 && (!pods || !now || !out)))
         return NHD_ERR_INVALID;
@@ -1282,13 +1293,34 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
         if (!std::isfinite(round_clock[r])) return fail(h, NHD_ERR_INVALID, "round clock %d is not finite", r);
         if (r > 0 && round_clock[r] < round_clock[r - 1]) return fail(h, NHD_ERR_INVALID, "round clocks go down at %d", r);
     }
-    for (int i = 0; i < n_pods && n_rounds > 0; i++)         /* a monotonic clock never goes back */
-        if (round_clock[0] < now[i])
+    /* the clock rules read the pods pending at the start only: a monotonic clock never goes back */
+    const auto at_start = [&](int i) { return !arrive_round || arrive_round[i] == 0; };
+    for (int i = 0; i < n_pods && n_rounds > 0; i++)
+        if (at_start(i) && round_clock[0] < now[i])
             return fail(h, NHD_ERR_INVALID, "round clock 0 is earlier than the clock of pod %d", i);
     if (n_tracked < 0 || n_releases < 0 || (n_tracked > 0 && (!tracked || !pods_used)) || (n_releases > 0 && !releases))
         return fail(h, NHD_ERR_INVALID, "%d tracked nodes, %d releases", n_tracked, n_releases);
     double t0 = -INFINITY;
-    for (int i = 0; i < n_pods; i++) t0 = std::max(t0, now[i]);
+    for (int i = 0; i < n_pods; i++) if (at_start(i)) t0 = std::max(t0, now[i]);
+    /* arrivals (nhd_plan_batch_arrivals): rounds in [0, n_rounds] never going down in pod order, and each arrival's
+     * clock inside its gap, not before the arrival before it in that gap.  first_of[g]: the first pod arriving in gap g
+     * or later (first_of[0] = 0), so gap g's arrivals are [first_of[g], first_of[g + 1]) */
+    std::vector<int> first_of((size_t)n_rounds + 2, n_pods);
+    first_of[0] = 0;
+    double t_start = -INFINITY;                                /* the latest clock of the round-0 pods so far */
+    for (int i = 0; i < n_pods && arrive_round; i++) {
+        const int g = arrive_round[i];
+        if (g != 0 && n_rounds == 0) return fail(h, NHD_ERR_INVALID, "pod %d arrives without rounds", i);
+        if (g < 0 || g > n_rounds) return fail(h, NHD_ERR_INVALID, "pod %d: arrival round %d outside [0, %d]", i, g, n_rounds);
+        if (i > 0 && g < arrive_round[i - 1]) return fail(h, NHD_ERR_INVALID, "arrival rounds go down at pod %d", i);
+        if (g == 0) { t_start = std::max(t_start, now[i]); continue; }
+        if (i > 0 && g == arrive_round[i - 1] && now[i] < now[i - 1])
+            return fail(h, NHD_ERR_INVALID, "arrival clocks go down at pod %d", i);
+        if (now[i] < (g > 1 ? round_clock[g - 2] : t_start) || now[i] > round_clock[g - 1])
+            return fail(h, NHD_ERR_INVALID, "pod %d: arrival clock outside the gap before round %d", i, g);
+        for (int k = g; k >= 1 && first_of[k] == n_pods; k--) first_of[k] = i;
+    }
+    const bool arrivals = first_of[1] < n_pods;
     for (int k = 0; k < n_releases; k++) {
         const nhd_release& rl = releases[k];
         if (rl.round < 1 || rl.round > n_rounds)
@@ -1303,13 +1335,15 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
     if (rc != NHD_OK) return rc;
     const bool track = n_tracked > 0 || n_releases > 0;
 
-    /* the tracked nodes' slots, the releases grouped by round and node (array order kept), the counts; the checks that
-     * need the records run on the device */
+    /* the tracked nodes' slots, the releases grouped by block and node (array order kept), the counts; the checks that
+     * need the records run on the device.  A block is the releases of one gap played between the same two solves:
+     * those before arrival i of the gap (clock <= now[i], after the arrival before it), or after the gap's last arrival
+     * and before its scan (i = first_of[round + 1]); without arrivals a round's releases are one block */
+    struct RelBlock { int round, pod, g0, g1; long long pairs; };
     const int N = h->n_nodes, T = n_tracked, R = n_releases;
     std::vector<int32_t> rel_area;
-    std::vector<int> group_first(n_rounds + 2, 0);
+    std::vector<RelBlock> blocks;
     long long neg0 = 0;
-    std::vector<long long> pairs_by_round(n_rounds + 1, 0);
     size_t off_slot = 0, off_rslot = 0, off_nrel = 0, off_nstart = 0, off_bad = 0;
     if (track) {
         off_slot = (size_t)T * NHD_MAX_NICS; off_rslot = off_slot + N; off_nrel = off_rslot + R; off_nstart = off_nrel + R;
@@ -1328,27 +1362,37 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
             if (slot[n] >= 0) return fail(h, NHD_ERR_INVALID, "node %d tracked twice", n);
             slot[n] = t;
         }
-        std::vector<int32_t> order((size_t)R);
+        std::vector<int32_t> order((size_t)R), before((size_t)R);
         for (int k = 0; k < R; k++) {
             const int32_t n = releases[k].node;
             if (n < 0 || n >= N || slot[n] < 0) return fail(h, NHD_ERR_INVALID, "release %d: node %d is not tracked", k, n);
             rel_area[off_rslot + k] = slot[n];
             order[k] = k;
-            for (int i = 0; i < NHD_MAX_NICS; i++) pairs_by_round[releases[k].round] += releases[k].nic_pairings[i];
+            const int g = releases[k].round;
+            before[k] = (int32_t)(std::lower_bound(now + first_of[g], now + first_of[g + 1], releases[k].clock) - now);
         }
         std::stable_sort(order.begin(), order.end(), [&](int32_t a, int32_t b) {
-            return std::make_pair(releases[a].round, slot[releases[a].node]) < std::make_pair(releases[b].round, slot[releases[b].node]);
+            return std::make_tuple(releases[a].round, before[a], slot[releases[a].node]) <
+                   std::make_tuple(releases[b].round, before[b], slot[releases[b].node]);
         });
         for (int k = 0; k < R; k++) {
             rel_area[off_nrel + k] = order[k];
-            const nhd_release& rl = releases[order[k]];
-            if (k == 0 || rl.round != releases[order[k - 1]].round || rl.node != releases[order[k - 1]].node) {
-                group_first[rl.round + 1]++;
+            const int a = order[k], p = k ? order[k - 1] : -1;
+            const nhd_release& rl = releases[a];
+            const bool new_block = k == 0 || rl.round != releases[p].round || before[a] != before[p];
+            if (new_block) blocks.push_back({rl.round, before[a], 0, 0, 0});
+            if (new_block || rl.node != releases[p].node) {
+                blocks.back().g1++;
                 rel_area.push_back(k);
             }
+            for (int i = 0; i < NHD_MAX_NICS; i++) blocks.back().pairs += rl.nic_pairings[i];
         }
         rel_area.push_back(R);
-        for (int r = 1; r <= n_rounds + 1; r++) group_first[r] += group_first[r - 1];
+        for (size_t b = 0, g = 0; b < blocks.size(); b++) {
+            blocks[b].g0 = (int)g;
+            g += blocks[b].g1;
+            blocks[b].g1 = (int)g;
+        }
         off_bad = rel_area.size();
         rel_area.push_back(0x7FFFFFFF);
         CK(cudaSetDevice(h->params.device));
@@ -1411,22 +1455,35 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
     }
     if (n_rounds == 0 && !track) {
         if (pod_round) memset(pod_round, 0, (size_t)n_pods * 4);
+        if (pod_clock) memcpy(pod_clock, now, (size_t)n_pods * 8);
         if ((rc = launch_solve(h, w, nodes, false, false, false)) != NHD_OK) return rc;
         if (why_counts && (rc = explain_counts(h, w, nodes, why_counts, what)) != NHD_OK) return rc;
         return fetch_bindings(h, w, n_pods, out);
     }
 
     const size_t P = (size_t)n_pods, grid0 = (P + ROUND_THREADS - 1) / ROUND_THREADS, why_bytes = P * NHD_WHY_COUNT * 4;
-    const size_t off_now = w.now_offset(), off_gm = off_now + P * 8;
-    CK(h->d_rpods.grow(off_gm + (w.n_names ? P * 8 : 0)));
-    CK(h->d_ridx.grow((3 * P + grid0) * 4));
+    const size_t off_now = w.now_offset(), off_gm = off_now + P * 8, pods_bytes = off_gm + (w.n_names ? P * 8 : 0);
+    CK(h->d_rpods.grow(pods_bytes));
+    CK(h->d_ridx.grow((3 * P + grid0 + 1) * 4));
     CK(h->d_rout.grow(P * sizeof(nhd_binding)));
     CK(h->h_rcount.grow(8));
     if (why_counts) {
         CK(h->d_rwhy.grow(why_bytes));
         CK(cudaMemsetAsync(h->d_rwhy, 0, why_bytes, h->stream));
     }
+    if (pod_clock) {            /* every pod's first attempt is at its own clock; each scan writes its clock over it */
+        CK(h->d_rclock.grow(P * 8));
+        CK(cudaMemcpyAsync(h->d_rclock, w.pod_arrays + off_now, P * 8, cudaMemcpyDeviceToDevice, h->stream));
+    }
+    if (arrivals) {
+        /* round 0 and the arrival runs solve from the staged pods, kept in d_apods, where no scan's pod list is
+         * written; the scans alternate between w.pod_arrays and d_rpods */
+        CK(h->d_apods.grow(pods_bytes));
+        w.pod_arrays.swap(h->d_apods);
+    }
+    const auto from_staged = [&]() { if (arrivals) w.pod_arrays.swap(h->d_apods); };   /* (called in pairs) */
     int32_t* const rows[2] = {h->d_ridx, h->d_ridx + P};
+    int32_t* const d_base = h->d_ridx + 3 * P + grid0;    /* with arrivals: pods the last scan left, for the next gap */
     if (track) {
         /* round 0's caller rows are the pods' own (its reason rows are scattered per segment) */
         std::vector<int32_t> iota(P);
@@ -1438,107 +1495,186 @@ static int32_t plan_batch(nhd_handle* h, const char* what, int32_t source, int32
     const int32_t* const d_slot = h->d_rel + off_slot;
     uint8_t* const pnodes = h->d_pnodes;
     long long cut_room = neg0;                /* negative count the plan's copy may hold: an upper bound on cuts */
-    RoundArgs ra;
-    ra.result = h->d_rout; ra.pod_round = h->d_ridx + 2 * P; ra.block_cnt = h->d_ridx + 3 * P;
-    ra.n_rounds = n_rounds; ra.survivors = h->h_rcount;
-    int n = n_pods, cur = 0;
-    for (int r = 0; r <= n_rounds && n > 0; r++) {
-        const bool last = r == n_rounds;
-        w.n_pods = n;
-        if (r > 0) { w.now0 = round_clock[r - 1]; w.const_clock = true; }
-        int32_t* const row = r || track ? rows[cur] : nullptr;
+    size_t next_block = 0;
+
+    /* the releases of gap r played right before arrival i (i = first_of[r + 1]: before the scan) */
+    const auto play = [&](int r, int i) -> int32_t {
+        for (; next_block < blocks.size() && blocks[next_block].round == r && blocks[next_block].pod == i; next_block++) {
+            const RelBlock& b = blocks[next_block];
+            ReleaseArgs rla;
+            rla.nodes = pnodes; rla.rel = h->d_rels; rla.rel_slot = h->d_rel + off_rslot;
+            rla.node_start = h->d_rel + off_nstart + b.g0; rla.node_rel = h->d_rel + off_nrel;
+            rla.n = b.g1 - b.g0; rla.count = d_count;
+            release_kernel<<<(rla.n + 127) / 128, 128, 0, h->stream>>>(rla);
+            CK(cudaGetLastError());
+            cut_room += b.pairs;
+        }
+        return NHD_OK;
+    };
+    /* pods [first, first + m) of w solved in order, committed unless this is the last scan, explained when asked (row:
+     * the scan's caller rows).  With tracked counts: in segments while a cut is possible, each starting at its first
+     * pod's own clock when per_pod (round 0 and the arrival runs), else at w.now0 */
+    const auto solve = [&](int first, int m, bool commit, bool explain, int32_t* row, bool per_pod) -> int32_t {
         if (!track) {
-            if ((rc = launch_solve(h, w, nodes, false, !last, false)) != NHD_OK) return rc;
-        } else {
-            const int groups = group_first[r + 1] - group_first[r];
-            if (groups > 0) {
-                ReleaseArgs rla;
-                rla.nodes = pnodes; rla.rel = h->d_rels; rla.rel_slot = h->d_rel + off_rslot;
-                rla.node_start = h->d_rel + off_nstart + group_first[r]; rla.node_rel = h->d_rel + off_nrel;
-                rla.n = groups; rla.count = d_count;
-                release_kernel<<<(groups + 127) / 128, 128, 0, h->stream>>>(rla);
-                CK(cudaGetLastError());
-            }
-            cut_room += pairs_by_round[r];
-            for (int seg = 0; seg < n;) {
-                w.seg = seg;
-                w.n_pods = n - seg;
-                if (r == 0) w.now0 = now[seg];
-                const bool may_cut = cut_room > 0;
-                const bool explain = last && why_counts;
-                if (!may_cut) {
-                    /* no claim can meet a negative count: the rest of the round is one segment, as without releases */
-                    const int m = w.n_pods;
-                    nhd_binding* const b = w.bindings();
-                    if ((rc = launch_solve(h, w, nodes, false, !last, false)) != NHD_OK) return rc;
-                    if (!last) {
-                        claim_count_kernel<<<(m + 127) / 128, 128, 0, h->stream>>>(b, m, d_slot, d_count, pnodes);
-                        CK(cudaGetLastError());
-                    }
-                    if (explain) {
-                        if ((rc = explain_rows(h, w, nodes)) != NHD_OK) return rc;
-                        round_why_kernel<<<(m * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, row + seg, m,
-                                                                                                 h->d_rwhy);
-                        CK(cudaGetLastError());
-                    }
-                    break;
-                }
+            w.seg = first;
+            w.n_pods = m;
+            const int32_t e = launch_solve(h, w, nodes, false, commit, false);
+            w.seg = 0;
+            return e;
+        }
+        int32_t e;
+        for (int seg = first; seg < first + m;) {
+            w.seg = seg;
+            w.n_pods = first + m - seg;
+            if (per_pod) w.now0 = now[seg];
+            if (cut_room <= 0) {
+                /* no claim can meet a negative count: the rest of the run is one segment, as without releases */
+                const int k = w.n_pods;
                 nhd_binding* const b = w.bindings();
-                int32_t* const cut_word = h->h_rcount + 1;
-                uint8_t* const seg_nodes = h->d_pseg;
-                CK(cudaMemcpyAsync(seg_nodes, pnodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
-                if ((rc = launch_solve(h, w, nodes, false, true, false)) != NHD_OK) return rc;
-                int m = w.n_pods;
-                claim_cut_kernel<<<1, CUT_THREADS, 0, h->stream>>>(b, m, d_slot, d_count, cut_word);
-                CK(cudaGetLastError());
-                CK(cudaStreamSynchronize(h->stream));
-                const int cut = *cut_word;
-                if (cut >= 0) {
-                    CK(cudaMemcpyAsync(pnodes, seg_nodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
-                    w.n_pods = m = cut + 1;
-                    if ((rc = launch_solve(h, w, nodes, false, true, false)) != NHD_OK) return rc;
-                    cut_room--;
+                if ((e = launch_solve(h, w, nodes, false, commit, false)) != NHD_OK) return e;
+                if (commit) {
+                    claim_count_kernel<<<(k + 127) / 128, 128, 0, h->stream>>>(b, k, d_slot, d_count, pnodes);
+                    CK(cudaGetLastError());
                 }
-                claim_count_kernel<<<(m + 127) / 128, 128, 0, h->stream>>>(b, m, d_slot, d_count, pnodes);
-                CK(cudaGetLastError());
                 if (explain) {
-                    if ((rc = explain_rows(h, w, seg_nodes)) != NHD_OK) return rc;
-                    round_why_kernel<<<(m * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, row + seg, m,
+                    if ((e = explain_rows(h, w, nodes)) != NHD_OK) return e;
+                    round_why_kernel<<<(k * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, row + seg, k,
                                                                                              h->d_rwhy);
                     CK(cudaGetLastError());
-                    if ((rc = explain_survivors(h, what)) != NHD_OK) return rc;
                 }
-                seg += m;
+                break;
             }
+            nhd_binding* const b = w.bindings();
+            int32_t* const cut_word = h->h_rcount + 1;
+            uint8_t* const seg_nodes = h->d_pseg;
+            CK(cudaMemcpyAsync(seg_nodes, pnodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
+            if ((e = launch_solve(h, w, nodes, false, true, false)) != NHD_OK) return e;
+            int k = w.n_pods;
+            claim_cut_kernel<<<1, CUT_THREADS, 0, h->stream>>>(b, k, d_slot, d_count, cut_word);
+            CK(cudaGetLastError());
+            CK(cudaStreamSynchronize(h->stream));
+            const int cut = *cut_word;
+            if (cut >= 0) {
+                CK(cudaMemcpyAsync(pnodes, seg_nodes, h->nodes_bytes, cudaMemcpyDeviceToDevice, h->stream));
+                w.n_pods = k = cut + 1;
+                if ((e = launch_solve(h, w, nodes, false, true, false)) != NHD_OK) return e;
+                cut_room--;
+            }
+            claim_count_kernel<<<(k + 127) / 128, 128, 0, h->stream>>>(b, k, d_slot, d_count, pnodes);
+            CK(cudaGetLastError());
+            if (explain) {
+                if ((e = explain_rows(h, w, seg_nodes)) != NHD_OK) return e;
+                round_why_kernel<<<(k * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, row + seg, k,
+                                                                                         h->d_rwhy);
+                CK(cudaGetLastError());
+                if ((e = explain_survivors(h, what)) != NHD_OK) return e;
+            }
+            seg += k;
+        }
+        w.seg = 0;
+        return NHD_OK;
+    };
+
+    RoundArgs ra;
+    ra.result = h->d_rout; ra.pod_round = h->d_ridx + 2 * P; ra.block_cnt = h->d_ridx + 3 * P;
+    ra.n_rounds = n_rounds;
+    /* n: the pods of the next scan, -1 while only the device knows it (the gap's hand-over reads it there) */
+    int n = first_of[1], cur = 0;
+    for (int r = 0; r <= n_rounds && (n != 0 || first_of[r] < n_pods); r++) {
+        const bool last = r == n_rounds;
+        if (r > 0) {
+            /* gap r: its releases and the runs of its arrivals between them, merged by clock, then the hand-over of
+             * the arrivals to scan r, behind the pods scan r - 1 left */
+            for (int i = first_of[r], end = first_of[r + 1];; ) {
+                if ((rc = play(r, i)) != NHD_OK) return rc;
+                if (i == end) break;
+                const int j = next_block < blocks.size() && blocks[next_block].round == r ? blocks[next_block].pod : end;
+                w.now0 = now[i];
+                w.const_clock = now[i] == now[j - 1];
+                from_staged();
+                rc = solve(i, j - i, true, false, nullptr, true);
+                from_staged();
+                if (rc != NHD_OK) return rc;
+                i = j;
+            }
+            if (first_of[r] < n_pods) {             /* scan r - 1 deferred its count to this hand-over */
+                const int a0 = first_of[r], m = first_of[r + 1] - a0, grid = std::max(1, (m + ROUND_THREADS - 1) / ROUND_THREADS);
+                RoundArgs rc_args = ra;
+                rc_args.out = w.out + a0; rc_args.n_pods = m;
+                round_count_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(rc_args);
+                ArrivalArgs aa;
+                from_staged();
+                aa.out = w.out + a0; aa.pod_type = w.pod_type() + a0; aa.now = w.now() + a0;
+                aa.pod_groups = w.n_names ? w.pod_groups() + a0 : nullptr;
+                from_staged();
+                aa.first = a0; aa.n_pods = m; aa.round = r; aa.n_rounds = n_rounds;
+                aa.result = h->d_rout; aa.pod_round = ra.pod_round; aa.pod_clock = pod_clock ? h->d_rclock.p : nullptr;
+                aa.block_cnt = ra.block_cnt; aa.base = d_base;
+                aa.next_pod_type = reinterpret_cast<int32_t*>(w.pod_arrays.p);
+                aa.next_now = reinterpret_cast<double*>(w.pod_arrays.p + off_now);
+                aa.next_pod_groups = w.n_names ? reinterpret_cast<uint64_t*>(w.pod_arrays.p + off_gm) : nullptr;
+                aa.next_row = rows[cur]; aa.next_clock = round_clock[r - 1]; aa.count = h->h_rcount;
+                arrival_advance_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(aa);
+                CK(cudaGetLastError());
+                CK(cudaStreamSynchronize(h->stream));
+                n = *h->h_rcount;
+            }
+        }
+        /* scan r (round 0: the pods pending at the start, at their own clocks) */
+        const bool defer = !last && first_of[r + 1] < n_pods;      /* the next gap's hand-over reads the count */
+        if (n > 0) {
             w.seg = 0;
             w.n_pods = n;
-        }
-        ra.out = w.out; ra.pod_type = w.pod_type(); ra.pod_groups = w.pod_groups(); ra.row = row;
-        ra.n_pods = n; ra.round = r;
-        ra.next_pod_type = last ? nullptr : reinterpret_cast<int32_t*>(h->d_rpods.p);
-        ra.next_now = last ? nullptr : reinterpret_cast<double*>(h->d_rpods.p + off_now);
-        ra.next_pod_groups = last || !w.n_names ? nullptr : reinterpret_cast<uint64_t*>(h->d_rpods.p + off_gm);
-        ra.next_row = last ? nullptr : rows[cur ^ 1];
-        ra.next_clock = last ? 0.0 : round_clock[r];
-        const int grid = (n + ROUND_THREADS - 1) / ROUND_THREADS;
-        if (!last) round_count_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(ra);
-        round_advance_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(ra);
-        CK(cudaGetLastError());
-        if (last) {
-            if (why_counts && !track) {
-                if ((rc = explain_rows(h, w, nodes)) != NHD_OK) return rc;
-                round_why_kernel<<<(n * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, ra.row, n, h->d_rwhy);
+            if (r > 0) { w.now0 = round_clock[r - 1]; w.const_clock = true; }
+            else {
+                w.now0 = now[0];
+                w.const_clock = true;
+                for (int i = 1; i < n; i++) if (now[i] != now[0]) { w.const_clock = false; break; }
+            }
+            int32_t* const row = r || track ? rows[cur] : nullptr;
+            if (r == 0) from_staged();
+            if ((rc = solve(0, n, !last, last && why_counts, row, r == 0)) != NHD_OK) { if (r == 0) from_staged(); return rc; }
+            ra.out = w.out; ra.pod_type = w.pod_type(); ra.pod_groups = w.pod_groups(); ra.row = row;
+            ra.n_pods = n; ra.round = r;
+            ra.next_pod_type = last ? nullptr : reinterpret_cast<int32_t*>(h->d_rpods.p);
+            ra.next_now = last ? nullptr : reinterpret_cast<double*>(h->d_rpods.p + off_now);
+            ra.next_pod_groups = last || !w.n_names ? nullptr : reinterpret_cast<uint64_t*>(h->d_rpods.p + off_gm);
+            ra.next_row = last ? nullptr : rows[cur ^ 1];
+            ra.next_clock = last ? 0.0 : round_clock[r];
+            ra.survivors = defer ? d_base : h->h_rcount.p;
+            const int grid = (n + ROUND_THREADS - 1) / ROUND_THREADS;
+            if (!last) round_count_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(ra);
+            round_advance_kernel<<<grid, ROUND_THREADS, 0, h->stream>>>(ra);
+            CK(cudaGetLastError());
+            if (pod_clock && r > 0) {
+                round_clock_kernel<<<(n + 255) / 256, 256, 0, h->stream>>>(row, n, round_clock[r - 1], h->d_rclock);
                 CK(cudaGetLastError());
             }
-            break;
+            if (r == 0) from_staged();
+            if (last) {
+                if (why_counts && !track) {
+                    if ((rc = explain_rows(h, w, nodes)) != NHD_OK) return rc;
+                    round_why_kernel<<<(n * NHD_WHY_COUNT + 255) / 256, 256, 0, h->stream>>>(h->d_xcounts, ra.row, n, h->d_rwhy);
+                    CK(cudaGetLastError());
+                }
+                break;
+            }
+        } else if (defer) {
+            CK(cudaMemsetAsync(d_base, 0, 4, h->stream));
         }
-        CK(cudaStreamSynchronize(h->stream));
-        n = *h->h_rcount;
+        if (last) break;
+        if (defer) {
+            n = -1;
+        } else if (n > 0) {
+            CK(cudaStreamSynchronize(h->stream));
+            n = *h->h_rcount;
+        }
         w.pod_arrays.swap(h->d_rpods);
         cur ^= 1;
     }
     if (why_counts) CK(cudaMemcpyAsync(why_counts, h->d_rwhy, why_bytes, cudaMemcpyDeviceToHost, h->stream));
     if (pod_round) CK(cudaMemcpyAsync(pod_round, ra.pod_round, P * 4, cudaMemcpyDeviceToHost, h->stream));
+    if (pod_clock) CK(cudaMemcpyAsync(pod_clock, h->d_rclock, P * 8, cudaMemcpyDeviceToHost, h->stream));
     if ((rc = fetch_bindings(h, w, n_pods, out, h->d_rout)) != NHD_OK) return rc;
     return why_counts && n > 0 ? explain_survivors(h, what) : NHD_OK;
 }
@@ -1568,6 +1704,18 @@ extern "C" int32_t nhd_plan_batch_releases(nhd_handle* h, int32_t source, int32_
 {
     return plan_batch(h, "nhd_plan_batch_releases", source, n_excluded, excluded, n_pods, pods, now, n_rounds,
                       round_clock, n_tracked, tracked, pods_used, n_releases, releases, out, why_counts, pod_round);
+}
+
+extern "C" int32_t nhd_plan_batch_arrivals(nhd_handle* h, int32_t source, int32_t n_excluded, const int32_t* excluded,
+                                           int32_t n_pods, const nhd_pod* pods, const double* now, int32_t n_rounds,
+                                           const double* round_clock, int32_t n_tracked, const int32_t* tracked,
+                                           const int16_t* pods_used, int32_t n_releases, const nhd_release* releases,
+                                           const int32_t* arrive_round, nhd_binding* out, uint32_t* why_counts,
+                                           int32_t* pod_round, double* pod_clock)
+{
+    return plan_batch(h, "nhd_plan_batch_arrivals", source, n_excluded, excluded, n_pods, pods, now, n_rounds,
+                      round_clock, n_tracked, tracked, pods_used, n_releases, releases, out, why_counts, pod_round,
+                      arrive_round, pod_clock);
 }
 
 /*

@@ -25,7 +25,9 @@
  * of a query would go on its own, nhd_query_batch), exclude_nodes_kernel (a plan's excluded nodes, nhd_plan_batch),
  * round_count / round_advance_kernel (the unplaced pods of a plan's round handed to its next round,
  * nhd_plan_batch_rounds), release_kernel / release_check_kernel / claim_cut_kernel / claim_count_kernel (deployed pods
- * ending between a plan's rounds and the signed NIC counters, nhd_plan_batch_releases) and scenario_plan_kernel (many independent small plans side by side, nhd_plan_scenarios).
+ * ending between a plan's rounds and the signed NIC counters, nhd_plan_batch_releases), arrival_advance_kernel /
+ * round_clock_kernel (a gap's arrivals handed to its scan and each pod's clock, nhd_plan_batch_arrivals) and
+ * scenario_plan_kernel (many independent small plans side by side, nhd_plan_scenarios).
  *
  * Device layout of the node array ("tiled AoSoA"): tiles of 32 nodes, 4 KB each:
  *     byte offset(node n, 16-byte chunk c) = (n / 32) * 4096 + c * 512 + (n % 32) * 16
@@ -2838,6 +2840,84 @@ __global__ void __launch_bounds__(ROUND_THREADS) round_advance_kernel(const Roun
         if (p0 + p < a.n_pods)
             reinterpret_cast<uint4*>(a.result)[(size_t)r * 8 + c] = reinterpret_cast<const uint4*>(a.out)[(size_t)(p0 + p) * 8 + c];
     }
+}
+
+/*
+ * Between a gap of a plan with arrivals (nhd_plan_batch_arrivals) and the scan after it.  The gap's arrivals were solved
+ * at their own clocks into out[], in pod order, straight from the staged pods (staged in caller order, so the arrival
+ * at i of the gap is caller row first + i).  Every binding goes to its caller row, every arrival's round and clock are
+ * written (final for a placed one; a failed one is retried by the scan, which rewrites them), and the failed arrivals
+ * are appended, in order, behind the *base pods the previous scan left in the scan's pod arrays (a device word that
+ * round_advance_kernel wrote), at the scan's clock.  *count (page-locked host word) = the scan's pod count.  The grid
+ * and the per-CTA counts are round_count_kernel's over the same out and n_pods (one CTA even for no arrivals, so that
+ * *count is written); no CTA waits for another.
+ */
+struct ArrivalArgs {
+    const nhd_binding* out;        /* the gap's arrivals' bindings, in pod order */
+    const int32_t* pod_type;       /* ... their pod types, node-group lists (null unless the pods mix them) and clocks, as
+                                      staged */
+    const uint64_t* pod_groups;
+    const double* now;
+    int first, n_pods, round, n_rounds;
+    nhd_binding* result;           /* [caller row] each pod's last attempt */
+    int32_t* pod_round;            /* [caller row] the round that placed the pod, or n_rounds */
+    double* pod_clock;             /* [caller row] the clock of the pod's last attempt, or null */
+    const int32_t* block_cnt;      /* [grid] failed arrivals per CTA (round_count_kernel) */
+    const int32_t* base;           /* pods already in the scan's arrays */
+    int32_t* next_pod_type;        /* the scan's pod set */
+    double* next_now;
+    uint64_t* next_pod_groups;
+    int32_t* next_row;
+    double next_clock;
+    int32_t* count;                /* pods of the scan: one word the host reads (page-locked host memory) */
+};
+
+__global__ void __launch_bounds__(ROUND_THREADS) arrival_advance_kernel(const ArrivalArgs a)
+{
+    __shared__ int32_t s_before[ROUND_THREADS / 32], s_mine[ROUND_THREADS / 32];
+    const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5;
+    const int i = blockIdx.x * ROUND_THREADS + tid;
+    const bool live = i < a.n_pods;
+    const int row = a.first + i;
+    const bool pending = live && a.out[i].status != NHD_PLACED;
+    if (live) {
+        a.pod_round[row] = pending ? a.n_rounds : a.round;
+        if (a.pod_clock) a.pod_clock[row] = a.now[i];
+    }
+    int32_t part = 0;                                                /* failed arrivals of the CTAs before this one */
+    for (int b = tid; b < (int)blockIdx.x; b += ROUND_THREADS) part += a.block_cnt[b];
+    for (int off = 16; off; off >>= 1) part += __shfl_sync(0xFFFFFFFFu, part, lane ^ off);
+    const unsigned m = __ballot_sync(0xFFFFFFFFu, pending);
+    if (lane == 0) { s_before[wid] = part; s_mine[wid] = __popc(m); }
+    __syncthreads();
+    int32_t pos = *a.base, total = pos;
+    for (int k = 0; k < ROUND_THREADS / 32; k++) {
+        pos += s_before[k] + (k < wid ? s_mine[k] : 0);
+        total += s_before[k] + s_mine[k];
+    }
+    if (pending) {
+        pos += __popc(m & ((1u << lane) - 1u));
+        a.next_pod_type[pos] = a.pod_type[i];
+        a.next_now[pos] = a.next_clock;
+        if (a.next_pod_groups) a.next_pod_groups[pos] = a.pod_groups[i];
+        a.next_row[pos] = row;
+    }
+    if (blockIdx.x == gridDim.x - 1 && tid == 0) *a.count = total;
+    /* each binding to its caller row, as round_advance_kernel copies them */
+    const int p0 = blockIdx.x * ROUND_THREADS + wid * 32;
+    for (int k = 0; k < 8; k++) {
+        const int p = k * 4 + (lane >> 3), c = lane & 7;
+        if (p0 + p < a.n_pods)
+            reinterpret_cast<uint4*>(a.result)[(size_t)(a.first + p0 + p) * 8 + c] =
+                reinterpret_cast<const uint4*>(a.out)[(size_t)(p0 + p) * 8 + c];
+    }
+}
+
+/* a scan's clock as the clock of the last attempt of each of its pods (row: the scan's pod -> caller row) */
+__global__ void round_clock_kernel(const int32_t* __restrict__ row, int n_pods, double clock, double* __restrict__ pod_clock)
+{
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n_pods) pod_clock[row[i]] = clock;
 }
 
 /* the last round's reason rows (explain_kernel's counts, one row per pod of that round) to the callers' rows */

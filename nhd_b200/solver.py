@@ -263,11 +263,28 @@ class Solver:
                                                   tracked=tracked, pods_used=pods_used, releases=releases)
         return (out, pod_round, counts) if explain else (out, pod_round)
 
+    def plan_batch_arrivals(self, pods, now, round_clocks, tracked, pods_used, releases, arrive_round,
+                            source='mirror', exclude=(), explain=False):
+        """``plan_batch_releases`` with pods created between the scans, on the batch path: ``arrive_round[i]`` 0 for a
+        pod pending at the start, else the round ``r`` (1 .. ``len(round_clocks)``) in whose gap the pod is created, at
+        ``now[i]``; the round-0 pods come first and ``(arrive_round, now)`` never goes down.  Each gap plays its
+        releases and its arrivals' first attempts merged by clock (a release first at an equal clock), and its scan
+        retries every arrived pod not placed yet, the gap's failed arrivals after the older pods.  The exclusions hold
+        throughout.  Returns ``(bindings, pod_round, pod_clock)``, ``pod_clock`` the clock of the attempt whose binding
+        is given; ``explain=True``: ``(bindings, pod_round, pod_clock, counts)``.  The same answer as ``plan_scenarios``
+        with this one timeline as a scenario with ``arrive``, from the batch path: meant for one large timeline.
+        Nothing is placed."""
+        out, pod_round, counts, pod_clock = self._plan_batch(
+            pods, now, source, exclude, explain, round_clocks=round_clocks, tracked=tracked, pods_used=pods_used,
+            releases=releases, arrive_round=arrive_round)
+        return (out, pod_round, pod_clock, counts) if explain else (out, pod_round, pod_clock)
+
     def _plan_batch(self, pods, now, source, exclude, explain, out=None, round_clocks=None, tracked=(), pods_used=(),
-                    releases=None):
+                    releases=None, arrive_round=None):
         """The three ``plan_batch*`` methods as one ``nhd_plan_batch_releases`` call (no rounds, no tracked nodes and no
         releases are what the two narrower entry points pass): ``(bindings, pod_round, counts or None)``, ``pod_round``
-        None without ``round_clocks``."""
+        None without ``round_clocks``.  With ``arrive_round`` the call is ``nhd_plan_batch_arrivals`` and the result
+        gains the pod clocks."""
         src = _source(source)
         pods = np.ascontiguousarray(pods, dtype=wire.POD_DTYPE)
         now = np.ascontiguousarray(now, dtype='<f8')
@@ -282,15 +299,20 @@ class Solver:
             out = np.zeros(len(pods), dtype=wire.BINDING_DTYPE)
         pod_round = None if round_clocks is None else np.zeros(len(pods), dtype='<i4')
         counts = np.zeros((len(pods), wire.WHY_COUNT), dtype='<u4') if explain else None
-        self._ck(self._L.nhd_plan_batch_releases(self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods),
-                                                 pods.ctypes.data, now.ctypes.data, len(clocks),
-                                                 clocks.ctypes.data if len(clocks) else None, len(tr),
-                                                 tr.ctypes.data if len(tr) else None,
-                                                 used.ctypes.data if len(tr) else None, len(rel),
-                                                 rel.ctypes.data if len(rel) else None, out.ctypes.data,
-                                                 counts.ctypes.data if explain else None,
-                                                 None if pod_round is None else pod_round.ctypes.data))
-        return out, pod_round, counts
+        args = [self._h, src, len(ex), ex.ctypes.data if len(ex) else None, len(pods), pods.ctypes.data,
+                now.ctypes.data, len(clocks), clocks.ctypes.data if len(clocks) else None, len(tr),
+                tr.ctypes.data if len(tr) else None, used.ctypes.data if len(tr) else None, len(rel),
+                rel.ctypes.data if len(rel) else None]
+        tail = [out.ctypes.data, counts.ctypes.data if explain else None,
+                None if pod_round is None else pod_round.ctypes.data]
+        if arrive_round is None:            # every existing call goes out as before
+            self._ck(self._L.nhd_plan_batch_releases(*args, *tail))
+            return out, pod_round, counts
+        arrive = np.ascontiguousarray(arrive_round, dtype='<i4').reshape(-1)
+        assert len(arrive) == len(pods)
+        pod_clock = np.zeros(len(pods), dtype='<f8')
+        self._ck(self._L.nhd_plan_batch_arrivals(*args, arrive.ctypes.data, *tail, pod_clock.ctypes.data))
+        return out, pod_round, counts, pod_clock
 
     def plan_scenarios(self, scenarios, source='mirror', explain=False):
         """Many independent dry runs in one call.  ``scenarios``: a sequence of ``Scenario`` records, or plain tuples of
